@@ -2,7 +2,7 @@
 """Benchmark of the hot path BASELINE.json names: ItemKNN cosine top-K rows/sec (and BPR samples/sec as a
 secondary figure) on a synthetic CSR URM.
 
-    python bench.py --gpus N --steps K --warmup W [--impl b200|reference] [--workload C5]
+    python bench.py --gpus N --steps K --warmup W [--impl b200|reference] [--workload C5] [--dump-outputs DIR]
 
 One JSON line on stdout (rank 0).  A "step" is one full pass of the similarity hot path over the workload
 (all n_items columns: accumulate + normalise + top-K, plus the all-gather when N > 1) with the URM already
@@ -12,6 +12,9 @@ device-side constructor work, kernel, CSR assembly and D2H all inside the timed 
 
 `--impl reference` times the reference's own Cython (oracle/_ref, compiled unmodified) on the host cores,
 column-sharded over worker processes with the reference's own start_col/end_col hook.
+
+`--dump-outputs DIR` writes the top-K table of the last timed step as .npy files (see dump_outputs) so that two builds can
+be compared output for output: the synthetic URM is seeded, so the inputs are the same from run to run.
 """
 import argparse
 import json
@@ -47,7 +50,7 @@ def emit_json(obj):
 
 # ----------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi sampled every 200 ms while the timed region runs (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled every 200 ms while the timed region runs: SM clock, power and throttle reasons."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -98,7 +101,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
 
 
 def ncu_traffic_per_launch(workload):
@@ -256,6 +259,32 @@ def parity_gate(X, table, W_ref, lo, hi, K, kind):
 
 
 # ----------------------------------------------------------------------------------------------------------
+def dump_outputs(directory, table, n_items, max_rows=16384, seed=0):
+    """The top-K table [n_items, K] of the timed path, for a fixed seeded sample of at most max_rows of its rows (the whole
+    table at C5 is 320 MB): rows.npy (the sampled row ids), cnt.npy (entries per row), idx.npy / val.npy ([rows, K]; the
+    slots past cnt are -1 / 0).  Each row is ordered by neighbour index, so that ties at equal similarity compare equal
+    whatever order a kernel emits them in.  Indices in float64 (exact), similarities in float32, about 40 MB at K = 200."""
+    import torch
+    idx_t, val_t, cnt_t = table
+    rng = np.random.default_rng(seed)
+    rows = np.sort(rng.choice(n_items, size=min(n_items, max_rows), replace=False))
+    sel = torch.from_numpy(rows).to(idx_t.device)
+    idx = idx_t.index_select(0, sel).cpu().numpy().astype(np.int64)
+    val = val_t.index_select(0, sel).cpu().numpy().astype(np.float32)
+    cnt = cnt_t.index_select(0, sel).cpu().numpy().astype(np.int64)
+    empty = np.arange(idx.shape[1])[None, :] >= cnt[:, None]
+    idx[empty] = np.iinfo(np.int64).max
+    val[empty] = 0.0
+    order = np.argsort(idx, axis=1, kind="stable")
+    idx = np.take_along_axis(idx, order, axis=1)
+    val = np.take_along_axis(val, order, axis=1)
+    idx[np.take_along_axis(empty, order, axis=1)] = -1
+    os.makedirs(directory, exist_ok=True)
+    for name, a in (("rows", rows.astype(np.float64)), ("cnt", cnt.astype(np.float64)), ("idx", idx.astype(np.float64)), ("val", val)):
+        np.save(os.path.join(directory, name + ".npy"), a)
+    log("[dump] %d sampled rows of the top-K table -> %s" % (len(rows), directory))
+
+
 def pinned_csr(X):
     """scipy CSR whose three arrays live in pinned host memory (so the e2e H2D runs at PCIe speed)."""
     import torch
@@ -339,6 +368,8 @@ def run_b200(args, rank, world, local_rank):
     barrier()
     launches = _lib.launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, n_items)
     elapsed_ms = ev0.elapsed_time(ev1)
     if world > 1:
         t = torch.tensor([elapsed_ms], device="cuda")
@@ -465,7 +496,7 @@ def run_b200(args, rank, world, local_rank):
             args.workload, nu, ni, dens, args.values),
             "windows": sim.n_windows, "binary_path": sim.binary_path,
             "parallelism": ("item-sharded x%d; " % world + gather) if world > 1 else "1 GPU",
-            "timing": "inputs (CSR+CSC %.2f GB) larger than the 126 MB L2; no explicit flush" % (2 * bpe * X.nnz / 1e9)},
+            "timing": "inputs (CSR+CSC %.2f GB) larger than the 50 MB L2; no explicit flush" % (2 * bpe * X.nnz / 1e9)},
         "clocks": clocks,
         "e2e": {"value": n_items / e2e_s, "unit": "rows/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                 "seconds_per_fit": e2e_s, "steps": e2e_steps, "pinned_inputs": e2e_pinned,
@@ -637,7 +668,7 @@ def tensor_leg(args):
     from recsys2019_deeplearning_evaluation_b200 import recommenders as R
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     peak_tf, peak_src = (float(json.load(open(pk))["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)") \
-        if os.path.exists(pk) else (1500.0, "fallback (B200_PROFILING.md)")
+        if os.path.exists(pk) else (989.0, "H100 SXM data sheet, dense bf16 (not measured)")
     t0 = time.time()
     X = synth_config("C4", values="binary")
     nu, ni = X.shape
@@ -678,7 +709,7 @@ def tensor_leg(args):
         flops = float(2.0 * (lens ** 2).sum() + float(ni) ** 3)
         sec = min(secs)
         res["ease"] = {"metric": "EASE_R fit seconds", "value": sec, "unit": "s", "higher_is_better": False, "seconds_all": secs,
-                       "what": "EASE_R_Recommender(host URM).fit(): H2D, Gram (similarity kernel, dense mode), blocked Cholesky inverse on tcgen05 (3xTF32), B on the device",
+                       "what": "EASE_R_Recommender(host URM).fit(): H2D, Gram (similarity kernel, dense mode), blocked Cholesky inverse on wgmma (3xTF32), B on the device",
                        "roofline": {"bound": "tensor", "achieved": flops / sec / 1e12, "peak": peak_tf, "unit": "TFLOP/s",
                                     "frac": flops / sec / 1e12 / peak_tf, "flops_per_fit": flops}}
         del ease
@@ -704,6 +735,8 @@ def main():
     ap.add_argument("--ref-workers", type=int, default=64, help="worker processes of the reference arm (capped by the host core count)")
     ap.add_argument("--ref-slice", type=int, default=250)
     ap.add_argument("--gather", default="peer", choices=["peer", "nccl"], help="N > 1: how the ranks' rows reach every rank")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's top-K table to DIR/*.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,6 +1,6 @@
 """The reference's run_example_usage.py (run_example_usage.py:1-83) on this package: same flow -- build a split, create
 the evaluators, fit a few recommenders with fit(**hyperparameters), evaluate, save and reload a model -- with the hot
-loops on a B200 and a synthetic data set instead of the Movielens1M reader (no network here).
+loops on the GPU and a synthetic data set instead of the Movielens1M reader (no network here).
 
     python examples/usage_example.py
 """

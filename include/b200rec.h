@@ -1,5 +1,5 @@
 /*
- * b200rec.h -- C ABI of libb200rec.so, the B200 (sm_100a) compute core that replaces the reference's
+ * b200rec.h -- C ABI of libb200rec.so, the H100 (sm_90a) compute core that replaces the reference's
  * three Cython extension classes and the inline numpy hot loops of IALS / EASE_R / P3alpha / RP3beta.
  *
  * Boundary (SURVEY.md section 8(b)).  Every entry point below names the reference interface it replaces

@@ -5,7 +5,7 @@ may import this.
 
 The three extension modules are compiled from the sources where they lie under /root/reference
 (read-only) -- no reference source is copied into this repository.  Only the resulting `.so` files are
-kept, in oracle/_ref/ (git-ignored, NOT gpurun-ignored, so they travel to the GPU box):
+kept, in oracle/_ref/ (git-ignored):
 
   Base/Similarity/Cython/Compute_Similarity_Cython.pyx                    -> Compute_Similarity_Cython*.so
   SLIM_BPR/Cython/SLIM_BPR_Cython_Epoch.pyx                               -> SLIM_BPR_Cython_Epoch*.so

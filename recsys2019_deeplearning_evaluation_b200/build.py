@@ -1,9 +1,8 @@
-"""In-tree build of libb200rec.so (sm_100a only).  `python -m recsys2019_deeplearning_evaluation_b200.build`.
+"""In-tree build of libb200rec.so (sm_90a only).  `python -m recsys2019_deeplearning_evaluation_b200.build`.
 (The checkers -- the C oracle and the compiled reference -- are built by oracle/build_oracle.py and oracle/build_ref.py,
 called from __graft_entry__.build().)
 
-nvcc cross-compiles without a GPU.  The resulting .so is git-ignored but travels to the GPU box with the
-gpurun snapshot.  Incremental: a source is recompiled only when it (or a header) is newer than its object.
+nvcc cross-compiles without a GPU.  The resulting .so and objects are git-ignored.  Incremental: a source is recompiled only when it (or a header) is newer than its object.
 """
 import glob
 import os
@@ -18,7 +17,7 @@ OBJ = os.path.join(PKG, "csrc", "_obj")
 LIB = os.path.join(PKG, "libb200rec.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC,
     "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
@@ -58,7 +57,7 @@ def build_lib(force=False, verbose=False):
                 sys.stderr.write(r.stdout)
             rebuilt = True
     if rebuilt or force or _newer(LIB, objs):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout)

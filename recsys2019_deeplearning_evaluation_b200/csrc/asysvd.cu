@@ -1,4 +1,4 @@
-// K2b: AsymmetricSVD epochs (Koren 2008), sm_100a.
+// K2b: AsymmetricSVD epochs (Koren 2008), sm_90a.
 //
 // Replaces MatrixFactorization/Cython/MatrixFactorization_Cython_Epoch.pyx:396-578 epochIteration_Cython_ASY_SVD_SGD
 // (batch size 1, :399), with sampleMSE_Cython :881-938 and adaptive_gradient :838-876.  The model is two n_items x f
@@ -8,7 +8,7 @@
 //
 // The recursion is strictly sequential (sample t+1 reads rows sample t wrote: two profiles of ~150 items out of 27 K share
 // an item more often than not), so ONE CTA walks the replayed sample stream in order and spreads the len_u x f reads and
-// read-modify-writes of a sample over its 32 warps.  Measured with per-phase cycle counters (profiles/r02_asysvd_phase_*):
+// read-modify-writes of a sample over its 32 warps.  Per-phase cycle counters showed that
 // the scalar one-warp-per-row version was ISSUE-bound (150 warp instructions per 32-element row, 24 K per sample on four
 // schedulers), not latency-bound -- so rows are padded to a multiple of four factors and handled as float4s, min(32, f/4)
 // lanes per row and several rows per warp instruction.

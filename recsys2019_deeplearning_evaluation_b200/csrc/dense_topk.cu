@@ -1,4 +1,4 @@
-// K1b: top-K along the rows or columns of a dense fp32 matrix resident in HBM, sm_100a.
+// K1b: top-K along the rows or columns of a dense fp32 matrix resident in HBM, sm_90a.
 //
 // Replaces the two numpy top-K loops the reference runs over item-item matrices:
 //   * Base/Recommender_utils.py:55-122 similarityMatrixTopK -- per COLUMN, the k largest of the NON-ZERO values

@@ -1,4 +1,4 @@
-// K5: EASE^R closed form on the device, sm_100a.
+// K5: EASE^R closed form on the device, sm_90a.
 //
 // Replaces EASE_R/EASE_R_Recommender.py:55-69:  G = X^T X (through Compute_Similarity, shrink 0, normalize False,
 // topK = n_items), G[diag] = item_popularity + l2_norm (nnz count per column, :62-63), P = inv(G) (np.linalg.inv on
@@ -10,8 +10,8 @@
 //      panel L21 = A21 inv(L11)^T and trailing update A22 -= L21 L21^T as GEMMs;
 //   2. inverse of the factor block column by block column, one batched GEMM pair per block diagonal;
 //   3. P = Linv^T Linv with the K range of every tile clipped to the non-zero (lower-triangular) part.
-// All three are O(n^3) GEMM work and run on the tensor cores: gemm_tc.cuh (tcgen05.mma kind::tf32 with a 3xTF32 operand
-// split for fp32-level accuracy -- the reference inverts in fp32 LAPACK -- accumulators in TMEM).  Only the 128 x 128
+// All three are O(n^3) GEMM work and run on the tensor cores: gemm_tc2.cuh / gemm_tc.cuh (wgmma .tf32 with a 3xTF32 operand
+// split for fp32-level accuracy -- the reference inverts in fp32 LAPACK -- accumulators in registers).  Only the 128 x 128
 // diagonal-block factorisations stay on the CUDA cores (one CTA each, O(n * NB^2) work in total).
 #include <algorithm>
 #include <vector>
@@ -95,8 +95,8 @@ __global__ void copy_block_kernel(const float* __restrict__ src, int lds, float*
   dst[(long long)r * ldd + c] = src[(long long)r * lds + c];
 }
 
-// 2 = gemm_tc2.cuh (default: packed operands + cp.async.bulk producer; B200, 17 792^3 triangular product: 21.5 ms against
-// 130.6 ms, EASE parity green), 1 = gemm_tc.cuh (the first kernel, kept selectable with B200REC_GEMM=1 for A/B timing)
+// 2 = gemm_tc2.cuh (default: packed operands + cp.async.bulk producer), 1 = gemm_tc.cuh (the first kernel, kept selectable
+// with B200REC_GEMM=1 for A/B timing)
 int g_gemm_version = -1;
 int gemm_version() {
   if (g_gemm_version < 0) {
@@ -132,7 +132,7 @@ void gemm_v2(cudaStream_t st, int M, int N, int K, float alpha, const float* A, 
     tc2::pack_tiles_kernel<TB><<<dim3(KC, RB, batch), tc2::THREADS, 2 * tc::TILE_BYTES, st>>>(B, ldb, sB, g_pack_b.get(), strideBp);
     count_launch();
   }
-  tc2::tc2_gemm_kernel<<<dim3(RB, RA, batch), tc2::THREADS, tc2::SMEM_BYTES, st>>>(
+  tc2::tc2_gemm_kernel<<<dim3(RB, RA, batch), tc2::GEMM_THREADS, tc2::SMEM_BYTES, st>>>(
       K, TRI ? 1 : 0, alpha, g_pack_a.get(), strideAp, share ? g_pack_a.get() : g_pack_b.get(), share ? strideAp : strideBp, beta, C, ldc, sC);
   count_launch();
 }
@@ -266,7 +266,7 @@ int b200_ease_from_gram_device(const float* d_G, int n_items, const int32_t* d_u
     B200_CUDA(cudaMemsetAsync(cnt.get(), 0, sizeof(int) * (size_t)n, st));
     copy_block_kernel<<<div_up((long long)n * n, 256), 256, 0, st>>>(d_G, n, A.get(), n_pad, n, n);
     count_launch();
-    if (nnz > 0) { col_count_kernel<<<148 * 8, 256, 0, st>>>(d_urm_indices, nnz, cnt.get()); count_launch(); }
+    if (nnz > 0) { col_count_kernel<<<sm_count() * 8, 256, 0, st>>>(d_urm_indices, nnz, cnt.get()); count_launch(); }
     set_diag_kernel<<<div_up(n_pad, 256), 256, 0, st>>>(A.get(), n, n_pad, cnt.get(), l2_norm);
     count_launch();
     int rc = b200_spd_inverse_device(A.get(), n_pad, work.get(), stream);

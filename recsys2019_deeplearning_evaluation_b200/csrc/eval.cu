@@ -1,4 +1,4 @@
-// Evaluation inner loop fused behind the top-N kernel (SURVEY.md 8(f).1), sm_100a.
+// Evaluation inner loop fused behind the top-N kernel (SURVEY.md 8(f).1), sm_90a.
 //
 // Replaces Base/Evaluation/Evaluator.py:305-388 (_compute_metrics_on_recommendation_list) and the per-user functions of
 // Base/Evaluation/metrics.py it calls: precision :214, precision_recall_min_denominator :225, recall :237,

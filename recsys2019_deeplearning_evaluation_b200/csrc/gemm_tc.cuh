@@ -1,17 +1,16 @@
-// fp32-accurate GEMM on the 5th-generation tensor cores (tcgen05, sm_100a): C = alpha * op(A) * op(B) + beta * C.
+// fp32-accurate GEMM on the Hopper tensor cores (wgmma, sm_90a): C = alpha * op(A) * op(B) + beta * C.
 //
 // Each operand element x is split into two TF32 numbers, x = hi + lo (hi = rna_tf32(x), lo = rna_tf32(x - hi)), and every
-// 128 x 128 x 8 step issues three tcgen05.mma.kind::tf32 instructions, hi*hi + hi*lo + lo*hi, into one fp32 accumulator
-// tile in tensor memory ("3xTF32": the dropped lo*lo term is ~2^-22 relative, so the result is fp32-accurate, which the
-// 1e-4 parity bar of the EASE_R inverse needs; a single TF32 pass is not).
+// 64 x 128 x 8 step of a warpgroup issues three wgmma.mma_async .tf32 instructions, hi*hi + hi*lo + lo*hi, into one fp32
+// accumulator tile held in registers ("3xTF32": the dropped lo*lo term is ~2^-22 relative, so the result is fp32-accurate,
+// which the 1e-4 parity bar of the EASE_R inverse needs; a single TF32 pass is not).
 //
-// One CTA (256 threads) per 128 x 128 output tile.  K is consumed in chunks of 32: all threads load the two operand
-// chunks from global memory, split them and store hi / lo tiles in shared memory in the canonical no-swizzle K-major
-// UMMA layout (8-row x 16-byte core matrices; LBO = 128 B between K-adjacent cores, SBO = 1024 B between 8-row groups),
-// two stages deep.  One elected thread issues the 12 MMAs of a chunk and commits them to the stage's mbarrier, which
-// gates the reuse of that stage's shared memory; loads of chunk k+1 overlap the MMAs of chunk k.  The accumulator
-// (128 lanes x 128 columns of TMEM) is read back with tcgen05.ld (32x32b.x32) by all 8 warps for the alpha/beta epilogue.
-// Descriptor bit layouts follow cute/arch/mma_sm100_desc.hpp (SmemDescriptor, InstrDescriptor).
+// One CTA (256 threads = two warpgroups) per 128 x 128 output tile; warpgroup g owns rows 64 g .. 64 g + 63.  K is consumed
+// in chunks of 32: all threads load the two operand chunks from global memory, split them and store hi / lo tiles in shared
+// memory in the canonical no-swizzle K-major layout (8-row x 16-byte core matrices; LBO = 128 B between K-adjacent cores,
+// SBO = 1024 B between 8-row groups), two stages deep.  The loads of chunk k+1 overlap the wgmmas of chunk k: a warpgroup
+// waits for its own wgmmas of chunk k before the block-wide barrier that publishes chunk k+1, so once that barrier is passed
+// nobody reads the stage chunk k+2 will overwrite.  Descriptor bit layout as cute/arch/mma_sm90_desc.hpp (GmmaDescriptor).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -22,9 +21,9 @@ namespace tc {
 constexpr int BM = 128, BN = 128, BK = 32;   // BK in fp32/tf32 elements (128 bytes per row)
 constexpr int TILE_BYTES = BM * BK * 4;      // 16 KB
 constexpr int STAGES = 2;
-constexpr int SMEM_BYTES = STAGES * 4 * TILE_BYTES + 64;  // {A_hi, A_lo, B_hi, B_lo} per stage + barriers
+constexpr int SMEM_BYTES = STAGES * 4 * TILE_BYTES;  // {A_hi, A_lo, B_hi, B_lo} per stage
 constexpr int THREADS = 256;
-constexpr uint32_t TMEM_COLS = 128;
+constexpr uint32_t WG_ROWS_BYTES = 64 / 8 * (BK / 4) * 128;  // 64 tile rows = 8 row groups of 1024 B
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -33,12 +32,8 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   d |= (uint64_t)((saddr >> 4) & 0x3FFFu);                     // start address, 16-byte units
   d |= (uint64_t)((128u >> 4) & 0x3FFFu) << 16;                // leading byte offset: next core matrix along K
   d |= (uint64_t)((((BK / 4) * 128u) >> 4) & 0x3FFFu) << 32;   // stride byte offset: next 8-row group
-  d |= (uint64_t)1 << 46;                                      // descriptor version 1 (sm_100)
-  return d;                                                    // base offset 0, layout type 0 = no swizzle
+  return d;                                                    // base offset 0, layout type 0 = no swizzle (interleave)
 }
-
-// kind::tf32, D = fp32, A and B K-major, M = 128, N = 128
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
 
 __device__ __forceinline__ uint32_t tile_offset(int row, int k) {
   return (uint32_t)((((row >> 3) * (BK / 4) + (k >> 2)) << 7) + ((row & 7) << 4) + ((k & 3) << 2));
@@ -101,14 +96,58 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "}\n" ::"r"(bar), "r"(parity) : "memory");
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+// ---- warpgroup MMA (every thread of the warpgroup executes these)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D(64 x 128) += A(64 x 8) B(128 x 8)^T: tf32 operands K-major in shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(IDESC), "r"(accumulate) : "memory");
+      "setp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc)
+      : "memory");
 }
+
+// D(64 x 64) += A(64 x 8) B(64 x 8)^T: tf32 operands K-major in shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc)
+      : "memory");
+}
+
+// D(64 x 32) += A(64 x 8) B(32 x 8)^T: tf32 operands K-major in shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a_desc), "l"(b_desc)
+      : "memory");
+}
+
+// Accumulator fragment of a 64 x N wgmma tile: register i of thread t (warp w = (t / 32) % 4, lane l) holds
+// row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
+__device__ __forceinline__ int frag_row(int i, int t) { return 16 * ((t >> 5) & 3) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int i, int t) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
 
 // TA: op(A)(m, k) = A[k * lda + m]; TB: op(B)(k, n) = B[n * ldb + k].  TRI: op(A) = L^T, op(B) = L with L lower
 // triangular, so only k >= max(m0, n0) contributes.  M, N multiples of 128, K a multiple of 32.  blockIdx.z = batch.
@@ -117,28 +156,16 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(int M, int N, int K
                                                              long long strideA, const float* __restrict__ B, int ldb, long long strideB,
                                                              float beta, float* C, int ldc, long long strideC) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t s_tmem_base;
   A += (long long)blockIdx.z * strideA;
   B += (long long)blockIdx.z * strideB;
   C += (long long)blockIdx.z * strideC;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   unsigned char* tiles = smem;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * 4 * TILE_BYTES);
-  const uint32_t bar0 = smem_u32(bars);
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 32) {
-    for (int s = 0; s < STAGES; ++s) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8u * s) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = s_tmem_base;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
   const int k_begin = TRI ? (max(m0, n0) / BK) * BK : 0;
   const int nk = (K - k_begin) / BK;
@@ -149,72 +176,37 @@ __global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(int M, int N, int K
     unsigned char* a_lo = tiles + (s * 4 + 1) * TILE_BYTES;
     unsigned char* b_hi = tiles + (s * 4 + 2) * TILE_BYTES;
     unsigned char* b_lo = tiles + (s * 4 + 3) * TILE_BYTES;
-    if (kb >= STAGES) mbar_wait(bar0 + 8u * s, (uint32_t)(((kb >> 1) - 1) & 1));  // MMAs that read this stage are done
     if (TA) load_tile_rowcontig(A, lda, m0, k0, a_hi, a_lo, tid); else load_tile_kcontig(A, lda, m0, k0, a_hi, a_lo, tid);
     if (TB) load_tile_kcontig(B, ldb, n0, k0, b_hi, b_lo, tid); else load_tile_rowcontig(B, ldb, n0, k0, b_hi, b_lo, tid);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
+    wgmma_wait<0>();  // this warpgroup's wgmmas of chunk kb-1 (the other stage) are done
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t ah = smem_u32(a_hi), al = smem_u32(a_lo), bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+    wgmma_fence();
+    const uint32_t ah = smem_u32(a_hi) + wg * WG_ROWS_BYTES, al = smem_u32(a_lo) + wg * WG_ROWS_BYTES;
+    const uint32_t bh = smem_u32(b_hi), bl = smem_u32(b_lo);
 #pragma unroll
-      for (int ks = 0; ks < BK / 8; ++ks) {  // one MMA consumes K = 8 tf32 = two core matrices = 256 bytes
-        const uint32_t o = ks * 256u;
-        umma_tf32(tmem, make_smem_desc(ah + o), make_smem_desc(bh + o), (kb > 0 || ks > 0) ? 1u : 0u);
-        umma_tf32(tmem, make_smem_desc(ah + o), make_smem_desc(bl + o), 1u);
-        umma_tf32(tmem, make_smem_desc(al + o), make_smem_desc(bh + o), 1u);
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar0 + 8u * s) : "memory");
+    for (int ks = 0; ks < BK / 8; ++ks) {  // one wgmma consumes K = 8 tf32 = two core matrices = 256 bytes
+      const uint32_t o = ks * 256u;
+      wgmma_m64n128k8_tf32(acc, make_smem_desc(ah + o), make_smem_desc(bh + o));
+      wgmma_m64n128k8_tf32(acc, make_smem_desc(ah + o), make_smem_desc(bl + o));
+      wgmma_m64n128k8_tf32(acc, make_smem_desc(al + o), make_smem_desc(bh + o));
     }
+    wgmma_commit();
   }
-  if (nk > 0) {
-    const int last = nk - 1;
-    mbar_wait(bar0 + 8u * (last & 1), (uint32_t)((last >> 1) & 1));
-  }
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  wgmma_wait<0>();
 
-  // epilogue: warp w reads TMEM lanes 32*(w%4) .. +31 (its row of the tile), columns 64*(w/4) .. +63
-  const int row = (warp & 3) * 32 + lane;
-  const int col0 = (warp >> 2) * 64;
-  float* crow = C + (long long)(m0 + row) * ldc + n0 + col0;
+  // epilogue: every thread writes its accumulator fragment, two adjacent columns per store
+  const int t = tid & 127;
 #pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    uint32_t v[32];
-    if (nk > 0) {
-      const uint32_t taddr = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(col0 + half * 32);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-            "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-            "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-            "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr)
-          : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    } else {
-#pragma unroll
-      for (int c = 0; c < 32; ++c) v[c] = 0u;
+  for (int i = 0; i < 64; i += 2) {
+    float2* dst = reinterpret_cast<float2*>(C + (long long)(m0 + wg * 64 + frag_row(i, t)) * ldc + n0 + frag_col(i, t));
+    float2 o = make_float2(alpha * acc[i], alpha * acc[i + 1]);
+    if (beta != 0.f) {
+      const float2 old = *dst;
+      o.x += beta * old.x; o.y += beta * old.y;
     }
-#pragma unroll
-    for (int c4 = 0; c4 < 8; ++c4) {
-      float4 o;
-      o.x = alpha * __uint_as_float(v[c4 * 4 + 0]);
-      o.y = alpha * __uint_as_float(v[c4 * 4 + 1]);
-      o.z = alpha * __uint_as_float(v[c4 * 4 + 2]);
-      o.w = alpha * __uint_as_float(v[c4 * 4 + 3]);
-      float4* dst = reinterpret_cast<float4*>(crow + half * 32 + c4 * 4);
-      if (beta != 0.f) {
-        const float4 old = *dst;
-        o.x += beta * old.x; o.y += beta * old.y; o.z += beta * old.z; o.w += beta * old.w;
-      }
-      *dst = o;
-    }
+    *dst = o;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS) : "memory");
 }
 
 }  // namespace tc

@@ -1,19 +1,16 @@
-// Second-generation 3xTF32 tcgen05 GEMM (sm_100a): pre-packed operands fed by the TMA engine's bulk copies.
+// Second-generation 3xTF32 wgmma GEMM (sm_90a): pre-packed operands fed by the TMA engine's bulk copies.
 //
-// STATUS: opt-in (B200REC_GEMM=2 at run time, see ease.cu); gemm_tc.cuh stays the default until this path has passed
-// tests/test_ease_gpu.py::test_gemm_versions on a B200 (it was written in a session without GPU time left).
-//
-// Why: the ncu capture of gemm_tc.cuh (profiles/r01_tc_gemm_c4.txt) shows the tensor pipe 7.8 % active -- the CTA spends
-// its time converting operands (cvt.rna.tf32, 72 % of the samples) and storing them transposed with 4-byte stores, and
-// the loads of chunk k+1 only start after the whole block has synchronised on chunk k.  Here
+// gemm_tc.cuh spends most of its time converting operands (cvt.rna.tf32) and storing them transposed with 4-byte stores,
+// and the loads of chunk k+1 only start after the whole block has synchronised on chunk k.  Here
 //   * a pack pass splits every operand ONCE into hi / lo TF32 parts and writes them in the exact shared-memory image of a
-//     128 x 32 UMMA tile (canonical no-swizzle K-major layout, same tile_offset as gemm_tc.cuh), hi and lo adjacent:
+//     128 x 32 wgmma tile (canonical no-swizzle K-major layout, same tile_offset as gemm_tc.cuh), hi and lo adjacent:
 //     packed[(row_block * KC + k_chunk) * 8192 floats] = {hi tile 16 KB, lo tile 16 KB};
-//   * the GEMM kernel is warp-specialised: one producer lane issues two 32 KB `cp.async.bulk` copies per 128x128x32
-//     step (A hi+lo, B hi+lo) that complete on the stage's "full" mbarrier, one MMA lane waits for it, issues the
-//     12 tcgen05.mma.kind::tf32 of the step (hi*hi + hi*lo + lo*hi) and commits them to the stage's "empty" mbarrier,
-//     three stages deep (192 KB); nobody else touches shared memory, no block-wide barrier inside the K loop;
-//   * the epilogue (all 8 warps, tcgen05.ld 32x32b.x32) is the one of gemm_tc.cuh.
+//   * the GEMM kernel is warp-specialised: one producer lane (warpgroup 0) issues two 32 KB `cp.async.bulk` copies per
+//     128x128x32 step (A hi+lo, B hi+lo) that complete on the stage's "full" mbarrier; each of the two consumer warpgroups
+//     waits for it, issues the 12 wgmmas of its 64 x 128 half of the step (hi*hi + hi*lo + lo*hi) and, once the wgmmas of
+//     the step before have completed, releases that step's stage on its "empty" mbarrier; three stages deep (192 KB), no
+//     block-wide barrier at all;
+//   * each consumer warpgroup writes its accumulators from registers (the epilogue of gemm_tc.cuh).
 // O(M K + N K) pack work against O(M N K) MMA work; the packed copies live in a workspace the caller provides.
 #pragma once
 #include "gemm_tc.cuh"
@@ -27,8 +24,9 @@ using tc::BN;
 using tc::TILE_BYTES;
 constexpr int STAGES = 3;
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;                  // A hi, A lo, B hi, B lo
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 128;       // + full[3], empty[3], done barriers
-constexpr int THREADS = 256;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 64;        // + full[3], empty[3] barriers
+constexpr int THREADS = 256;                                 // pack kernel
+constexpr int GEMM_THREADS = 384;                            // producer warpgroup + two consumer warpgroups
 constexpr int PAIR_FLOATS = 2 * TILE_BYTES / 4;              // one packed (hi, lo) tile pair: 8192 floats
 
 // One CTA packs one 128 x 32 tile of op(X): KCONTIG = the k index is contiguous in memory (tile(row, k) = src[row*ld + k]),
@@ -56,12 +54,11 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 
 // C = alpha * op(A) op(B) + beta * C from packed operands.  TRI: only k >= max(m0, n0) contributes (L^T L products).
 // grid = (N/128, M/128, batch).
-__global__ void __launch_bounds__(THREADS, 1) tc2_gemm_kernel(int K, int tri, float alpha, const float* __restrict__ Ap, long long strideAp,
-                                                              const float* __restrict__ Bp, long long strideBp, float beta, float* C,
-                                                              int ldc, long long strideC) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1) tc2_gemm_kernel(int K, int tri, float alpha, const float* __restrict__ Ap,
+                                                                   long long strideAp, const float* __restrict__ Bp, long long strideBp,
+                                                                   float beta, float* C, int ldc, long long strideC) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t s_tmem_base;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int mb = blockIdx.y, nb = blockIdx.x;
   const int m0 = mb * BM, n0 = nb * BN;
   const int KC = K / BK;
@@ -69,30 +66,25 @@ __global__ void __launch_bounds__(THREADS, 1) tc2_gemm_kernel(int K, int tri, fl
   Bp += (long long)blockIdx.z * strideBp + (long long)nb * KC * PAIR_FLOATS;
   C += (long long)blockIdx.z * strideC;
   const uint32_t tiles = tc::smem_u32(smem);
-  const uint32_t bar0 = tiles + STAGES * STAGE_BYTES;  // full[s] = bar0 + 8 s, empty[s] = bar0 + 8 (STAGES + s), done = bar0 + 16 STAGES
-  const uint32_t bar_done = bar0 + 16u * STAGES;
+  const uint32_t bar0 = tiles + STAGES * STAGE_BYTES;  // full[s] = bar0 + 8 s, empty[s] = bar0 + 8 (STAGES + s)
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&s_tmem_base)), "r"(tc::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 32) {
-    for (int b = 0; b < 2 * STAGES + 1; ++b) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8u * b) : "memory");
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8u * s) : "memory");
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], 2;" ::"r"(bar0 + 8u * (STAGES + s)) : "memory");  // one arrival per consumer
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = s_tmem_base;
 
   const int kc_begin = tri ? max(m0, n0) / BK : 0;
   const int nk = KC - kc_begin;
 
-  if (warp == 0) {
-    if (lane == 0) {  // ---- producer: two 32 KB bulk copies per stage
+  if (wg == 0) {
+    if (tid == 0) {  // ---- producer: two 32 KB bulk copies per stage
       for (int kb = 0; kb < nk; ++kb) {
         const int s = kb % STAGES, it = kb / STAGES;
-        if (it > 0) tc::mbar_wait(bar0 + 8u * (STAGES + s), (uint32_t)((it - 1) & 1));  // the MMAs that read this stage are done
+        if (it > 0) tc::mbar_wait(bar0 + 8u * (STAGES + s), (uint32_t)((it - 1) & 1));  // the wgmmas that read this stage are done
         const uint32_t full = bar0 + 8u * s;
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "r"((uint32_t)STAGE_BYTES) : "memory");
         const uint32_t dst = tiles + (uint32_t)s * STAGE_BYTES;
@@ -100,72 +92,43 @@ __global__ void __launch_bounds__(THREADS, 1) tc2_gemm_kernel(int K, int tri, fl
         bulk_g2s(dst + 2 * TILE_BYTES, Bp + (long long)(kc_begin + kb) * PAIR_FLOATS, 2 * TILE_BYTES, full);
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {  // ---- MMA issuer
-      for (int kb = 0; kb < nk; ++kb) {
-        const int s = kb % STAGES, it = kb / STAGES;
-        tc::mbar_wait(bar0 + 8u * s, (uint32_t)(it & 1));  // both copies of this stage have landed
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t ah = tiles + (uint32_t)s * STAGE_BYTES, al = ah + TILE_BYTES, bh = ah + 2 * TILE_BYTES, bl = ah + 3 * TILE_BYTES;
-#pragma unroll
-        for (int ks = 0; ks < BK / 8; ++ks) {  // one MMA consumes K = 8 tf32 = two core matrices = 256 bytes
-          const uint32_t o = ks * 256u;
-          tc::umma_tf32(tmem, tc::make_smem_desc(ah + o), tc::make_smem_desc(bh + o), (kb > 0 || ks > 0) ? 1u : 0u);
-          tc::umma_tf32(tmem, tc::make_smem_desc(ah + o), tc::make_smem_desc(bl + o), 1u);
-          tc::umma_tf32(tmem, tc::make_smem_desc(al + o), tc::make_smem_desc(bh + o), 1u);
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar0 + 8u * (STAGES + s)) : "memory");
-      }
-      if (nk > 0) asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_done) : "memory");
-    }
-    __syncwarp();
+    return;
   }
-  if (nk > 0) tc::mbar_wait(bar_done, 0u);  // every MMA of the tile has completed
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 
-  // epilogue (as gemm_tc.cuh): warp w reads TMEM lanes 32*(w%4) .. +31 (its rows of the tile), columns 64*(w/4) .. +63
-  const int row = (warp & 3) * 32 + lane;
-  const int col0 = (warp >> 2) * 64;
-  float* crow = C + (long long)(m0 + row) * ldc + n0 + col0;
+  // ---- consumers: warpgroup 1 + h computes rows 64 h .. 64 h + 63 of the tile
+  const int h = wg - 1, t = tid & 127;
+  float acc[64];
 #pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    uint32_t v[32];
-    if (nk > 0) {
-      const uint32_t taddr = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(col0 + half * 32);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-            "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-            "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-            "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr)
-          : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    } else {
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int kb = 0; kb < nk; ++kb) {
+    const int s = kb % STAGES, it = kb / STAGES;
+    tc::mbar_wait(bar0 + 8u * s, (uint32_t)(it & 1));  // both copies of this stage have landed
+    const uint32_t ah = tiles + (uint32_t)s * STAGE_BYTES, al = ah + TILE_BYTES, bh = ah + 2 * TILE_BYTES, bl = ah + 3 * TILE_BYTES;
+    const uint32_t ra = (uint32_t)h * tc::WG_ROWS_BYTES;
+    tc::wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 32; ++c) v[c] = 0u;
+    for (int ks = 0; ks < BK / 8; ++ks) {  // one wgmma consumes K = 8 tf32 = two core matrices = 256 bytes
+      const uint32_t o = ks * 256u;
+      tc::wgmma_m64n128k8_tf32(acc, tc::make_smem_desc(ah + ra + o), tc::make_smem_desc(bh + o));
+      tc::wgmma_m64n128k8_tf32(acc, tc::make_smem_desc(ah + ra + o), tc::make_smem_desc(bl + o));
+      tc::wgmma_m64n128k8_tf32(acc, tc::make_smem_desc(al + ra + o), tc::make_smem_desc(bh + o));
     }
-#pragma unroll
-    for (int c4 = 0; c4 < 8; ++c4) {
-      float4 o;
-      o.x = alpha * __uint_as_float(v[c4 * 4 + 0]);
-      o.y = alpha * __uint_as_float(v[c4 * 4 + 1]);
-      o.z = alpha * __uint_as_float(v[c4 * 4 + 2]);
-      o.w = alpha * __uint_as_float(v[c4 * 4 + 3]);
-      float4* dst = reinterpret_cast<float4*>(crow + half * 32 + c4 * 4);
-      if (beta != 0.f) {
-        const float4 old = *dst;
-        o.x += beta * old.x; o.y += beta * old.y; o.z += beta * old.z; o.w += beta * old.w;
-      }
-      *dst = o;
-    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<1>();  // the wgmmas of step kb - 1 are done: its stage may be refilled
+    if (kb > 0 && t == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar0 + 8u * (STAGES + (kb - 1) % STAGES)) : "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tc::TMEM_COLS) : "memory");
+  tc::wgmma_wait<0>();
+
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    float2* dst = reinterpret_cast<float2*>(C + (long long)(m0 + h * 64 + tc::frag_row(i, t)) * ldc + n0 + tc::frag_col(i, t));
+    float2 o = make_float2(alpha * acc[i], alpha * acc[i + 1]);
+    if (beta != 0.f) {
+      const float2 old = *dst;
+      o.x += beta * old.x; o.y += beta * old.y;
+    }
+    *dst = o;
+  }
 }
 
 }  // namespace tc2

@@ -1,4 +1,4 @@
-// K4: implicit-ALS half epochs (per-row normal equations), sm_100a.
+// K4: implicit-ALS half epochs (per-row normal equations), sm_90a.
 //
 // Replaces MatrixFactorization/IALSRecommender.py:137-201: for every warm user (then every warm item)
 //     A = Y_p^T diag(c - 1) Y_p,   B = Y^T Y + A + reg * I,   x = B^{-1} Y_p^T c
@@ -12,7 +12,7 @@
 // same register tiling over row chunks with fp64 atomics.
 // Everything is fp64 like the reference (:204-210): with the reference's all-positive initial factors the systems
 // have condition numbers ~1e6, beyond what an fp32 factorisation resolves to the 1e-4 parity bar.
-// ROUND-1 STATUS: CUDA-core fp64; the tensor-core (tcgen05) Gram accumulation is the round-2 item (DESIGN.md K4).
+// CUDA-core fp64; the tensor-core kernel for n_factors >= 128 is ials_v2.cuh (DESIGN.md K4).
 // n_factors <= 208: the packed fp64 matrix lives in shared memory.  208 < n_factors <= 256 (BASELINE.json configs[3]):
 // the first R rows of the packed matrix stay in shared memory, the last ones in a per-CTA slab of global memory, and
 // the register-tiled Gram accumulation takes two passes over the profile (136 fp64 accumulators do not fit one).
@@ -266,9 +266,10 @@ bool run_v2(cudaStream_t st, const int* rows, int n_solve, const int* ptr, const
   DevBuf<int> redo(1);
   B200_CUDA(cudaMemsetAsync(redo.get(), 0, sizeof(int), st));
   const size_t smem = ials2::smem_bytes(f);
-  B200_CUDA(cudaFuncSetAttribute(ials2::ials_rows_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  auto kern = f > 128 ? ials2::ials_rows_v2_kernel<true> : ials2::ials_rows_v2_kernel<false>;
+  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = std::max(1, std::min(n_solve, sm_count()));
-  ials2::ials_rows_v2_kernel<<<grid, ials2::T, smem, st>>>(rows, n_solve, ptr, idx, conf, Y, YtY, f, reg, X, info, redo.get(), 2);
+  kern<<<grid, ials2::T, smem, st>>>(rows, n_solve, ptr, idx, conf, Y, YtY, f, reg, X, info, redo.get(), 2);
   B200_CUDA(cudaGetLastError());
   count_launch();
   int h_redo = 0;
@@ -300,7 +301,6 @@ int b200_ials_half_epoch_device(const int32_t* d_rows, int n_solve, const int32_
     // (well-conditioned systems; B200REC_IALS_V2=0 switches it off); a row whose refinement does not contract sends the half
     // epoch back to the fp64 kernel below
     const int v2_env = getenv("B200REC_IALS_V2") ? atoi(getenv("B200REC_IALS_V2")) : -1;  // 0 off, 1 every size, unset: where it wins
-    // measured on C4 (profiles/r02_ials_v2_c4.txt): 256 factors 1.06 s per epoch against 11.7 s, 128 factors 0.56 s against 0.83 s
     const bool want_v2 = v2_env == 1 || (v2_env != 0 && f >= 128);
     if (want_v2 && n_other >= 4 * f) {
       if (ials::run_v2(st, d_rows, n_solve, d_ptr, d_idx, d_conf, d_Y, n_other, f, reg, d_X, d_YtY_work, info.get())) {

@@ -1,18 +1,21 @@
-// K4 on the tensor cores, second generation (sm_100a): implicit-ALS half epochs for n_factors <= 256.
+// K4 on the tensor cores, second generation (sm_90a): implicit-ALS half epochs for n_factors <= 256.
 //
 // Replaces MatrixFactorization/IALSRecommender.py:137-201 like ials.cu (per warm row:  A = Y_p^T diag(c - 1) Y_p,
-// B = Y^T Y + A + reg I,  x = B^-1 Y_p^T c), with the dense contraction on tcgen05 as BASELINE.json's north_star asks.
+// B = Y^T Y + A + reg I,  x = B^-1 Y_p^T c), with the dense contraction on the tensor cores (wgmma) as BASELINE.json's
+// north_star asks.
 //
 // Why a second generation.  ials.cu accumulates the Gram in fp64 registers and factors a packed fp64 matrix that no longer
-// fits shared memory above 208 factors: one C4 epoch at 256 factors takes 11.7 s.  The first tensor-core kernel (one
-// 128 x 128 accumulator, fp64 Cholesky, round 1) only covered 128 factors and was 3x slower than the fp64 kernel it was
-// meant to replace -- scalar staging and an unblocked factorisation (profiles/r02_hotpath3_c4_timings.txt).  Here:
+// fits shared memory above 208 factors, so it is slow there.  The first tensor-core kernel (one 128 x 128 accumulator,
+// fp64 Cholesky) only covered 128 factors and was slower than the fp64 kernel it was meant to replace -- scalar staging and an unblocked factorisation.  Here:
 //   * Gram on the tensor core, 3xTF32 (fp32-accurate).  The profile's factor rows are scaled by sqrt(c - 1) while they are
 //     staged, so ONE operand serves both sides of  A = (sqrt(c-1) Y_p)^T (sqrt(c-1) Y_p): per 32 profile entries a
-//     256 x 32 hi tile and a lo tile (K-major UMMA layout, 128-bit shared stores, two stages).  Only the lower triangle is
-//     formed: accumulator D0 = rows 0..127 x columns 0..127 (M = 128, N = 128), D1 = rows 128..255 x columns 0..255
-//     (M = 128, N = 256); 384 of the 512 TMEM columns.  One elected thread issues the 24 MMAs of a step and commits them to
-//     the stage's mbarrier; the staging of the next step overlaps them.
+//     256 x 32 hi tile and a lo tile (K-major wgmma layout, 128-bit shared stores, two stages).  Only the lower triangle is
+//     formed, in register accumulators of the four warpgroups.  Above 128 factors (TWO) it is cut into the 20 blocks of
+//     64 rows x 32 columns that meet the lower triangle of 256 x 256; block b (row-major order) belongs to warpgroup b % 4
+//     (5 blocks, 80 fp32 per thread, three m64n32k8 wgmmas per block and 8 profile entries).  Up to 128 factors each
+//     warpgroup owns one 64 x 64 block of the 128 x 128 matrix (the fourth one, above the diagonal, is discarded).  Every
+//     warpgroup issues the same instruction sequence whatever n_factors is, so the wgmmas pipeline.  The staging of the
+//     next step overlaps the wgmmas of this one.
 //   * B in fp32, lower triangle, rows padded to 16 bytes (133 KB at 256 factors: it takes over the staging buffers), then a
 //     right-looking blocked Cholesky with 32-wide panels: the diagonal block in the registers of one warp (shuffles), the
 //     panel by one thread per row, the trailing update by warps that own 16 x 32 blocks of it so that their 128-bit
@@ -34,42 +37,21 @@ constexpr int STAGES = 2;
 constexpr int TILE = 256 * KC * 4;       // one 256 x 32 fp32 tile: 32 KB
 constexpr int NB = 32;                   // Cholesky panel width
 constexpr int NBP = NB + 1;              // row stride of the stored diagonal-block inverses (no shared bank across rows)
-constexpr uint32_t TMEM_COLS = 512;
-// kind::tf32, D = fp32, A and B K-major, M = 128, N = 128 / 256 (cute/arch/mma_sm100_desc.hpp InstrDescriptor)
-constexpr uint32_t IDESC_N128 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-constexpr uint32_t IDESC_N256 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+constexpr int GB = 5;                    // Gram blocks (64 x 32) per warpgroup: 20 blocks of the lower triangle / 4
 
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
+// block b of the lower triangle of a 256 x 256 matrix in 64 x 32 blocks, row-major: rows 64 rb.., columns 32 cb..
+__device__ __forceinline__ void gram_block(int b, int& rb, int& cb) {
+  rb = b < 2 ? 0 : b < 6 ? 1 : b < 12 ? 2 : 3;
+  cb = b - (rb == 0 ? 0 : rb == 1 ? 2 : rb == 2 ? 6 : 12);
 }
 
 // lower triangle, row r starts at roff(r) floats: rows are padded to multiples of 4 floats so that every 4-aligned column
 // offset of every row is 16-byte aligned
 __device__ __host__ __forceinline__ int roff(int r) { const int q = r >> 2, m = r & 3; return 4 * (q + 1) * (2 * q + m); }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 struct Smem {
   float* L;        // padded lower triangle (aliases the staging tiles)
   unsigned char* tiles;
-  uint64_t* bars;
   double *b0, *xs, *rs, *part;  // rhs, solution, residual / correction, [NW][f] partial sums
   float* dinv;     // [f / 32][32][33] inverses of the diagonal blocks of L (lower triangular, row-major, padded rows)
   float* sw;       // [KC] sqrt(c - 1) of the step's entries
@@ -126,12 +108,12 @@ __device__ __forceinline__ void solve_backward(const Smem& S, double* v, int f) 
   }
 }
 
+template <bool TWO>
 __global__ void __launch_bounds__(T, 1) ials_rows_v2_kernel(const int* __restrict__ rows, int n_solve, const int* __restrict__ ptr,
                                                             const int* __restrict__ idx, const float* __restrict__ conf,
                                                             const double* __restrict__ Y, const double* __restrict__ YtY, int f,
                                                             double reg, double* X, int* info, int* redo, int n_refine) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t s_tmem_base;
   __shared__ double s_norm[3];  // |r|^2 before the last / the first correction, |b|^2
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   Smem S;
@@ -141,7 +123,6 @@ __global__ void __launch_bounds__(T, 1) ials_rows_v2_kernel(const int* __restric
     o = (o + 127) & ~(size_t)127;
     S.L = reinterpret_cast<float*>(smem);
     S.tiles = smem;
-    S.bars = reinterpret_cast<uint64_t*>(smem + o); o += 64;
     S.b0 = reinterpret_cast<double*>(smem + o); o += sizeof(double) * f;
     S.xs = reinterpret_cast<double*>(smem + o); o += sizeof(double) * f;
     S.rs = reinterpret_cast<double*>(smem + o); o += sizeof(double) * f;
@@ -152,23 +133,25 @@ __global__ void __launch_bounds__(T, 1) ials_rows_v2_kernel(const int* __restric
     S.rk = reinterpret_cast<int*>(smem + o); o += sizeof(int) * KC;
     S.rdiag = reinterpret_cast<float*>(smem + o);
   }
-  const uint32_t bar0 = tc::smem_u32(S.bars);
-  const bool two = f > 128;  // rows 128.. exist: the second accumulator is in use
-
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&s_tmem_base)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  // this warpgroup's Gram blocks (64 rows x BW columns): their first row / column and the shared-memory byte offsets of their
+  // A (64 tile rows) and B (BW tile rows) operands; one tile row group of 8 is 1024 B
+  constexpr int NBLK = TWO ? GB : 1, BW = TWO ? 32 : 64;
+  const int wg = tid >> 7, t = tid & 127;
+  int r0[NBLK], c0[NBLK];
+  uint32_t a_off[NBLK], b_off[NBLK];
+#pragma unroll
+  for (int j = 0; j < NBLK; ++j) {
+    int rb, cb;
+    if (TWO) gram_block(wg + 4 * j, rb, cb);
+    else { rb = (wg == 1 || wg == 2) ? 1 : 0; cb = wg >> 1; }
+    r0[j] = rb * 64;
+    c0[j] = cb * BW;
+    a_off[j] = (uint32_t)r0[j] * 128u;
+    b_off[j] = (uint32_t)c0[j] * 128u;
   }
-  if (tid == 32) {
-    for (int s = 0; s < STAGES; ++s) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8u * s) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = s_tmem_base;
+  float acc[NBLK][BW / 2];
 
-  unsigned gk = 0;  // steps issued by this CTA so far (all rows): stage = gk & 1, its barrier phase = (gk >> 1) & 1
+  unsigned gk = 0;  // steps issued by this CTA so far (all rows): stage = gk & 1
   for (int srow = blockIdx.x; srow < n_solve; srow += gridDim.x) {
     const int row = rows[srow];
     const int p0 = ptr[row], p1 = ptr[row + 1];
@@ -176,6 +159,10 @@ __global__ void __launch_bounds__(T, 1) ials_rows_v2_kernel(const int* __restric
 
     // ================= Gram on the tensor core
     double my_rhs = 0.0;  // threads m and m + 256 each hold half of b0[m] = (Y_p^T c)[m]  (IALSRecommender.py:201)
+#pragma unroll
+    for (int j = 0; j < NBLK; ++j)
+#pragma unroll
+      for (int i = 0; i < BW / 2; ++i) acc[j][i] = 0.f;
     for (int kb = 0; kb < nk; ++kb, ++gk) {
       const int s = (int)(gk & 1u);
       unsigned char* t_hi = S.tiles + (size_t)(s * 2 + 0) * TILE;
@@ -188,7 +175,6 @@ __global__ void __launch_bounds__(T, 1) ials_rows_v2_kernel(const int* __restric
         S.sw[tid] = sqrtf(fmaxf(c - 1.f, 0.f));
         S.cw[tid] = q < p1 ? (double)c : 0.0;
       }
-      if (gk >= (unsigned)STAGES) tc::mbar_wait(bar0 + 8u * s, (uint32_t)(((gk >> 1) - 1u) & 1u));  // the MMAs that read this stage are done
       __syncthreads();
       // tile(m, k) = sqrt(c_k - 1) * Y[rk[k]][m]; thread = (factor m, half of the step's entries), four entries per 128-bit
       // store; zero past f / the profile
@@ -211,67 +197,44 @@ __global__ void __launch_bounds__(T, 1) ials_rows_v2_kernel(const int* __restric
         }
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
+      tc::wgmma_wait<0>();  // this warpgroup's wgmmas of the previous step (the other stage) are done
       __syncthreads();
-      if (tid == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t th = tc::smem_u32(t_hi), tl = tc::smem_u32(t_lo);
+      tc::wgmma_fence();
+      const uint32_t th = tc::smem_u32(t_hi), tl = tc::smem_u32(t_lo);
 #pragma unroll
-        for (int ks = 0; ks < KC / 8; ++ks) {
-          const uint32_t o = ks * 256u;
-          const uint32_t acc = (kb > 0 || ks > 0) ? 1u : 0u;
-          // D0: rows 0..127 x columns 0..127
-          umma(tmem, tc::make_smem_desc(th + o), tc::make_smem_desc(th + o), IDESC_N128, acc);
-          umma(tmem, tc::make_smem_desc(th + o), tc::make_smem_desc(tl + o), IDESC_N128, 1u);
-          umma(tmem, tc::make_smem_desc(tl + o), tc::make_smem_desc(th + o), IDESC_N128, 1u);
-          if (two) {  // D1: rows 128..255 (operand A starts 128 rows = 16 KB into the tile) x columns 0..255
-            umma(tmem + 128u, tc::make_smem_desc(th + 16384u + o), tc::make_smem_desc(th + o), IDESC_N256, acc);
-            umma(tmem + 128u, tc::make_smem_desc(th + 16384u + o), tc::make_smem_desc(tl + o), IDESC_N256, 1u);
-            umma(tmem + 128u, tc::make_smem_desc(tl + 16384u + o), tc::make_smem_desc(th + o), IDESC_N256, 1u);
-          }
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar0 + 8u * s) : "memory");
-      }
-    }
-    if (nk > 0) {
-      // every outstanding step: the tiles are about to be overwritten by L
-      if (nk > 1) { const unsigned prev = gk - 2u; tc::mbar_wait(bar0 + 8u * (prev & 1u), (uint32_t)((prev >> 1) & 1u)); }
-      const unsigned last = gk - 1u;
-      tc::mbar_wait(bar0 + 8u * (last & 1u), (uint32_t)((last >> 1) & 1u));
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    __syncthreads();
-
-    // ================= accumulators -> B = A + Y^T Y + reg I, fp32, lower triangle.  Warp w owns TMEM lanes 32 (w % 4) .. + 31
-    // (a row of each accumulator per thread) and half of the columns.
-    {
-      const int g = warp & 3, hcol = warp >> 2;  // hcol in [0, NW / 4)
-      for (int acc_i = 0; acc_i < (two ? 2 : 1); ++acc_i) {
-        const int r = acc_i * 128 + g * 32 + lane;             // row of B
-        const int ncol = acc_i == 0 ? 128 : 256;               // columns this accumulator holds
-        const int cbeg = hcol * (ncol / (NW / 4)), cend = cbeg + ncol / (NW / 4);
-        for (int c0 = cbeg; c0 < cend; c0 += 32) {
-          if (c0 > acc_i * 128 + g * 32 + 31) continue;         // above the diagonal for every row of this warp (uniform)
-          uint32_t v[32];
-          if (nk > 0) {
-            tmem_ld32(tmem + ((uint32_t)(g * 32) << 16) + (uint32_t)(acc_i * 128 + c0), v);
+      for (int ks = 0; ks < KC / 8; ++ks) {
+        const uint32_t o = ks * 256u;
+#pragma unroll
+        for (int j = 0; j < NBLK; ++j) {
+          const uint64_t ah = tc::make_smem_desc(th + a_off[j] + o), al = tc::make_smem_desc(tl + a_off[j] + o);
+          const uint64_t bh = tc::make_smem_desc(th + b_off[j] + o), bl = tc::make_smem_desc(tl + b_off[j] + o);
+          if constexpr (TWO) {
+            tc::wgmma_m64n32k8_tf32(acc[j], ah, bh);
+            tc::wgmma_m64n32k8_tf32(acc[j], ah, bl);
+            tc::wgmma_m64n32k8_tf32(acc[j], al, bh);
           } else {
-#pragma unroll
-            for (int q = 0; q < 32; ++q) v[q] = 0u;
-          }
-          if (r < f) {
-            float* Lr = S.L + roff(r);
-#pragma unroll
-            for (int q = 0; q < 32; ++q) {
-              const int c = c0 + q;
-              if (c <= r) Lr[c] = (float)((double)__uint_as_float(v[q]) + YtY[(size_t)c * f + r] + (r == c ? reg : 0.0));  // Y^T Y is symmetric: coalesced over r
-            }
+            tc::wgmma_m64n64k8_tf32(acc[j], ah, bh);
+            tc::wgmma_m64n64k8_tf32(acc[j], ah, bl);
+            tc::wgmma_m64n64k8_tf32(acc[j], al, bh);
           }
         }
+      }
+      tc::wgmma_commit();
+    }
+    tc::wgmma_wait<0>();
+    __syncthreads();  // every warpgroup's wgmmas are done: the tiles are about to be overwritten by L
+
+    // ================= accumulators -> B = A + Y^T Y + reg I, fp32, lower triangle, from this warpgroup's blocks
+#pragma unroll
+    for (int j = 0; j < NBLK; ++j) {
+#pragma unroll
+      for (int i = 0; i < BW / 2; ++i) {
+        const int r = r0[j] + tc::frag_row(i, t), c = c0[j] + tc::frag_col(i, t);
+        if (r < f && c <= r) S.L[roff(r) + c] = (float)((double)acc[j][i] + YtY[(size_t)c * f + r] + (r == c ? reg : 0.0));
       }
     }
     if (tid >= 256 && tid - 256 < f) S.rs[tid - 256] = my_rhs;  // the upper half's share of the right-hand side
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();  // every warp has read the accumulators: the next row may overwrite them
+    __syncthreads();
     if (tid < f) { const double b = my_rhs + S.rs[tid]; S.b0[tid] = b; S.xs[tid] = b; }
     __syncthreads();
 
@@ -465,15 +428,12 @@ __global__ void __launch_bounds__(T, 1) ials_rows_v2_kernel(const int* __restric
     if (tid < f) X[(size_t)row * f + tid] = S.xs[tid];
     __syncthreads();
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS) : "memory");
 }
 
 inline size_t smem_bytes(int f) {
   size_t o = std::max<size_t>((size_t)roff(f) * 4, (size_t)STAGES * 2 * TILE);
   o = (o + 127) & ~(size_t)127;
-  o += 64 + sizeof(double) * (3 * (size_t)f + NW * (size_t)f + KC) + sizeof(float) * ((size_t)((f + NB - 1) / NB) * NB * NBP + KC) + sizeof(int) * KC + sizeof(float) * NB;
+  o += sizeof(double) * (3 * (size_t)f + NW * (size_t)f + KC) + sizeof(float) * ((size_t)((f + NB - 1) / NB) * NB * NBP + KC) + sizeof(int) * KC + sizeof(float) * NB;
   return o + 64;
 }
 

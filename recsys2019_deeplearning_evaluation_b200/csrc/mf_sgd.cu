@@ -1,4 +1,4 @@
-// K2: matrix-factorisation SGD epochs (BPR-MF and FunkSVD), sm_100a.
+// K2: matrix-factorisation SGD epochs (BPR-MF and FunkSVD), sm_90a.
 //
 // Replaces MatrixFactorization/Cython/MatrixFactorization_Cython_Epoch.pyx:
 //   epochIteration_Cython_BPR_SGD :583-678, epochIteration_Cython_FUNK_SVD_SGD :289-390,

@@ -1,4 +1,4 @@
-// K6: batch scoring behind _compute_item_score / recommend, sm_100a.
+// K6: batch scoring behind _compute_item_score / recommend, sm_90a.
 //
 // Replaces
 //   Base/BaseSimilarityMatrixRecommender.py:73-92   item scores = URM[users] . W_sparse           (SpMM -> dense block)

@@ -2,12 +2,11 @@
 // namespace b200::sim).  Replaces Compute_Similarity_Cython.pyx:327-408 (gather / accumulate) and :467-568 (normalise,
 // top-K, emit) for every-stored-value-is-1 data, like the window kernel, with a different on-chip representation.
 //
-// What the measurements of the two earlier kernels say (profiles/r02_k1_variants_c5.txt, per C5 column):
-//   window kernel (16-bit counters, 2 windows of 200 KB)  75 K cycles: 30 K of them a latency-bound gather (CSC entry ->
-//     row bounds -> row, two dependent trips to memory with 64 row segments in flight per SM) and 45 K sweeping / selecting
-//     over 2 x 100 K cells;
-//   bitmap kernel K1-C (three thermometer bitmaps, TMA ring)  97 K cycles: shared-memory atomics that RETURN a value run at
-//     about one per cycle per SM (52 K cycles for the 50 K gathered entries of a column), and it ran a radix select per level.
+// What per-phase cycle counters of the two earlier kernels showed:
+//   window kernel (16-bit counters, 2 windows of 200 KB): a latency-bound gather (CSC entry -> row bounds -> row, two
+//     dependent trips to memory) and more time sweeping / selecting over 2 x 100 K cells;
+//   bitmap kernel K1-C (three thermometer bitmaps, TMA ring): shared-memory atomics that RETURN a value run at about one
+//     per cycle per SM, and it ran a radix select per level.
 // So: counters must be bumped with fire-and-forget atomics, the gather needs one dependent trip and many rows in flight,
 // and the per-column passes must touch few bytes.
 //
@@ -18,16 +17,15 @@
 // candidates computes that sum anyway; a column that fails the check is handed to the window kernel (redo list), as are the
 // columns the host routes there directly (dense co-occurrence).  Exactness is unchanged.
 //
-// What bounds it now (profiles/r02_k1d_*, C5: 26.1 ms per pass, 37.8 K SM cycles per column): the 50 K shared-memory atomics
-// of a column issue at ~11 cycles per warp instruction when both CTAs of an SM gather at once (45 K cycles for two columns),
-// and nothing overlaps them with the ~31 K cycles of sweep / select / emit that follow: the two CTAs fall into lockstep.
-// Measured and left out (same runs): a bank-spread accumulator (word = (j >> 8) << 5 | j & 31 with rows re-sorted by bank:
+// What bounds it: the ~50 K shared-memory atomics of a C5 column issue slowly when both CTAs of an SM gather at once, and
+// nothing overlaps them with the sweep / select / emit that follow: the two CTAs fall into lockstep.
+// Tried and left out: a bank-spread accumulator (word = (j >> 8) << 5 | j & 31 with rows re-sorted by bank:
 // average bank crowding 3.1 -> 2.0 in simulation) changed nothing, so bank conflicts are not the limit; L2 prefetches of the
 // next column's rows and pre-loaded row locations changed nothing either; a per-SM token that lets one CTA gather at a time
-// showed that ONE CTA's gather alone also takes 45 K cycles (latency-bound with 16 warps x 4 rows in flight), so anti-phase
-// buys nothing; replacing the returning atomics of the candidate collection by a two-pass sweep with prefix sums moved 9 K
-// cycles from the sweep into the second pass, and an atomic-free one-pass sweep (per-warp candidate regions, shuffle prefix
-// sums, two vectors in flight) left the sweep at 16 K cycles: its shared loads queue behind the OTHER CTA's atomics.  What would: more CTAs per SM in different phases (two neighbour windows of
+// showed that ONE CTA's gather alone takes as long (latency-bound with 16 warps x 4 rows in flight), so anti-phase
+// buys nothing; replacing the returning atomics of the candidate collection by a two-pass sweep with prefix sums only moved
+// time from the sweep into the second pass, and an atomic-free one-pass sweep (per-warp candidate regions, shuffle prefix
+// sums, two vectors in flight) did not shorten the sweep: its shared loads queue behind the OTHER CTA's atomics.  What would: more CTAs per SM in different phases (two neighbour windows of
 // 50 KB counters each: 3-4 CTAs) or two accumulators per CTA with warp-specialised gather / select.
 //
 // Gather.  The CSC side stores, per entry, where the user's padded row lives (csc_seg: start and length in 16-byte

@@ -1,4 +1,4 @@
-// K1: sparse column-column similarity with exact top-K selection, sm_100a.
+// K1: sparse column-column similarity with exact top-K selection, sm_90a.
 //
 // Replaces Base/Similarity/Cython/Compute_Similarity_Cython.pyx:327-408 (computeItemSimilarities, the
 // Gustavson row-gather into an n_columns accumulator) and :467-568 (normalise, top-K, emit).
@@ -1224,7 +1224,7 @@ struct b200_sim_s {
 
 namespace {
 
-constexpr int GRID1D = 148 * 8;
+constexpr int GRID1D = 132 * 8;  // grid-stride loops: 8 CTAs per SM of an H100
 
 typedef void (*sim_kernel_t)(const KParams);
 template <int F>

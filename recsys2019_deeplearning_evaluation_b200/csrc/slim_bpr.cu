@@ -1,4 +1,4 @@
-// K3: SLIM-BPR epochs on a dense (optionally symmetric) item-item matrix S, sm_100a.
+// K3: SLIM-BPR epochs on a dense (optionally symmetric) item-item matrix S, sm_90a.
 //
 // Replaces SLIM_BPR/Cython/SLIM_BPR_Cython_Epoch.pyx: epochIteration_Cython :211-335, sampleBPR_Cython :436-480,
 // adaptive_gradient :395-433 (per-ITEM scalar state shared by the positive and negative roles), symmetric storage

@@ -1,4 +1,4 @@
-// K7: SLIM ElasticNet -- one non-negative (optionally signed) elastic-net regression per item, on the Gram matrix, sm_100a.
+// K7: SLIM ElasticNet -- one non-negative (optionally signed) elastic-net regression per item, on the Gram matrix, sm_90a.
 //
 // Replaces the per-item loop of SLIM_ElasticNet/SLIMElasticNetRecommender.py:77-131, i.e. scikit-learn's
 // ElasticNet(precompute=True, fit_intercept=False, max_iter=100, tol=1e-4).fit(URM with column j zeroed, URM[:, j]) -- the

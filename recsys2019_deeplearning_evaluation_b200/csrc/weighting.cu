@@ -1,4 +1,4 @@
-// URM feature weighting in front of the KNN similarity (SURVEY.md 8(f).3), sm_100a.
+// URM feature weighting in front of the KNN similarity (SURVEY.md 8(f).3), sm_90a.
 //
 // Replaces Base/IR_feature_weighting.py:13-78 as KNN/ItemKNNCFRecommender.py:42-50 and KNN/UserKNNCFRecommender.py:43-51
 // apply it: okapi_BM_25(URM.T).T and TF_IDF(URM.T).T -- items are the "documents" (rows of URM.T), users the "terms".
@@ -85,7 +85,7 @@ int b200_feature_weighting_device(int mode, int n_users, int n_items, int64_t nn
     if (mode == B200_WEIGHT_BM25) {
       colsum.alloc((size_t)n_items);
       B200_CUDA(cudaMemsetAsync(colsum.get(), 0, sizeof(double) * (size_t)n_items, st));
-      weighting::colsum_kernel<<<148 * 8, 256, 0, st>>>(d_indices, d_data, nnz, colsum.get());
+      weighting::colsum_kernel<<<sm_count() * 8, 256, 0, st>>>(d_indices, d_data, nnz, colsum.get());
       weighting::total_kernel<<<1, 1024, 0, st>>>(colsum.get(), n_items, total.get());
       count_launch(2);
     }

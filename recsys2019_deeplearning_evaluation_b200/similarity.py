@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's similarity boundary, backed by libb200rec.so (sm_100a).
+"""Host-side mirror of the reference's similarity boundary, backed by libb200rec.so (sm_90a).
 
 `Compute_Similarity_Cython` keeps the constructor / `compute_similarity(start_col, end_col)` signature, argument
 meaning and error behaviour of Base/Similarity/Cython/Compute_Similarity_Cython.pyx:52-611 (reference paths are

@@ -9,10 +9,10 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with -m gpu)")
 
 
-# The driver runs `pytest tests -x -q -m gpu`: a failure hides everything collected after it.  The headline path goes
+# Under `pytest tests -x -q -m gpu` a failure hides everything collected after it.  The headline path goes
 # first (similarity kernel and its reference goldens, then the SGD trainers), the remaining files keep their
 # alphabetical order behind them.
 _ORDER = ["test_similarity_gpu", "test_golden_gpu", "test_scale_parity_gpu", "test_mf_gpu", "test_slim_gpu",

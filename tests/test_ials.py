@@ -82,7 +82,7 @@ def test_cuda_factor_sizes_against_restatement(f):
 @pytest.mark.gpu
 @pytest.mark.parametrize("f", [8, 64, 100, 128, 160, 256])
 def test_tensor_core_kernel_every_size_against_restatement(f, monkeypatch):
-    """ials_v2.cuh (tcgen05 3xTF32 Gram, blocked fp32 Cholesky, fp64 refinement) forced on for every factor count it serves
+    """ials_v2.cuh (wgmma 3xTF32 Gram, blocked fp32 Cholesky, fp64 refinement) forced on for every factor count it serves
     (by default it takes over above 128 factors), on a shape with enough rows on the other side to be eligible
     (n_other >= 4 f), ratings as confidences (c - 1 varies per entry: the sqrt(c - 1) operand scaling)."""
     from threadpoolctl import threadpool_limits

@@ -20,5 +20,5 @@ for src in sorted(glob.glob(os.path.join(B.CSRC, "*.cu"))):
         obj = os.path.join(B.OBJ, base + ".o")
     objs.append(obj)
 lib = os.path.join(out_dir, "libb200rec_%s.so" % name)
-subprocess.check_call([B._nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", lib] + objs)
+subprocess.check_call([B._nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", lib] + objs)
 print(lib)

@@ -1,4 +1,4 @@
-"""Text summary of one kernel of an ncu report (headline raw metrics + hottest source lines) for profiles/.
+"""Text summary of one kernel of an ncu report (headline raw metrics + hottest source lines).
 usage: python tools/ncu_summary.py <report.ncu-rep> <lib.so> <kernel-substring> <title> [mangled-substring]
 The optional mangled substring (e.g. ILi0ELb1ELb1E for sim_topk_kernel<0, true, true>) picks ONE template instantiation for
 the SASS-offset -> source-line mapping; without it the first instantiation in the cubin is used, which is wrong for the others."""
