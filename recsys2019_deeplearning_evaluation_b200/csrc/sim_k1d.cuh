@@ -157,13 +157,14 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
   for (int i = tid; i < ntile; i += D_THREADS) tcnt[i] = 0;
   long long prof_t = p.prof ? clock64() : 0;
   const int K = p.K;
+  const int n_items = p.n_range_dev ? *p.n_range_dev : p.n_range;
 
   for (;;) {
     __syncthreads();
     if (tid == 0) { ds.item = atomicAdd(p.counter, 1); ds.nbuf = 0; ds.adds = 0; ds.nibsum = 0; ds.ncand = 0; }
     __syncthreads();
     const int item = ds.item;
-    if (item >= p.n_range) break;
+    if (item >= n_items) break;
     const int4 wi = __ldg(p.worklist + item);
     const int col = wi.x, lc = wi.y, cs = wi.z, ce = wi.w;
     const size_t out_base = (size_t)lc * K;
@@ -406,6 +407,260 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Pair path: every co-occurrence count C[i][j] = C[j][i] is gathered once.
+//
+// The kernel above builds C[i][j] in pass i and again in pass j: it streams the whole row of every user of column i.  On a
+// call that covers every column, the upper pass streams only the part of each row after i (rows are sorted by the new
+// index), so pass i counts the neighbours j > i: half the gathered entries and half the shared atomics.  It appends every
+// cell with count >= 3 to a global list of (i, j, count) pairs; the exchange scatters each pair into the candidate lists of
+// both i and j, and the select kernel applies the rule of the kernel above to those lists: with at least K positive keys
+// and no count-2 / count-1 cell that can reach the floor sim(3, largest norm term) (bounded by the smallest norm term of
+// the columns with at least 2 / 1 users), the K best count >= 3 cells are the answer -- the same keys from the same counts
+// and norm terms, so the output is the same.  Every other column (fewer
+// than K candidates, count-2 / count-1 cells that matter, a list longer than the key registers) is appended to a device
+// redo list that the kernel above then computes in full.  A counter overflow in the upper pass (the nibble checksum over
+// the suffix increments) or a full pair list sets a flag on the device, and the select kernel then hands EVERY column to
+// the kernel above: exactness never depends on the pair path.  Whether a handle takes the path at all is decided at create
+// time from the norm terms and the column lengths (k1d_pair_gate in sim_topk.cu): a column handed back costs a full pass
+// on top of the upper pass, so the path only pays when the select kernel can decide nearly every column.
+
+constexpr int U_STAGE = 2048;  // count >= 3 cells of one column staged in shared memory before one global reservation
+constexpr int U_STEPS = 1;     // loads of 32 chunks in flight per warp (more spill at 64 registers)
+
+struct K1DUpShared {
+  int item, adds, nibsum, ncand, nst;
+  unsigned long long base;
+};
+
+__global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KParams p) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ K1DUpShared us;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int W = p.bm_words;
+  const int Wr = (p.n_cols + 7) >> 3;
+  unsigned* acc = reinterpret_cast<unsigned*>(smem_raw);
+  unsigned* stage = acc + W;
+  for (int i = tid; i < W; i += D_THREADS) acc[i] = 0u;
+  if (blockIdx.x == 0 && tid == 0 && p.fail_every > 0) atomicExch(p.pair_fail, 1);  // test hook: exercises the fallback
+  long long prof_t = p.prof ? clock64() : 0;
+
+  for (;;) {
+    __syncthreads();
+    if (tid == 0) {
+      // once the call has fallen back, the remaining columns are not worth gathering
+      us.item = *(volatile int*)p.pair_fail ? p.n_range : atomicAdd(p.counter, 1);
+      us.adds = 0; us.nibsum = 0; us.ncand = 0; us.nst = 0;
+    }
+    __syncthreads();
+    const int item = us.item;
+    if (item >= p.n_range) break;
+    const int4 wi = __ldg(p.worklist_up + item);
+    const int col = wi.x, cs = wi.z, ce = wi.w;
+
+    // ---------------- gather over the row suffixes: chunks that start at or before `col` are masked by j > col.  A suffix
+    // is half a row on average (C5: ~13 chunks), so one row per warp load would leave most lanes idle and issue as many
+    // loads and atomic instructions as the whole row; instead the 32 suffixes of a batch are one stream of chunks, every
+    // lane of every load busy.  Rows with chunks sit compacted in the low lanes; lane r holds row r's [beg, end) in the
+    // stream, and the row of stream position f is the number of rows that end at or before f.
+    int expect = 0;
+    for (int k0 = cs + warp * 32; k0 < ce; k0 += D_WARPS * 32) {
+      const int nrows = min(32, ce - k0);
+      int2 seg = make_int2(0, 0);
+      if (lane < nrows) seg = __ldg(p.csc_suf + k0 + lane);
+      expect += 4 * (seg.y >> 3) - (seg.y & 7);
+      const unsigned nz = __ballot_sync(0xffffffffu, (seg.y >> 3) > 0);
+      const int nr = __popc(nz);
+      const int src = lane < nr ? (int)__fns(nz, 0, lane + 1) : 0;
+      const int rstart = __shfl_sync(0xffffffffu, seg.x, src);
+      const int sy = __shfl_sync(0xffffffffu, seg.y, src);
+      const int rn = lane < nr ? (sy >> 3) : 0;
+      int end = rn;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, end, off);
+        if (lane >= off) end += t;
+      }
+      const int beg = end - rn;
+      const int total = __shfl_sync(0xffffffffu, end, 31);
+      for (int b0 = 0; b0 < total; b0 += 32 * U_STEPS) {
+        int4 v[U_STEPS];
+#pragma unroll
+        for (int q = 0; q < U_STEPS; ++q) {
+          const int base = b0 + 32 * q, f = base + lane;
+          const unsigned before = __ballot_sync(0xffffffffu, lane < nr && end <= base);
+          const unsigned ends = __reduce_or_sync(0xffffffffu, (lane < nr && end > base && end - base < 32) ? (1u << (end - base)) : 0u);
+          const int row = (__popc(before) + __popc(ends & ((2u << lane) - 1u))) & 31;
+          const int rb = __shfl_sync(0xffffffffu, beg, row), rs = __shfl_sync(0xffffffffu, rstart, row);
+          if (f < total) v[q] = __ldg(reinterpret_cast<const int4*>(p.csr_idx1) + (size_t)rs + (f - rb));
+        }
+#pragma unroll
+        for (int q = 0; q < U_STEPS; ++q) {
+          if (b0 + 32 * q + lane < total) {
+            const int jj[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              const int j = jj[c];
+              if (j < p.n_cols && j > col) atomicAdd(&acc[j >> 3], 1u << ((j & 7) << 2));
+            }
+          }
+        }
+      }
+    }
+    expect = __reduce_add_sync(0xffffffffu, expect);
+    if (lane == 0 && expect) atomicAdd(&us.adds, expect);
+    __syncthreads();
+    PROF_MARK(8);
+
+    // ---------------- sweep of the words that hold j > col: checksum, count >= 3 cells into the stage, clear
+    {
+      int ns = 0;
+      uint4* acc4 = reinterpret_cast<uint4*>(acc);
+      for (int i4 = (((col + 1) >> 3) >> 2) + tid; i4 < ((Wr + 3) >> 2); i4 += D_THREADS) {
+        const uint4 w4 = acc4[i4];
+        if (!(w4.x | w4.y | w4.z | w4.w)) continue;
+        acc4[i4] = make_uint4(0u, 0u, 0u, 0u);
+        const unsigned ww[4] = {w4.x, w4.y, w4.z, w4.w};
+        unsigned bytes = 0u, any = 0u, m[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          bytes += (ww[e] & 0x0F0F0F0Fu) + ((ww[e] >> 4) & 0x0F0F0F0Fu);
+          m[e] = nib_ge3(ww[e]);
+          any |= m[e];
+        }
+        ns += (int)__dp4a(bytes, 0x01010101u, 0u);
+        if (any) {
+          const int c3 = __popc(m[0]) + __popc(m[1]) + __popc(m[2]) + __popc(m[3]);
+          int pos = atomicAdd(&us.ncand, c3);
+          // the staged cells form a prefix [0, nst) of the positions; a vector past the stage reserves its own slots
+          const bool staged = pos + c3 <= U_STAGE;
+          unsigned long long g = 0ull;
+          if (staged) atomicAdd(&us.nst, c3);
+          else g = atomicAdd(p.n_pairs, (unsigned long long)c3);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            unsigned mm = m[e];
+            while (mm) {
+              const int q = (__ffs(mm) - 1) >> 2;
+              mm &= mm - 1;
+              const unsigned cd = ((unsigned)((i4 * 4 + e) * 8 + q) << 4) | ((ww[e] >> (q << 2)) & 15u);
+              if (staged) {
+                stage[pos++] = cd;
+              } else {
+                if (g < (unsigned long long)p.pair_cap) p.pairs[g] = ((u64)col << 32) | cd;
+                else atomicExch(p.pair_fail, 1);
+                ++g;
+              }
+            }
+          }
+        }
+      }
+      ns = __reduce_add_sync(0xffffffffu, ns);
+      if (lane == 0 && ns) atomicAdd(&us.nibsum, ns);
+    }
+    __syncthreads();
+    const int nst = us.nst;
+    if (tid == 0) {
+      if (us.nibsum != us.adds) atomicExch(p.pair_fail, 1);  // a counter overflowed: the call falls back
+      us.base = nst ? atomicAdd(p.n_pairs, (unsigned long long)nst) : 0ull;
+      if (us.base + nst > (unsigned long long)p.pair_cap) atomicExch(p.pair_fail, 1);
+    }
+    __syncthreads();
+    const unsigned long long base = us.base;
+    if (base + nst <= (unsigned long long)p.pair_cap)
+      for (int t = tid; t < nst; t += D_THREADS) p.pairs[base + t] = ((u64)col << 32) | stage[t];
+    PROF_MARK(9);
+  }
+}
+
+// Exchange, step 1: candidates per column (both ends of every pair).  Skipped when the call has fallen back.
+__global__ void k1d_pair_degree_kernel(const KParams p, int* deg) {
+  if (*p.pair_fail) return;
+  const long long n = (long long)min(*p.n_pairs, (u64)p.pair_cap);
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const u64 pr = p.pairs[q];
+    atomicAdd(deg + (int)(pr >> 32), 1);
+    atomicAdd(deg + (int)(((unsigned)pr) >> 4), 1);
+  }
+}
+
+// Exchange, step 2 (after the exclusive scan of deg into cand_off): every pair into the lists of both ends as
+// (neighbour << 4 | count).  Counting deg back down leaves it zero for the next call.
+__global__ void k1d_pair_scatter_kernel(const KParams p, int* deg) {
+  if (*p.pair_fail) return;
+  const long long n = (long long)min(*p.n_pairs, (u64)p.pair_cap);
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const u64 pr = p.pairs[q];
+    const unsigned i = (unsigned)(pr >> 32), lo = (unsigned)pr, j = lo >> 4, c = lo & 15u;
+    p.cand[p.cand_off[i] + atomicSub(deg + i, 1) - 1] = lo;
+    p.cand[p.cand_off[j] + atomicSub(deg + j, 1) - 1] = (i << 4) | c;
+  }
+}
+
+// One CTA per column of the work list: keys from the candidate list, the decision rule of sim_k1d_kernel's collected path,
+// the K best, emit -- or the column goes to the redo list (all columns when the call has fallen back).
+template <int F>
+__global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_select_kernel(const KParams p) {
+  __shared__ u64 buf[4 * D_THREADS];
+  __shared__ K1DShared ds;
+  const int tid = threadIdx.x;
+  const int item = blockIdx.x;
+  const int4 wi = __ldg(p.worklist + item);
+  if (*(volatile int*)p.pair_fail) {
+    if (tid == 0) { p.wl_redo[item] = wi; atomicAdd(p.n_redo, 1); }  // every column, in the work list's order
+    return;
+  }
+  long long prof_t = p.prof ? clock64() : 0;
+  const int col = wi.x, lc = wi.y, K = p.K;
+  const int s = p.cand_off[col], n = p.cand_off[col + 1] - s;
+  bool ok = n <= 4 * D_THREADS;
+  int n_have = 0;
+  if (ok) {
+    if (tid == 0) ds.nbuf = 0;
+    const float Ai = p.A[col];
+    u64 keys[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int t = q * D_THREADS + tid;
+      keys[q] = 0ull;
+      if (t < n) {
+        const unsigned cd = p.cand[s + t];
+        const int2 bn = __ldg(p.BN + (cd >> 4));
+        const float sv = sim_value<F>(p, (float)(cd & 15u), Ai, __int_as_float(bn.x));
+        if (sv > 0.f) keys[q] = (((u64)__float_as_uint(sv)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)bn.y);
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      if (keys[q]) buf[atomicAdd(&ds.nbuf, 1)] = keys[q];
+    __syncthreads();
+    n_have = ds.nbuf;
+    ok = false;
+    if (n_have >= K) {
+      // floor of the K-th best: (count 3, largest norm term); no count-2 / count-1 cell may reach it.  A count-c cell's
+      // neighbour has at least c users, so its norm term is at least lvl_b<c> (an empty column's 0 does not count)
+      const float fl = sim_value<F>(p, 3.f, Ai, p.tbnd[p.ntile]) * (1.f - 1e-6f);
+      if (fl > 0.f) ok = !(sim_value<F>(p, 2.f, Ai, p.lvl_b2) >= fl) && !(sim_value<F>(p, 1.f, Ai, p.lvl_b1) >= fl);
+    }
+  }
+  PROF_MARK(10);
+  if (!ok) {
+    if (tid == 0) p.wl_redo[atomicAdd(p.n_redo, 1)] = wi;
+    return;
+  }
+  int kept;
+  d_select(buf, n_have, K, &ds, &kept);
+  const size_t out_base = (size_t)lc * K;
+  for (int t = tid; t < kept; t += D_THREADS) {
+    const u64 k64 = buf[t];
+    emit_entry(p, out_base + t, (int)(0xFFFFFFFFu - (unsigned)k64), __uint_as_float((unsigned)(k64 >> 32)));
+  }
+  for (int t = kept + tid; t < K; t += D_THREADS) emit_entry(p, out_base + t, -1, 0.f);
+  if (tid == 0) emit_count(p, lc, kept);
+  PROF_MARK(11);
+}
+
 // tb[t] = norm term at neighbour min(t << D_TILE_LOG2, n_cols - 1), t = 0 .. ntile
 __global__ void k1d_tile_bounds_kernel(const int2* __restrict__ BN, int n_cols, int ntile, float* tb) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -423,4 +678,38 @@ __global__ void k1d_csc_seg_kernel(const int* __restrict__ csc_idx, const int* _
     const int len = csr_ptr[u + 1] - csr_ptr[u];
     seg[q] = make_int2(s >> 2, (((e - s) >> 2) << 2) | ((e - s) - len));
   }
+}
+
+// csc_suf[q] = the suffix of CSC entry q's padded row after the entry's column c, for the upper pass (csc_pos[q] = the
+// entry's position in the CSR, so its place in the user's row is csc_pos[q] - csr_ptr[u]).  x = start in 16-byte chunks of the chunk that holds the next
+// position, y = chunks << 3 | entries of those chunks that produce no increment (the ones at or before c, and the padding;
+// 0..6).  suf_work[c] = the increments of all of column c's suffixes, the work of its upper pass (sort key of the upper
+// pass's longest-first order, with iota[c] = c as the value).  One warp per column.
+__global__ void k1d_csc_suffix_kernel(const int* __restrict__ csc_ptr, const int* __restrict__ csc_idx, const int* __restrict__ csr_ptr,
+                                      const int* __restrict__ csc_pos, const int* __restrict__ split1, int n_cols, int2* suf,
+                                      unsigned long long* suf_work, int* iota) {
+  const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (c >= n_cols) return;
+  unsigned long long w = 0;
+  for (int q = csc_ptr[c] + lane; q < csc_ptr[c + 1]; q += 32) {
+    const int u = csc_idx[q];
+    const int r0 = csr_ptr[u], len = csr_ptr[u + 1] - r0;
+    const int next = csc_pos[q] - r0 + 1;
+    const int s = split1[2 * (size_t)u], e = split1[2 * (size_t)u + 1];
+    const int nch = ((e - s) >> 2) - (next >> 2);
+    suf[q] = make_int2((s >> 2) + (next >> 2), nch > 0 ? (nch << 3) | ((next & 3) + (e - s) - len) : 0);
+    w += (unsigned long long)(len - next);
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
+  if (lane == 0) { suf_work[c] = w; iota[c] = c; }
+}
+
+// the upper pass's work list: every column (new numbering, in the order `perm`) as (new column, original column, csc range)
+__global__ void k1d_upper_worklist_kernel(const int* __restrict__ perm, const int2* __restrict__ BN, const int* __restrict__ csc_ptr,
+                                          int n_cols, int4* wl) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_cols) return;
+  const int c = perm[k];
+  wl[k] = make_int4(c, BN[c].y, csc_ptr[c], csc_ptr[c + 1]);
 }

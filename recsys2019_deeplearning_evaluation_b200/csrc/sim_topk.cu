@@ -29,7 +29,9 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
+#include <cstring>
 #include <vector>
 
 #include "common.cuh"
@@ -115,8 +117,22 @@ struct KParams {
   const int4* __restrict__ worklist;
   int* redo;
   int* fail;
-  const int* n_range_dev;  // window kernel: the number of columns to process is read from here when set
-  unsigned long long* prof;  // optional [8] per-phase cycle counters (thread 0 of every CTA), test/bench hook
+  const int* n_range_dev;  // window kernel / K1-D kernel: the number of columns to process is read from here when set
+  // K1-D pair path (sim_k1d.cuh): per CSC entry the suffix of the user's padded row after the column, the work items in
+  // suffix-work order, the list of (i, j, count >= 3) pairs with j > i and its capacity, the candidate lists built from it,
+  // the flag that sends the whole call down the K1-D kernel, and the columns that the select kernel hands to the K1-D kernel
+  const int2* __restrict__ csc_suf;
+  const int4* __restrict__ worklist_up;
+  u64* pairs;
+  u64* n_pairs;
+  long long pair_cap;
+  const int* __restrict__ cand_off;
+  unsigned* cand;
+  int* pair_fail;
+  int4* wl_redo;
+  int* n_redo;
+  float lvl_b1, lvl_b2;  // smallest norm term of the columns with >= 1 / >= 2 users (the neighbours a count-1 / -2 cell can have)
+  unsigned long long* prof;  // optional [16] per-phase cycle counters (thread 0 of every CTA), test/bench hook
 };
 
 __device__ __forceinline__ void emit_entry(const KParams& p, size_t pos, int idx, float val) {
@@ -129,7 +145,7 @@ __device__ __forceinline__ void emit_count(const KParams& p, int row, int n) {
 }
 
 template <int F>
-__device__ __forceinline__ float sim_value(const KParams& p, float d, float a, float b) {
+__host__ __device__ __forceinline__ float sim_value(const KParams& p, float d, float a, float b) {
   if (F == F_PROD) return d / (a * b + p.se);
   if (F == F_NONORM) return d / p.shrink_div;
   if (F == F_JACCARD) return d / (a + b - d + p.se);
@@ -1213,9 +1229,26 @@ struct b200_sim_s {
   std::vector<int> h_old2new, h_csc_ptr;
   int n_sparse_last = 0, n_dense_last = 0;
   std::vector<unsigned long long> h_work;  // by ORIGINAL column index
+  // K1-D pair path (sim_k1d.cuh): row suffixes, the upper pass's work list (every column), pair list (capacity from the
+  // expected pair count), candidate lists (deg: per-column counts, zero between calls), control words (pair count,
+  // fallback flag, redo count), redo list, scan scratch (all allocated by the first call that takes the path), the select
+  // kernel's level bounds, upper-pass geometry
+  DevBuf<int2> csc_suf;
+  DevBuf<int4> worklist_up, wl_redo;
+  DevBuf<u64> pairs;
+  long long pair_cap = 0;
+  double pairs_expected = 0.0;
+  float lvl_b1 = 0.f, lvl_b2 = 0.f;
+  DevBuf<unsigned> cand;
+  DevBuf<int> deg, cand_off, pair_ctl;
+  DevBuf<unsigned char> scan_tmp;
+  size_t scan_tmp_bytes = 0, smem_up_bytes = 0;
+  int ctas_up = 0;
+  bool pair_path_last = false;  // the cached routing qualifies for the pair path
   DevBuf<int> counter, order;
   std::vector<int> h_order;  // cached LPT order for [order_lo, order_hi)
   int order_lo = -1, order_hi = -1;
+  bool order_k1c = false;
   DevBuf<unsigned long long> prof;
   bool prof_on = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -1255,10 +1288,82 @@ sim_kernel_t k1d_kernel_for(int formula) {
   }
 }
 
+sim_kernel_t k1d_select_kernel_for(int formula) {
+  switch (formula) {
+    case F_PROD: return sim_k1d_select_kernel<F_PROD>;
+    case F_NONORM: return sim_k1d_select_kernel<F_NONORM>;
+    case F_JACCARD: return sim_k1d_select_kernel<F_JACCARD>;
+    case F_DICE: return sim_k1d_select_kernel<F_DICE>;
+    default: return sim_k1d_select_kernel<F_TVERSKY>;
+  }
+}
+
 int bits_for(long long n) {
   int b = 1;
   while ((1ll << b) < n) ++b;
   return b;
+}
+
+// Whether the K1-D pair path pays on this data.  It saves about half of a K1-D pass when the select kernel decides a column
+// itself, and costs a full K1-D pass more for every column it hands back, so it is taken only when at least 90 % of the
+// non-empty columns are expected to pass the select kernel's rule: with users drawn independently, column c has
+// n_cols * P(Poisson(lambda_c) >= 3) cells with count >= 3 (lambda_c = gathered entries off the diagonal / n_cols), which
+// must reach K, and
+// no count-2 / count-1 cell may reach the floor sim(3, largest norm term).  Sets the smallest norm terms of the neighbours
+// a count-1 / count-2 cell can have, and the expected number of pairs (which sizes the pair list).
+template <int F>
+bool k1d_pair_gate_f(b200_sim_s* h, const KParams& p, const std::vector<int>& cnt, const std::vector<int2>& bn, const std::vector<float>& a) {
+  const int n = h->n_cols;
+  auto bval = [&](int j) { float b; std::memcpy(&b, &bn[(size_t)j].x, sizeof b); return b; };
+  float b1 = FLT_MAX, b2 = FLT_MAX;
+  for (int j = 0; j < n; ++j) {
+    if (cnt[(size_t)j] >= 1) b1 = std::min(b1, bval(j));
+    if (cnt[(size_t)j] >= 2) b2 = std::min(b2, bval(j));
+  }
+  h->lvl_b1 = b1;
+  h->lvl_b2 = b2;
+  const float bmax = bval(n - 1);
+  long long nonempty = 0, pass = 0;
+  double cells = 0.0;
+  for (int c = 0; c < n; ++c) {
+    if (cnt[(size_t)c] == 0) continue;
+    ++nonempty;
+    const double lam = (double)(h->h_work[(size_t)bn[(size_t)c].y] - (unsigned long long)cnt[(size_t)c]) / (double)n;
+    const double est = (double)n * std::max(0.0, 1.0 - std::exp(-lam) * (1.0 + lam + 0.5 * lam * lam));
+    cells += est;
+    const float ai = a[(size_t)c];
+    const float fl = sim_value<F>(p, 3.f, ai, bmax) * (1.f - 1e-6f);
+    if (est >= (double)h->K && fl > 0.f && !(sim_value<F>(p, 2.f, ai, b2) >= fl) && !(sim_value<F>(p, 1.f, ai, b1) >= fl)) ++pass;
+  }
+  h->pairs_expected = 0.5 * cells;
+  return nonempty > 0 && (double)pass >= 0.9 * (double)nonempty;
+}
+
+// the formula constants of KParams
+void set_formula_params(KParams& p, const b200_sim_s* h) {
+  p.se = h->shrink + 1e-6f;
+  p.shrink_div = h->shrink != 0.f ? h->shrink : 1.f;
+  p.ta = h->ta; p.tb = h->tb;
+}
+
+bool k1d_pair_gate(b200_sim_s* h, const int* d_cnt, cudaStream_t st) {
+  const int n = h->n_cols;
+  std::vector<int> cnt((size_t)n);
+  std::vector<int2> bn((size_t)n);
+  std::vector<float> a((size_t)n);
+  B200_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaMemcpyAsync(bn.data(), h->BN.get(), sizeof(int2) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaMemcpyAsync(a.data(), h->A.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaStreamSynchronize(st));
+  KParams p{};
+  set_formula_params(p, h);
+  switch (h->formula) {
+    case F_PROD: return k1d_pair_gate_f<F_PROD>(h, p, cnt, bn, a);
+    case F_NONORM: return k1d_pair_gate_f<F_NONORM>(h, p, cnt, bn, a);
+    case F_JACCARD: return k1d_pair_gate_f<F_JACCARD>(h, p, cnt, bn, a);
+    case F_DICE: return k1d_pair_gate_f<F_DICE>(h, p, cnt, bn, a);
+    default: return k1d_pair_gate_f<F_TVERSKY>(h, p, cnt, bn, a);
+  }
 }
 
 void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, const float* h_data,
@@ -1373,6 +1478,7 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     count_launch(2);
     B200_CUDA(cudaStreamSynchronize(st));
   }
+  DevBuf<int> csc_pos;  // binary path: CSR position of every CSC entry (its place in the user's sorted row), for K1-D
   if (nnz) {
     DevBuf<int> rowid(nnz1), iota(nnz1), keys_out(nnz1), perm(nnz1);
     rowid_iota_kernel<<<div_up((long long)n_rows * 32, 256), 256, 0, st>>>(h->csr_ptr.get(), n_rows, rowid.get(), iota.get()); count_launch();
@@ -1385,6 +1491,7 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     if (h->binary) {
       h->csc_idx.alloc((size_t)nnz);
       build_csc_kernel<<<GRID1D, 256, 0, st>>>(perm.get(), rowid.get(), data_sorted.get(), nullptr, nnz, nullptr, h->csc_idx.get());
+      csc_pos = std::move(perm);
     } else {
       h->csc_ent.alloc((size_t)nnz);
       h->csr_ent.alloc((size_t)nnz + 8);
@@ -1467,6 +1574,8 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     const long long total = (long long)n_rows * (n_win + 1);
     split_kernel<<<div_up(total, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), n_rows, n_win, win, h->split.get()); count_launch();
   }
+  DevBuf<unsigned long long> suf_work;  // K1-D upper-pass work per new column, and the new column indices
+  DevBuf<int> suf_iota;
   if (h->binary) {  // padded, 16-byte aligned (row, window) segments
     const long long n_seg = (long long)n_rows * n_win;
     B200_REQUIRE((long long)nnz + 3 * n_seg < (1ll << 31), "matrix too large for 32-bit positions in the padded row layout");
@@ -1507,11 +1616,18 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       h->csc_seg.alloc((size_t)nnz + 2);
       B200_CUDA(cudaMemsetAsync(h->csc_seg.get() + nnz, 0, 2 * sizeof(int2), st));
       k1d_csc_seg_kernel<<<GRID1D, 256, 0, st>>>(h->csc_idx.get(), split1.get(), h->csr_ptr.get(), nnz, h->csc_seg.get()); count_launch();
+      h->csc_suf.alloc((size_t)nnz);
+      suf_work.alloc((size_t)n_cols);
+      suf_iota.alloc((size_t)n_cols);
+      k1d_csc_suffix_kernel<<<div_up((long long)n_cols * 32, 256), 256, 0, st>>>(h->csc_ptr.get(), h->csc_idx.get(), h->csr_ptr.get(),
+                                                                                 csc_pos.get(), split1.get(), n_cols, h->csc_suf.get(),
+                                                                                 suf_work.get(), suf_iota.get()); count_launch();
       B200_CUDA(cudaStreamSynchronize(st));
     }
     h->csr_idx = std::move(idx_pad);
     h->split = std::move(split_pad);
   }
+  csc_pos.release();
   // ---- per-column work (for LPT ordering and the bytes model), reported by ORIGINAL column index
   {
     DevBuf<unsigned long long> work((size_t)n_cols);
@@ -1568,9 +1684,37 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       // the whole unified L1 / shared array as shared memory: without it the driver sizes the carve-out for ONE block and the
       // second CTA of an SM never becomes resident
       B200_CUDA(cudaFuncSetAttribute(k1d_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+
+      // pair path: the upper pass needs the counters and the stage (two CTAs per SM when both fit, like the K1-D kernel), and
+      // it only pays when the select kernel can decide most columns itself (k1d_pair_gate); its buffers are allocated by the
+      // first call that takes it
+      cudaFuncAttributes fu{};
+      B200_CUDA(cudaFuncGetAttributes(&fu, sim_k1d_upper_kernel));
+      h->smem_up_bytes = ((size_t)h->bm_words + U_STAGE) * 4;
+      h->ctas_up = 0;
+      for (int ctas = 2; ctas >= 1 && h->ctas_up == 0; --ctas)
+        if ((long long)h->smem_up_bytes <= std::min<long long>((long long)sm_total / ctas - 1024, (long long)max_smem) - (long long)fu.sharedSizeBytes)
+          h->ctas_up = ctas;
+      if (h->ctas_up > 0 && !k1d_pair_gate(h, cnt_new.get(), st)) h->ctas_up = 0;
+      if (h->ctas_up > 0) {
+        B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_up_bytes));
+        B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        h->worklist_up.alloc((size_t)n_cols);
+        // the upper pass's longest-first order: every column by descending suffix work (empty columns do nothing there)
+        DevBuf<unsigned long long> keys_out((size_t)n_cols);
+        DevBuf<int> perm((size_t)n_cols);
+        size_t tb = 0;
+        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, suf_work.get(), keys_out.get(), suf_iota.get(), perm.get(), n_cols, 0, 64, st));
+        DevBuf<unsigned char> tmp(tb + 16);
+        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tb, suf_work.get(), keys_out.get(), suf_iota.get(), perm.get(), n_cols, 0, 64, st));
+        k1d_upper_worklist_kernel<<<div_up(n_cols, 256), 256, 0, st>>>(perm.get(), h->BN.get(), h->csc_ptr.get(), n_cols, h->worklist_up.get());
+        count_launch(5);
+        B200_CUDA(cudaStreamSynchronize(st));
+      }
     }
   }
   if (!h->k1c) { h->csr_idx1.release(); h->csc_seg.release(); }
+  if (h->ctas_up == 0) h->csc_suf.release();
 }
 
 }  // namespace
@@ -1697,14 +1841,18 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   // Routing + longest-processing-time-first order of the local columns (cached per range).  With K1-D the columns whose
   // expected hits per neighbour (gathered entries / n_cols) stay below k1c_lambda go to the nibble-counter kernel (`worklist`);
   // the rest -- and whatever that kernel hands back -- go to the window kernel (`order`).
-  if (h->order_lo != start_col || h->order_hi != end_col) {
+  if (h->order_lo != start_col || h->order_hi != end_col || h->order_k1c != use_k1c) {
     const unsigned long long* w = h->h_work.data() + start_col;
     std::vector<int> sparse;
     h->h_order.clear();
+    int n_nonempty_dense = 0;
     for (int i = 0; i < n_range; ++i) {
       const bool sp = use_k1c && w[i] > 0 && (double)w[i] <= h->k1c_lambda * (double)h->n_cols;
       (sp ? sparse : h->h_order).push_back(i);
+      if (!sp && w[i] > 0) ++n_nonempty_dense;
     }
+    // the pair path needs every pair's pass in this call: the whole column range, every non-empty column on K1-D
+    h->pair_path_last = h->ctas_up > 0 && use_k1c && start_col == 0 && end_col == h->n_cols && n_nonempty_dense == 0 && !sparse.empty();
     auto by_work = [w](int a, int b) { return w[a] > w[b]; };
     std::stable_sort(h->h_order.begin(), h->h_order.end(), by_work);
     std::stable_sort(sparse.begin(), sparse.end(), by_work);
@@ -1721,7 +1869,9 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     B200_CUDA(cudaStreamSynchronize(st));
     h->order_lo = start_col;
     h->order_hi = end_col;
+    h->order_k1c = use_k1c;
   }
+  const bool pair_path = h->pair_path_last && n_peers == 0;
   const int n_sparse = use_k1c ? h->n_sparse_last : 0, n_dense = use_k1c ? h->n_dense_last : n_range;
   B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
   KParams p;
@@ -1729,9 +1879,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.acc_cells = h->acc_words;
   p.lpu_log2 = h->lpu_log2;
   p.tileB = h->tileB.get();
-  p.se = h->shrink + 1e-6f;
-  p.shrink_div = h->shrink != 0.f ? h->shrink : 1.f;
-  p.ta = h->ta; p.tb = h->tb;
+  set_formula_params(p, h);
   p.csr_ptr = h->csr_ptr.get(); p.csr_ent = h->csr_ent.get(); p.csr_idx = h->csr_idx.get();
   p.split = h->split.get();
   p.csc_ptr = h->csc_ptr.get(); p.csc_ent = h->csc_ent.get(); p.csc_idx = h->csc_idx.get();
@@ -1752,8 +1900,54 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.csr_idx1 = h->csr_idx1.get(); p.csc_seg = h->csc_seg.get(); p.worklist = h->worklist.get();
   p.redo = h->order.get(); p.fail = h->fail.get();
   p.n_range_dev = nullptr;
+  p.csc_suf = h->csc_suf.get(); p.worklist_up = h->worklist_up.get();
+  if (pair_path && h->pairs.n == 0) {
+    // first call on the pair path: the pair list holds twice the expected pairs (a fuller list sets the fallback flag), the
+    // candidate lists twice that; candidate positions stay below 2^31
+    h->pair_cap = std::min<long long>((long long)(2.0 * h->pairs_expected) + (1 << 16), (1ll << 30) - 1);
+    h->pairs.alloc((size_t)h->pair_cap);
+    h->cand.alloc(2 * (size_t)h->pair_cap);
+    h->deg.alloc((size_t)h->n_cols + 1);
+    h->cand_off.alloc((size_t)h->n_cols + 1);
+    h->pair_ctl.alloc(4);  // [0..1] pair count (64-bit), [2] fallback flag, [3] redo count
+    h->wl_redo.alloc((size_t)h->n_cols);
+    B200_CUDA(cudaMemsetAsync(h->deg.get(), 0, sizeof(int) * ((size_t)h->n_cols + 1), st));
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, h->scan_tmp_bytes, h->deg.get(), h->cand_off.get(), h->n_cols + 1, st));
+    h->scan_tmp.alloc(h->scan_tmp_bytes + 16);
+  }
+  p.pairs = h->pairs.get(); p.pair_cap = h->pair_cap;
+  p.n_pairs = reinterpret_cast<u64*>(h->pair_ctl.get());
+  p.pair_fail = h->pair_ctl.get() + 2; p.n_redo = h->pair_ctl.get() + 3;
+  p.cand_off = h->cand_off.get(); p.cand = h->cand.get(); p.wl_redo = h->wl_redo.get();
+  p.lvl_b1 = h->lvl_b1; p.lvl_b2 = h->lvl_b2;
   B200_CUDA(cudaEventRecord(h->ev0, st));
-  if (n_sparse > 0) {
+  if (pair_path) {
+    // upper pass -> exchange -> select; the select kernel's redo list (every column after a fallback) goes through the K1-D
+    // kernel, which hands its overflowed columns to the window kernel as below.  No host round trip.
+    B200_CUDA(cudaMemcpyAsync(h->fail.get(), &h->n_dense_last, sizeof(int), cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemsetAsync(h->pair_ctl.get(), 0, 4 * sizeof(int), st));
+    KParams q = p;
+    q.n_range = h->n_cols;  // the upper pass's work list holds every column
+    sim_k1d_upper_kernel<<<std::min(h->n_cols, h->n_sm * h->ctas_up), D_THREADS, h->smem_up_bytes, st>>>(q);
+    q.n_range = n_sparse;
+    B200_CUDA(cudaGetLastError());
+    k1d_pair_degree_kernel<<<GRID1D, 256, 0, st>>>(q, h->deg.get());
+    B200_CUDA(cudaGetLastError());
+    size_t tb = h->scan_tmp_bytes;
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), tb, h->deg.get(), h->cand_off.get(), h->n_cols + 1, st));
+    k1d_pair_scatter_kernel<<<GRID1D, 256, 0, st>>>(q, h->deg.get());
+    B200_CUDA(cudaGetLastError());
+    k1d_select_kernel_for(h->formula)<<<n_sparse, D_THREADS, 0, st>>>(q);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
+    q.worklist = h->wl_redo.get();
+    q.n_range_dev = p.n_redo;
+    k1d_kernel_for(h->formula)<<<std::min(n_sparse, h->n_sm * h->ctas_per_sm), D_THREADS, h->smem1_bytes, st>>>(q);
+    B200_CUDA(cudaGetLastError());
+    count_launch(7);
+    B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
+    p.n_range_dev = h->fail.get();
+  } else if (n_sparse > 0) {
     // nibble-counter kernel first; columns with an overflowed counter are appended to the window kernel's list, whose length
     // the window kernel then reads from the device (no host round trip between the two launches)
     B200_CUDA(cudaMemcpyAsync(h->fail.get(), &h->n_dense_last, sizeof(int), cudaMemcpyHostToDevice, st));
@@ -1846,17 +2040,17 @@ int b200_sim_debug_set_cap(b200_sim_t h, int cap) {
   });
 }
 
-int b200_sim_debug_phase_cycles(b200_sim_t h, int enable, uint64_t* out8) {
+int b200_sim_debug_phase_cycles(b200_sim_t h, int enable, uint64_t* out16) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_debug_phase_cycles: NULL handle");
     if (h->prof.n == 0) {
-      h->prof.alloc(8);
-      B200_CUDA(cudaMemset(h->prof.get(), 0, 8 * sizeof(unsigned long long)));
+      h->prof.alloc(16);
+      B200_CUDA(cudaMemset(h->prof.get(), 0, 16 * sizeof(unsigned long long)));
     }
-    if (out8) {
+    if (out16) {
       B200_CUDA(cudaDeviceSynchronize());
-      B200_CUDA(cudaMemcpy(out8, h->prof.get(), 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-      B200_CUDA(cudaMemset(h->prof.get(), 0, 8 * sizeof(unsigned long long)));
+      B200_CUDA(cudaMemcpy(out16, h->prof.get(), 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+      B200_CUDA(cudaMemset(h->prof.get(), 0, 16 * sizeof(unsigned long long)));
     }
     h->prof_on = enable != 0;
   });

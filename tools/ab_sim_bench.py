@@ -25,11 +25,23 @@ if sys.argv[1] == "--child":
     L = _lib.load()
     _lib.check(L.b200_sim_debug_phase_cycles(sim._h, 1, None))
     sim.compute_topk_device(0, n); torch.cuda.synchronize()
-    out = (ctypes.c_uint64 * 8)()
+    out = (ctypes.c_uint64 * 16)()
     _lib.check(L.b200_sim_debug_phase_cycles(sim._h, 0, out))
     cyc = np.array(list(out), dtype=np.float64) / n
-    print("%-10s kernel ms %s  checksum %s  cycles/col stage=%.0f mac=%.0f boot=%.0f scan=%.0f eval=%.0f select=%.0f emit=%.0f" % (
-        sys.argv[3], " ".join("%.2f" % m for m in ms), chk, *cyc[:7]), flush=True)
+    print("%-10s kernel ms %s  checksum %s  cycles/col stage=%.0f mac=%.0f boot=%.0f scan=%.0f eval=%.0f select=%.0f emit=%.0f"
+          "  pair path: upper-gather=%.0f upper-sweep=%.0f sel-keys=%.0f sel-emit=%.0f" % (
+              sys.argv[3], " ".join("%.2f" % m for m in ms), chk, *cyc[:7], *cyc[8:12]), flush=True)
+    # device time per kernel of one call (a profiled run of its own): the gather / exchange / select split
+    from torch.profiler import profile, ProfilerActivity
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        sim.compute_topk_device(0, n); torch.cuda.synchronize()
+    per = {}
+    for e in prof.events():
+        if e.device_type.name == "CUDA":
+            key = e.name.split("<")[0].split("(")[0].replace("void ", "").replace("b200::sim::", "")
+            per[key] = per.get(key, 0.0) + e.device_time_total / 1e3
+    print("%-10s kernel split ms: %s" % (sys.argv[3], ", ".join("%s %.2f" % kv for kv in sorted(per.items(), key=lambda kv: -kv[1]))),
+          flush=True)
     sys.exit(0)
 
 from recsys2019_deeplearning_evaluation_b200.synth import synth_config

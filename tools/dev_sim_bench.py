@@ -25,7 +25,7 @@ from recsys2019_deeplearning_evaluation_b200 import _lib
 L = _lib.load()
 _lib.check(L.b200_sim_debug_phase_cycles(sim._h, 1, None))
 tab = sim.compute_topk_device(0, X.shape[1]); torch.cuda.synchronize()
-out = (ctypes.c_uint64 * 8)()
+out = (ctypes.c_uint64 * 16)()
 _lib.check(L.b200_sim_debug_phase_cycles(sim._h, 0, out))
 cyc = np.array(list(out), dtype=np.float64)
 en, tb, nb, nw = (ctypes.c_int32() for _ in range(4))
