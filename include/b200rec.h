@@ -129,8 +129,8 @@ int b200_sim_debug_set_cap(b200_sim_t h, int cap);
 /* TEST/BENCH HOOK: per-phase SM-cycle counters of the top-K kernels, summed over CTAs (thread 0's clock):
  * [0] stage  [1] accumulate  [2] bootstrap histogram  [3] scan+clear  [4] evaluate+compact  [5] select
  * [6] emit (window kernel); the bitmap kernel reports [1] accumulate  [2] level >= 3  [3] level 2  [4] level 1  [6] emit+clear;
- * its pair path reports [8] upper-pass gather  [9] upper-pass sweep + pair append  [10] select kernel: keys + decision
- * [11] select kernel: select + emit.  enable!=0 turns counting on for later launches; out16 (nullable) receives and resets
+ * its pair path reports [8] upper-pass gather  [9] upper-pass sweep + own-list write  [10] select kernel: keys + decision
+ * [11] select kernel: select + emit (one warp per column: lane 0's clock, summed over warps).  enable!=0 turns counting on for later launches; out16 (nullable) receives and resets
  * the counters. */
 int b200_sim_debug_phase_cycles(b200_sim_t h, int enable, uint64_t* out16);
 

@@ -412,21 +412,25 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
 //
 // The kernel above builds C[i][j] in pass i and again in pass j: it streams the whole row of every user of column i.  On a
 // call that covers every column, the upper pass streams only the part of each row after i (rows are sorted by the new
-// index), so pass i counts the neighbours j > i: half the gathered entries and half the shared atomics.  It appends every
-// cell with count >= 3 to a global list of (i, j, count) pairs; the exchange scatters each pair into the candidate lists of
-// both i and j, and the select kernel applies the rule of the kernel above to those lists: with at least K positive keys
+// index), so pass i counts the neighbours j > i: half the gathered entries and half the shared atomics.  It writes column
+// i's cells with count >= 3 as one contiguous own list and counts them into deg[j]; the exchange copies each cell into the
+// mirror list of j, so column c's candidates are its own list plus its mirror list, and the select kernel (one warp per
+// column) applies the rule of the kernel above to them: with at least K positive keys
 // and no count-2 / count-1 cell that can reach the floor sim(3, largest norm term) (bounded by the smallest norm term of
 // the columns with at least 2 / 1 users), the K best count >= 3 cells are the answer -- the same keys from the same counts
 // and norm terms, so the output is the same.  Every other column (fewer
-// than K candidates, count-2 / count-1 cells that matter, a list longer than the key registers) is appended to a device
+// than K candidates, count-2 / count-1 cells that matter, more than S_CAP candidates) is appended to a device
 // redo list that the kernel above then computes in full.  A counter overflow in the upper pass (the nibble checksum over
-// the suffix increments) or a full pair list sets a flag on the device, and the select kernel then hands EVERY column to
+// the suffix increments) or a full list sets a flag on the device, and the select kernel then hands EVERY column to
 // the kernel above: exactness never depends on the pair path.  Whether a handle takes the path at all is decided at create
 // time from the norm terms and the column lengths (k1d_pair_gate in sim_topk.cu): a column handed back costs a full pass
 // on top of the upper pass, so the path only pays when the select kernel can decide nearly every column.
 
 constexpr int U_STAGE = 2048;  // count >= 3 cells of one column staged in shared memory before one global reservation
 constexpr int U_STEPS = 1;     // loads of 32 chunks in flight per warp (more spill at 64 registers)
+// own_n flag: the column's cells overflowed its stage; the cells past it went to the loose list, so its own list is
+// incomplete and the select kernel hands the column to the redo list (it has more than S_CAP candidates anyway)
+constexpr int OWN_SPILLED = (int)0x80000000u;
 
 struct K1DUpShared {
   int item, adds, nibsum, ncand, nst;
@@ -512,7 +516,8 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
     __syncthreads();
     PROF_MARK(8);
 
-    // ---------------- sweep of the words that hold j > col: checksum, count >= 3 cells into the stage, clear
+    // ---------------- sweep of the words that hold j > col: checksum, count >= 3 cells into the stage (past it: the loose
+    // list), clear; every cell counts into deg[j] (fire-and-forget)
     {
       int ns = 0;
       uint4* acc4 = reinterpret_cast<uint4*>(acc);
@@ -536,18 +541,20 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
           const bool staged = pos + c3 <= U_STAGE;
           unsigned long long g = 0ull;
           if (staged) atomicAdd(&us.nst, c3);
-          else g = atomicAdd(p.n_pairs, (unsigned long long)c3);
+          else g = atomicAdd(p.n_loose, (unsigned long long)c3);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             unsigned mm = m[e];
             while (mm) {
               const int q = (__ffs(mm) - 1) >> 2;
               mm &= mm - 1;
-              const unsigned cd = ((unsigned)((i4 * 4 + e) * 8 + q) << 4) | ((ww[e] >> (q << 2)) & 15u);
+              const int j = (i4 * 4 + e) * 8 + q;
+              const unsigned cd = ((unsigned)j << 4) | ((ww[e] >> (q << 2)) & 15u);
               if (staged) {
                 stage[pos++] = cd;
               } else {
-                if (g < (unsigned long long)p.pair_cap) p.pairs[g] = ((u64)col << 32) | cd;
+                atomicAdd(p.deg + j, 1);
+                if (g < (unsigned long long)p.loose_cap) p.loose[g] = ((u64)col << 32) | cd;
                 else atomicExch(p.pair_fail, 1);
                 ++g;
               }
@@ -562,80 +569,152 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
     const int nst = us.nst;
     if (tid == 0) {
       if (us.nibsum != us.adds) atomicExch(p.pair_fail, 1);  // a counter overflowed: the call falls back
-      us.base = nst ? atomicAdd(p.n_pairs, (unsigned long long)nst) : 0ull;
+      us.base = nst ? atomicAdd(p.n_own, (unsigned long long)nst) : 0ull;
       if (us.base + nst > (unsigned long long)p.pair_cap) atomicExch(p.pair_fail, 1);
+      p.own_off[col] = (int)us.base;  // < pair_cap < 2^30 unless the call has fallen back
+      p.own_n[col] = nst | (us.ncand > nst ? OWN_SPILLED : 0);
     }
     __syncthreads();
     const unsigned long long base = us.base;
     if (base + nst <= (unsigned long long)p.pair_cap)
-      for (int t = tid; t < nst; t += D_THREADS) p.pairs[base + t] = ((u64)col << 32) | stage[t];
+      for (int t = tid; t < nst; t += D_THREADS) {
+        const unsigned cd = stage[t];
+        p.own[base + t] = cd;
+        atomicAdd(p.deg + (cd >> 4), 1);
+      }
     PROF_MARK(9);
   }
 }
 
-// Exchange, step 1: candidates per column (both ends of every pair).  Skipped when the call has fallen back.
-__global__ void k1d_pair_degree_kernel(const KParams p, int* deg) {
-  if (*p.pair_fail) return;
-  const long long n = (long long)min(*p.n_pairs, (u64)p.pair_cap);
-  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-    const u64 pr = p.pairs[q];
-    atomicAdd(deg + (int)(pr >> 32), 1);
-    atomicAdd(deg + (int)(((unsigned)pr) >> 4), 1);
+// Exchange (after the exclusive scan of deg into mir_off): every cell (i, j, count) of the own lists (one warp per column
+// i) and of the loose list into the mirror list of j as (i << 4 | count).  Counting deg back down leaves it zero for the
+// next call; after a fallback nothing is exchanged and deg is cleared.  Launched with n_cols warps.
+__global__ void k1d_pair_scatter_kernel(const KParams p) {
+  const long long t0 = blockIdx.x * (long long)blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+  if (*p.pair_fail) {
+    for (long long q = t0; q <= p.n_cols; q += nt) p.deg[q] = 0;
+    return;
+  }
+  const int i = (int)(t0 >> 5), lane = threadIdx.x & 31;
+  if (i < p.n_cols) {
+    const int s = p.own_off[i], n = p.own_n[i] & ~OWN_SPILLED;
+    for (int t = lane; t < n; t += 32) {
+      const unsigned cd = p.own[s + t], j = cd >> 4;
+      p.mir[p.mir_off[j] + atomicSub(p.deg + j, 1) - 1] = ((unsigned)i << 4) | (cd & 15u);
+    }
+  }
+  const long long nl = (long long)min(*p.n_loose, (u64)p.loose_cap);
+  for (long long q = t0; q < nl; q += nt) {
+    const u64 e = p.loose[q];
+    const unsigned cd = (unsigned)e, j = cd >> 4;
+    p.mir[p.mir_off[j] + atomicSub(p.deg + j, 1) - 1] = ((unsigned)(e >> 32) << 4) | (cd & 15u);
   }
 }
 
-// Exchange, step 2 (after the exclusive scan of deg into cand_off): every pair into the lists of both ends as
-// (neighbour << 4 | count).  Counting deg back down leaves it zero for the next call.
-__global__ void k1d_pair_scatter_kernel(const KParams p, int* deg) {
-  if (*p.pair_fail) return;
-  const long long n = (long long)min(*p.n_pairs, (u64)p.pair_cap);
-  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-    const u64 pr = p.pairs[q];
-    const unsigned i = (unsigned)(pr >> 32), lo = (unsigned)pr, j = lo >> 4, c = lo & 15u;
-    p.cand[p.cand_off[i] + atomicSub(deg + i, 1) - 1] = lo;
-    p.cand[p.cand_off[j] + atomicSub(deg + j, 1) - 1] = (i << 4) | c;
+constexpr int S_WARPS = 4;            // columns (warps) per CTA of the select kernel: shared memory allows 3 CTAs per SM
+constexpr int S_CAP = 4 * D_THREADS;  // the longest candidate list the select kernel decides (the K1-D kernel's key buffer)
+constexpr int S_ILP = 16;             // candidates per lane in flight while the keys are built (C5: ~430 per column)
+struct SelWarp {
+  u64 key[S_CAP];
+  int hist[256];
+};
+
+// One warp: the K-th largest key of buf[0..n), so that exactly the K largest keys are >= it (0 when n <= K: nothing is
+// cut).  Keys are distinct and non-zero.  d_select's MSB-first radix select with 8-bit digits on one warp and its own
+// histogram: it starts below the leading digits that every key shares and stops as soon as a whole bin is taken.
+__device__ u64 w_select(const u64* buf, int* hist, int n, int K) {
+  const int lane = threadIdx.x & 31;
+  if (n <= K) return 0ull;
+  u64 o = 0ull, a = ~0ull;
+  for (int q = lane; q < n; q += 32) { const u64 k = buf[q]; o |= k; a &= k; }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) { o |= __shfl_xor_sync(0xffffffffu, o, off); a &= __shfl_xor_sync(0xffffffffu, a, off); }
+  const u64 diff = o ^ a;
+  int pass = diff ? (63 - __clzll((long long)diff)) >> 3 : 0;
+  u64 prefix = pass < 7 ? (o >> ((pass + 1) * 8)) << ((pass + 1) * 8) : 0ull;
+  int need = K;
+  const int one = n > 0 ? 1 : 0;  // a run-time 1, as in d_select
+  for (; pass >= 0; --pass) {
+    const int shift = pass * 8;
+    for (int b = lane; b < 256; b += 32) hist[b] = 0;
+    __syncwarp();
+    for (int q = lane; q < n; q += 32) {
+      const u64 k = buf[q];
+      if (pass == 7 || (k >> (shift + 8)) == (prefix >> (shift + 8))) atomicAdd(&hist[(int)((k >> shift) & 255ull)], one);
+    }
+    __syncwarp();
+    int c[8], local = 0;  // bins 255 .. 0, eight per lane, highest bins in lane 0
+#pragma unroll
+    for (int b = 0; b < 8; ++b) { c[b] = hist[255 - (lane * 8 + b)]; local += c[b]; }
+    int incl = local;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, off);
+      if (lane >= off) incl += t;
+    }
+    int cum = incl - local, digit = -1, rest = 0, bincnt = 0;
+#pragma unroll
+    for (int b = 0; b < 8; ++b) {
+      if (cum < need && cum + c[b] >= need) { digit = 255 - (lane * 8 + b); rest = need - cum; bincnt = c[b]; }
+      cum += c[b];
+    }
+    const int src = __ffs(__ballot_sync(0xffffffffu, digit >= 0)) - 1;
+    digit = __shfl_sync(0xffffffffu, digit, src);
+    need = __shfl_sync(0xffffffffu, rest, src);
+    bincnt = __shfl_sync(0xffffffffu, bincnt, src);
+    prefix |= ((u64)digit) << shift;
+    __syncwarp();  // every lane has read the histogram before the next pass clears it
+    if (bincnt == need) break;
   }
+  return prefix;
 }
 
-// One CTA per column of the work list: keys from the candidate list, the decision rule of sim_k1d_kernel's collected path,
-// the K best, emit -- or the column goes to the redo list (all columns when the call has fallen back).
+// One warp per column of the work list: keys from the column's own and mirror lists, the decision rule of sim_k1d_kernel's
+// collected path, the K best, emit -- or the column goes to the redo list (all columns when the call has fallen back).
+// No block barriers: a column's three dependent loads (list bounds, list, norm terms) overlap with the other warps' work.
 template <int F>
-__global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_select_kernel(const KParams p) {
-  __shared__ u64 buf[4 * D_THREADS];
-  __shared__ K1DShared ds;
-  const int tid = threadIdx.x;
-  const int item = blockIdx.x;
+__global__ void __launch_bounds__(32 * S_WARPS) sim_k1d_select_kernel(const KParams p) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  SelWarp& sw = reinterpret_cast<SelWarp*>(smem_raw)[threadIdx.x >> 5];
+  const int lane = threadIdx.x & 31;
+  const int item = blockIdx.x * S_WARPS + (threadIdx.x >> 5);
+  if (item >= p.n_range) return;
   const int4 wi = __ldg(p.worklist + item);
   if (*(volatile int*)p.pair_fail) {
-    if (tid == 0) { p.wl_redo[item] = wi; atomicAdd(p.n_redo, 1); }  // every column, in the work list's order
+    if (lane == 0) { p.wl_redo[item] = wi; atomicAdd(p.n_redo, 1); }  // every column, in the work list's order
     return;
   }
   long long prof_t = p.prof ? clock64() : 0;
   const int col = wi.x, lc = wi.y, K = p.K;
-  const int s = p.cand_off[col], n = p.cand_off[col + 1] - s;
-  bool ok = n <= 4 * D_THREADS;
+  const int so = p.own_off[col], no = p.own_n[col];  // no < 0: OWN_SPILLED
+  const int sm = p.mir_off[col], n = no + (p.mir_off[col + 1] - sm);
+  bool ok = no >= 0 && n <= S_CAP;
   int n_have = 0;
   if (ok) {
-    if (tid == 0) ds.nbuf = 0;
     const float Ai = p.A[col];
-    u64 keys[4];
+    for (int t0 = 0; t0 < n; t0 += 32 * S_ILP) {
+      unsigned cd[S_ILP];
+      int2 bn[S_ILP];
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int t = q * D_THREADS + tid;
-      keys[q] = 0ull;
-      if (t < n) {
-        const unsigned cd = p.cand[s + t];
-        const int2 bn = __ldg(p.BN + (cd >> 4));
-        const float sv = sim_value<F>(p, (float)(cd & 15u), Ai, __int_as_float(bn.x));
-        if (sv > 0.f) keys[q] = (((u64)__float_as_uint(sv)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)bn.y);
+      for (int q = 0; q < S_ILP; ++q) {
+        const int t = t0 + 32 * q + lane;
+        cd[q] = t < n ? (t < no ? p.own[so + t] : p.mir[sm + (t - no)]) : 0u;
+      }
+#pragma unroll
+      for (int q = 0; q < S_ILP; ++q)
+        if (t0 + 32 * q + lane < n) bn[q] = __ldg(p.BN + (cd[q] >> 4));
+#pragma unroll
+      for (int q = 0; q < S_ILP; ++q) {
+        u64 key = 0ull;
+        if (t0 + 32 * q + lane < n) {
+          const float sv = sim_value<F>(p, (float)(cd[q] & 15u), Ai, __int_as_float(bn[q].x));
+          if (sv > 0.f) key = (((u64)__float_as_uint(sv)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)bn[q].y);
+        }
+        const unsigned b = __ballot_sync(0xffffffffu, key != 0ull);
+        if (key) sw.key[n_have + __popc(b & ((1u << lane) - 1u))] = key;
+        n_have += __popc(b);
       }
     }
-    __syncthreads();
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-      if (keys[q]) buf[atomicAdd(&ds.nbuf, 1)] = keys[q];
-    __syncthreads();
-    n_have = ds.nbuf;
     ok = false;
     if (n_have >= K) {
       // floor of the K-th best: (count 3, largest norm term); no count-2 / count-1 cell may reach it.  A count-c cell's
@@ -644,21 +723,29 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_select_kernel(const KPar
       if (fl > 0.f) ok = !(sim_value<F>(p, 2.f, Ai, p.lvl_b2) >= fl) && !(sim_value<F>(p, 1.f, Ai, p.lvl_b1) >= fl);
     }
   }
-  PROF_MARK(10);
+  PROF_MARK_WARP(10);
   if (!ok) {
-    if (tid == 0) p.wl_redo[atomicAdd(p.n_redo, 1)] = wi;
+    if (lane == 0) p.wl_redo[atomicAdd(p.n_redo, 1)] = wi;
     return;
   }
-  int kept;
-  d_select(buf, n_have, K, &ds, &kept);
+  __syncwarp();
+  const u64 thr = w_select(sw.key, sw.hist, n_have, K);
+  // emit while compacting: the kept keys of every 32 take the next output slots in lane order
   const size_t out_base = (size_t)lc * K;
-  for (int t = tid; t < kept; t += D_THREADS) {
-    const u64 k64 = buf[t];
-    emit_entry(p, out_base + t, (int)(0xFFFFFFFFu - (unsigned)k64), __uint_as_float((unsigned)(k64 >> 32)));
+  int kept = 0;
+  for (int t0 = 0; t0 < n_have; t0 += 32) {
+    const int t = t0 + lane;
+    const u64 k64 = t < n_have ? sw.key[t] : 0ull;
+    const bool keep = t < n_have && k64 >= thr;
+    const unsigned b = __ballot_sync(0xffffffffu, keep);
+    if (keep)
+      emit_entry(p, out_base + kept + __popc(b & ((1u << lane) - 1u)), (int)(0xFFFFFFFFu - (unsigned)k64),
+                 __uint_as_float((unsigned)(k64 >> 32)));
+    kept += __popc(b);
   }
-  for (int t = kept + tid; t < K; t += D_THREADS) emit_entry(p, out_base + t, -1, 0.f);
-  if (tid == 0) emit_count(p, lc, kept);
-  PROF_MARK(11);
+  for (int t = kept + lane; t < K; t += 32) emit_entry(p, out_base + t, -1, 0.f);
+  if (lane == 0) emit_count(p, lc, kept);
+  PROF_MARK_WARP(11);
 }
 
 // tb[t] = norm term at neighbour min(t << D_TILE_LOG2, n_cols - 1), t = 0 .. ntile

@@ -119,15 +119,24 @@ struct KParams {
   int* fail;
   const int* n_range_dev;  // window kernel / K1-D kernel: the number of columns to process is read from here when set
   // K1-D pair path (sim_k1d.cuh): per CSC entry the suffix of the user's padded row after the column, the work items in
-  // suffix-work order, the list of (i, j, count >= 3) pairs with j > i and its capacity, the candidate lists built from it,
-  // the flag that sends the whole call down the K1-D kernel, and the columns that the select kernel hands to the K1-D kernel
+  // suffix-work order; the own lists (column i's count >= 3 cells (j << 4 | count), j > i, one contiguous run per column:
+  // start and length by column), their capacity and fill; the loose list of (i << 32 | j << 4 | count) cells that did not fit
+  // a column's stage, its capacity and fill; the per-column mirror counts (deg) and offsets and the mirror lists built from
+  // them ((i << 4 | count) in the list of j); the flag that sends the whole call down the K1-D kernel, and the columns that
+  // the select kernel hands to the K1-D kernel
   const int2* __restrict__ csc_suf;
   const int4* __restrict__ worklist_up;
-  u64* pairs;
-  u64* n_pairs;
+  unsigned* own;
+  int* own_off;
+  int* own_n;  // | OWN_SPILLED when the column's cells overflowed its stage
+  u64* n_own;
   long long pair_cap;
-  const int* __restrict__ cand_off;
-  unsigned* cand;
+  u64* loose;
+  u64* n_loose;
+  long long loose_cap;
+  int* deg;
+  const int* __restrict__ mir_off;
+  unsigned* mir;
   int* pair_fail;
   int4* wl_redo;
   int* n_redo;
@@ -238,6 +247,15 @@ __device__ __forceinline__ float lower_bound_scale(const KParams& p, float a, fl
 #define PROF_MARK(ph)                                                        \
   do {                                                                      \
     if (p.prof && threadIdx.x == 0) {                                       \
+      const long long _t = clock64();                                       \
+      atomicAdd(p.prof + (ph), (unsigned long long)(_t - prof_t));          \
+      prof_t = _t;                                                          \
+    }                                                                       \
+  } while (0)
+// the same from lane 0 of every warp (kernels that work one column per warp; prof_t per warp)
+#define PROF_MARK_WARP(ph)                                                   \
+  do {                                                                      \
+    if (p.prof && (threadIdx.x & 31) == 0) {                                \
       const long long _t = clock64();                                       \
       atomicAdd(p.prof + (ph), (unsigned long long)(_t - prof_t));          \
       prof_t = _t;                                                          \
@@ -1229,18 +1247,18 @@ struct b200_sim_s {
   std::vector<int> h_old2new, h_csc_ptr;
   int n_sparse_last = 0, n_dense_last = 0;
   std::vector<unsigned long long> h_work;  // by ORIGINAL column index
-  // K1-D pair path (sim_k1d.cuh): row suffixes, the upper pass's work list (every column), pair list (capacity from the
-  // expected pair count), candidate lists (deg: per-column counts, zero between calls), control words (pair count,
-  // fallback flag, redo count), redo list, scan scratch (all allocated by the first call that takes the path), the select
-  // kernel's level bounds, upper-pass geometry
+  // K1-D pair path (sim_k1d.cuh): row suffixes, the upper pass's work list (every column), own lists (capacity from the
+  // expected pair count) with their per-column start and length, loose list, mirror lists (deg: per-column counts, zero
+  // between calls), control words (own and loose fill, fallback flag, redo count), redo list, scan scratch (all allocated
+  // by the first call that takes the path), the select kernel's level bounds, upper-pass geometry
   DevBuf<int2> csc_suf;
   DevBuf<int4> worklist_up, wl_redo;
-  DevBuf<u64> pairs;
-  long long pair_cap = 0;
+  DevBuf<unsigned> own, mir;
+  DevBuf<u64> loose;
+  long long pair_cap = 0, loose_cap = 0;
   double pairs_expected = 0.0;
   float lvl_b1 = 0.f, lvl_b2 = 0.f;
-  DevBuf<unsigned> cand;
-  DevBuf<int> deg, cand_off, pair_ctl;
+  DevBuf<int> own_off, own_n, deg, mir_off, pair_ctl;
   DevBuf<unsigned char> scan_tmp;
   size_t scan_tmp_bytes = 0, smem_up_bytes = 0;
   int ctas_up = 0;
@@ -1699,6 +1717,8 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       if (h->ctas_up > 0) {
         B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_up_bytes));
         B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_WARPS * sizeof(SelWarp))));
+        B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         h->worklist_up.alloc((size_t)n_cols);
         // the upper pass's longest-first order: every column by descending suffix work (empty columns do nothing there)
         DevBuf<unsigned long long> keys_out((size_t)n_cols);
@@ -1901,50 +1921,54 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.redo = h->order.get(); p.fail = h->fail.get();
   p.n_range_dev = nullptr;
   p.csc_suf = h->csc_suf.get(); p.worklist_up = h->worklist_up.get();
-  if (pair_path && h->pairs.n == 0) {
-    // first call on the pair path: the pair list holds twice the expected pairs (a fuller list sets the fallback flag), the
-    // candidate lists twice that; candidate positions stay below 2^31
+  if (pair_path && h->own.n == 0) {
+    // first call on the pair path: the own lists hold twice the expected pairs (a fuller list sets the fallback flag), the
+    // loose list (cells past a column's stage: rare) a quarter of that, the mirror lists both; positions stay below 2^31
     h->pair_cap = std::min<long long>((long long)(2.0 * h->pairs_expected) + (1 << 16), (1ll << 30) - 1);
-    h->pairs.alloc((size_t)h->pair_cap);
-    h->cand.alloc(2 * (size_t)h->pair_cap);
+    h->loose_cap = h->pair_cap / 4 + (1 << 16);
+    h->own.alloc((size_t)h->pair_cap);
+    h->loose.alloc((size_t)h->loose_cap);
+    h->mir.alloc((size_t)(h->pair_cap + h->loose_cap));
+    h->own_off.alloc((size_t)h->n_cols);
+    h->own_n.alloc((size_t)h->n_cols);
     h->deg.alloc((size_t)h->n_cols + 1);
-    h->cand_off.alloc((size_t)h->n_cols + 1);
-    h->pair_ctl.alloc(4);  // [0..1] pair count (64-bit), [2] fallback flag, [3] redo count
+    h->mir_off.alloc((size_t)h->n_cols + 1);
+    h->pair_ctl.alloc(6);  // [0..1] own fill (64-bit), [2] fallback flag, [3] redo count, [4..5] loose fill (64-bit)
     h->wl_redo.alloc((size_t)h->n_cols);
     B200_CUDA(cudaMemsetAsync(h->deg.get(), 0, sizeof(int) * ((size_t)h->n_cols + 1), st));
-    B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, h->scan_tmp_bytes, h->deg.get(), h->cand_off.get(), h->n_cols + 1, st));
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, h->scan_tmp_bytes, h->deg.get(), h->mir_off.get(), h->n_cols + 1, st));
     h->scan_tmp.alloc(h->scan_tmp_bytes + 16);
   }
-  p.pairs = h->pairs.get(); p.pair_cap = h->pair_cap;
-  p.n_pairs = reinterpret_cast<u64*>(h->pair_ctl.get());
+  p.own = h->own.get(); p.own_off = h->own_off.get(); p.own_n = h->own_n.get(); p.pair_cap = h->pair_cap;
+  p.n_own = reinterpret_cast<u64*>(h->pair_ctl.get());
   p.pair_fail = h->pair_ctl.get() + 2; p.n_redo = h->pair_ctl.get() + 3;
-  p.cand_off = h->cand_off.get(); p.cand = h->cand.get(); p.wl_redo = h->wl_redo.get();
+  p.loose = h->loose.get(); p.n_loose = reinterpret_cast<u64*>(h->pair_ctl.get() + 4); p.loose_cap = h->loose_cap;
+  p.deg = h->deg.get(); p.mir_off = h->mir_off.get(); p.mir = h->mir.get(); p.wl_redo = h->wl_redo.get();
   p.lvl_b1 = h->lvl_b1; p.lvl_b2 = h->lvl_b2;
   B200_CUDA(cudaEventRecord(h->ev0, st));
   if (pair_path) {
-    // upper pass -> exchange -> select; the select kernel's redo list (every column after a fallback) goes through the K1-D
-    // kernel, which hands its overflowed columns to the window kernel as below.  No host round trip.
+    // upper pass (own lists, deg) -> exchange (mirror lists) -> select; the select kernel's redo list (every column after a
+    // fallback) goes through the K1-D kernel, which hands its overflowed columns to the window kernel as below.  No host
+    // round trip.
     B200_CUDA(cudaMemcpyAsync(h->fail.get(), &h->n_dense_last, sizeof(int), cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemsetAsync(h->pair_ctl.get(), 0, 4 * sizeof(int), st));
+    B200_CUDA(cudaMemsetAsync(h->pair_ctl.get(), 0, 6 * sizeof(int), st));
     KParams q = p;
     q.n_range = h->n_cols;  // the upper pass's work list holds every column
     sim_k1d_upper_kernel<<<std::min(h->n_cols, h->n_sm * h->ctas_up), D_THREADS, h->smem_up_bytes, st>>>(q);
     q.n_range = n_sparse;
     B200_CUDA(cudaGetLastError());
-    k1d_pair_degree_kernel<<<GRID1D, 256, 0, st>>>(q, h->deg.get());
-    B200_CUDA(cudaGetLastError());
     size_t tb = h->scan_tmp_bytes;
-    B200_CUDA(cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), tb, h->deg.get(), h->cand_off.get(), h->n_cols + 1, st));
-    k1d_pair_scatter_kernel<<<GRID1D, 256, 0, st>>>(q, h->deg.get());
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), tb, h->deg.get(), h->mir_off.get(), h->n_cols + 1, st));
+    k1d_pair_scatter_kernel<<<div_up((long long)h->n_cols * 32, 256), 256, 0, st>>>(q);
     B200_CUDA(cudaGetLastError());
-    k1d_select_kernel_for(h->formula)<<<n_sparse, D_THREADS, 0, st>>>(q);
+    k1d_select_kernel_for(h->formula)<<<div_up(n_sparse, S_WARPS), 32 * S_WARPS, S_WARPS * sizeof(SelWarp), st>>>(q);
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
     q.worklist = h->wl_redo.get();
     q.n_range_dev = p.n_redo;
     k1d_kernel_for(h->formula)<<<std::min(n_sparse, h->n_sm * h->ctas_per_sm), D_THREADS, h->smem1_bytes, st>>>(q);
     B200_CUDA(cudaGetLastError());
-    count_launch(7);
+    count_launch(6);
     B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
     p.n_range_dev = h->fail.get();
   } else if (n_sparse > 0) {
