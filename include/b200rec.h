@@ -227,12 +227,14 @@ int b200_asysvd_last_epoch_ms(b200_asysvd_t h, float* ms);
  * K3: SLIM-BPR epochs on a dense / symmetric item-item matrix  (hot path ii)
  * replaces  SLIM_BPR/Cython/SLIM_BPR_Cython_Epoch.pyx:60-480  (ctor :88-134, epochIteration_Cython :211-335,
  *           sampleBPR_Cython :436-480, adaptive_gradient :395-433, get_S :340-388, Triangular_Matrix :1223-1415)
- * The tree-sparse training mode (train_with_sparse_weights, Sparse_Matrix_Tree_CSR :579-1031) keeps its semantics on the
- * dense array: b200_slim_enable_tree / b200_slim_tree_prune below.
+ * The tree-sparse training mode (train_with_sparse_weights, Sparse_Matrix_Tree_CSR :579-1031) keeps S row-sparse on the
+ * device, so a catalogue whose dense S does not fit trains on one GPU: b200_slim_enable_tree / b200_slim_tree_prune /
+ * b200_slim_tree_csr below.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct b200_slim_s* b200_slim_t;
 
-/* URM_mask: CSR, sorted indices (pyx:100-119).  S starts at zero.  hogwild == 0: the batch-1 recursion in stream
+/* URM_mask: CSR, sorted indices (pyx:100-119).  S starts at zero; the dense n_items^2 fp32 S is allocated by the first call
+ * that needs it, so a handle that becomes a tree handle never holds one.  hogwild == 0: the batch-1 recursion in stream
  * order on one CTA (the reference's semantics); hogwild != 0: all SMs, atomics, no ordering between samples. */
 int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* h_indptr,
                      const int32_t* h_indices, float learning_rate, float li_reg, float lj_reg, int symmetric,
@@ -247,14 +249,23 @@ int b200_slim_get_samples(b200_slim_t h, int32_t* u, int32_t* i, int32_t* j);
 int b200_slim_get_S_dense(b200_slim_t h, float* h_out, float* d_out);
 int b200_slim_last_epoch_ms(b200_slim_t h, float* ms);
 /* train_with_sparse_weights=True (pyx:111-134): call once after b200_slim_create (symmetric = 0, hogwild = 0) and before the
- * first epoch.  A byte map records the cells the reference's row trees would hold (add_value, pyx:617-680); every epoch cuts
- * the rows that hold >= topK cells back to their topK largest after the samples n with n % (n_users / 5) == 0
+ * first epoch.  S is a row-sorted CSR of the cells the reference's row trees would hold (add_value, pyx:617-680).  The epoch
+ * runs as segments between the samples n with n % (n_users / 5) == 0; before a segment, the cells it will create are added
+ * with value 0 (the sample stream does not depend on S), every update gets the index of its cell, and the sequential kernel
+ * updates those cells.  After each segment but the last, rows holding more than topK cells keep their topK largest
  * (rebalance_tree, pyx:318-319, :782-802; ties keep the higher column like the reference's stable qsort, :991).
- * topK = 0 is the reference's topK=False: nothing is ever removed. */
+ * topK = 0 is the reference's topK=False: nothing is ever removed.  Device memory follows the cell count (12 bytes per
+ * cell plus about 3x that for the segment's sort), not n_items^2. */
 int b200_slim_enable_tree(b200_slim_t h, int topK);
 /* the selection get_S() applies IN PLACE before it emits the rows (get_scipy_csr(TopK), pyx:762-763); touch_diagonal != 0
  * first creates the diagonal cells with value 0 like get_S does (pyx:349-350) -- they count towards a row's length */
 int b200_slim_tree_prune(b200_slim_t h, int touch_diagonal, void* stream);
+/* the tree state as CSR without an n_items^2 buffer: the non-zero off-diagonal cells, indices sorted within each row.
+ * b200_slim_tree_csr_nnz gives their count; b200_slim_tree_csr fills indptr[n_items + 1], indices[nnz], data[nnz] (host). */
+int b200_slim_tree_csr_nnz(b200_slim_t h, int64_t* nnz);
+int b200_slim_tree_csr(b200_slim_t h, int64_t* indptr, int32_t* indices, float* data);
+/* the cells the row-sparse structure holds now, zero-valued ones included (12 bytes of device memory each) */
+int b200_slim_tree_cells(b200_slim_t h, int64_t* cells);
 /* Column-sharded S for catalogues whose dense S does not fit one GPU (SURVEY.md 8(e) K3; the reference's answer to that is
  * the tree-sparse mode, pyx:509-1031): this handle owns S[:, col_lo:col_hi) as an [n_items, col_hi - col_lo] slab (full
  * matrix, not the triangular storage).  Every rank creates one with the SAME random_seed and draws the same Philox sample

@@ -67,6 +67,9 @@ SIGNATURES = {
     "b200_slim_last_epoch_ms": (ctypes.c_int, [c_void, c_float_p]),
     "b200_slim_enable_tree": (ctypes.c_int, [c_void, ctypes.c_int]),
     "b200_slim_tree_prune": (ctypes.c_int, [c_void, ctypes.c_int, c_void]),
+    "b200_slim_tree_csr_nnz": (ctypes.c_int, [c_void, ctypes.POINTER(ctypes.c_int64)]),
+    "b200_slim_tree_csr": (ctypes.c_int, [c_void, c_void, c_void, c_void]),
+    "b200_slim_tree_cells": (ctypes.c_int, [c_void, ctypes.POINTER(ctypes.c_int64)]),
     "b200_slim_enet_device": (ctypes.c_int, [c_void, c_void, ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_double, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_float, c_void, c_void, c_void]),
     "b200_asysvd_create": (ctypes.c_int, [ctypes.POINTER(c_void), ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, c_void, c_void, c_void,

@@ -3,9 +3,12 @@
 // Replaces SLIM_BPR/Cython/SLIM_BPR_Cython_Epoch.pyx: epochIteration_Cython :211-335, sampleBPR_Cython :436-480,
 // adaptive_gradient :395-433 (per-ITEM scalar state shared by the positive and negative roles), symmetric storage
 // Triangular_Matrix :1272-1330, get_S :340-388 (diagonal zeroed).  S is dense fp32 in HBM (C2: 55 MB, L2-resident).
-// The tree-sparse training mode (train_with_sparse_weights, Sparse_Matrix_Tree_CSR :579-1031) keeps its SEMANTICS on the
-// same dense array: a byte map records which cells the reference's row trees would hold, and the periodic
-// rebalance_tree(TopK) :782-802 / the in-place selection of get_scipy_csr(TopK) :762-763 is slim_tree_prune_kernel.
+// The tree-sparse training mode (train_with_sparse_weights, Sparse_Matrix_Tree_CSR :579-1031) keeps S ROW-SPARSE: a
+// row-sorted CSR of the cells the reference's row trees hold.  The sample stream of an epoch does not depend on S, so
+// before a segment (the samples between two rebalance_tree(TopK) cuts, :318-319, :782-802) runs, the cells it will create
+// are known: the structure is rebuilt with them (value 0, which is what a cell that does not exist yet reads), a slot map
+// gives every update of the segment the index of its cell, and the sequential kernel runs on `val[slot]`.  The cut and the
+// in-place selection of get_scipy_csr(TopK) :762-763 keep the K largest cells of each longer row.
 //
 // Two execution modes (DESIGN.md "K3"):
 //   * sequential (the reference's semantics exactly): the recursion is batch-1 and every sample reads cells the
@@ -13,6 +16,9 @@
 //     the x_uij reduction and the 2*len_u updates of a sample are spread over the CTA's threads.
 //   * hogwild: all SMs, one warp per sample, float atomics on S (Hogwild races), Philox or replayed stream.
 // Roofline: HBM/L2, 4*len_u*4 bytes per sample for S (two row gathers read + written) + 4*len_u for the profile.
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 #include <stdlib.h>
 
 #include <algorithm>
@@ -36,7 +42,9 @@ struct Params {
   const int* su; const int* si; const int* sj;
   long long n_samples;
   double* pow_out;
-  unsigned char* exists;   // tree mode: 1 where the reference's row tree holds a cell (add_value creates it, pyx:617-680)
+  float* val;              // tree mode: the values of the row-sparse cells (TreeStore)
+  const long long* slot_i; // tree mode: per update of the segment, in sample order, the cell of (i, s) (-1: s == i, never
+  const long long* slot_j; //   written, reads 0) and of (j, s) in val
   long long first;         // first sample of this launch (tree mode runs an epoch as segments between two prunings)
   int chain_pow;           // continue the Adam powers from pow_out (segment > 0) instead of b1_pow / b2_pow
   int prof;                // B200REC_SLIM_PROF=1: thread 0 times the phases of the sequential kernel (development hook)
@@ -74,6 +82,10 @@ constexpr int SEQ_WARPS = SEQ_THREADS / 32;
 // profile entry are fetched while the current sample runs, and thread 0 requests the adaptive state of i and j before the
 // reduction: what is left on the critical path of a sample is one trip for the S cells, the reduction, the gradient, and the
 // update of cells that are in L1 by then.
+// CELLS is how a cell is addressed: DENSE_CELLS through cell(p, a, b) in S; SLOT_CELLS (tree mode) through the segment's
+// slot map into val, with the same thread <-> profile-entry mapping and reduction order, so the fp32 arithmetic is the same.
+enum CellAddr { DENSE_CELLS = 0, SLOT_CELLS = 1 };
+template <int CELLS>
 __global__ void __launch_bounds__(SEQ_THREADS) slim_sequential_kernel(const Params p) {
   __shared__ float red[SEQ_WARPS];
   __shared__ float s_gi, s_gj;
@@ -84,12 +96,18 @@ __global__ void __launch_bounds__(SEQ_THREADS) slim_sequential_kernel(const Para
   if (tid < 6) prof[tid] = 0ull;
   __syncthreads();  // pow_out is rewritten at the end
   const long long last = p.first + p.n_samples;
-  // sample n in (u, i, j, s, e, sn0); sample n + 1 in (nu, ni, nj)
+  // sample n in (u, i, j, s, e, sn0); sample n + 1 in (nu, ni, nj).  SLOT_CELLS: the slots of this thread's entry of
+  // sample n in (ci0, cj0) (cj0 = -1: no entry), the sample's first update at `base` of the slot map
   int u = 0, i = 0, j = 0, s = 0, e = 0, sn0 = -1, nu = 0, ni = 0, nj = 0;
+  long long base = 0, ci0 = -1, cj0 = -1;
   if (p.n_samples > 0) {
     u = p.su[p.first]; i = p.si[p.first]; j = p.sj[p.first];
     s = p.indptr[u]; e = p.indptr[u + 1];
-    if (s + tid < e) sn0 = p.indices[s + tid];
+    if constexpr (CELLS == DENSE_CELLS) {
+      if (s + tid < e) sn0 = p.indices[s + tid];
+    } else {
+      if (s + tid < e) { ci0 = p.slot_i[tid]; cj0 = p.slot_j[tid]; }
+    }
   }
   if (p.n_samples > 1) { nu = p.su[p.first + 1]; ni = p.si[p.first + 1]; nj = p.sj[p.first + 1]; }
   if (p.prof && tid == 0) tprev = clock64();
@@ -104,13 +122,24 @@ __global__ void __launch_bounds__(SEQ_THREADS) slim_sequential_kernel(const Para
       else if (p.sgd_mode == ADAM) { st_i0 = p.m1[i]; st_i1 = p.m2[i]; st_j0 = p.m1[j]; st_j1 = p.m2[j]; }
     }
     float x = 0.f;
-    if (sn0 >= 0) x = p.S[cell(p, i, sn0)] - p.S[cell(p, j, sn0)];  // pyx:242-255
-    for (int k = s + tid + SEQ_THREADS; k < e; k += SEQ_THREADS) {
-      const int sn = p.indices[k];
-      x += p.S[cell(p, i, sn)] - p.S[cell(p, j, sn)];
-    }
     int nsn0 = -1;
-    if (ns + tid < ne) nsn0 = p.indices[ns + tid];  // the next sample's profile entry of this thread
+    long long nci0 = -1, ncj0 = -1;
+    const long long nbase = base + (e - s);
+    if constexpr (CELLS == DENSE_CELLS) {
+      if (sn0 >= 0) x = p.S[cell(p, i, sn0)] - p.S[cell(p, j, sn0)];  // pyx:242-255
+      for (int k = s + tid + SEQ_THREADS; k < e; k += SEQ_THREADS) {
+        const int sn = p.indices[k];
+        x += p.S[cell(p, i, sn)] - p.S[cell(p, j, sn)];
+      }
+      if (ns + tid < ne) nsn0 = p.indices[ns + tid];  // the next sample's profile entry of this thread
+    } else {
+      if (cj0 >= 0) x = (ci0 >= 0 ? p.val[ci0] : 0.f) - p.val[cj0];
+      for (long long q = base + tid + SEQ_THREADS; q < nbase; q += SEQ_THREADS) {
+        const long long a = p.slot_i[q];
+        x += (a >= 0 ? p.val[a] : 0.f) - p.val[p.slot_j[q]];
+      }
+      if (n + 1 < last && ns + tid < ne) { nci0 = p.slot_i[nbase + tid]; ncj0 = p.slot_j[nbase + tid]; }  // the next sample's slots
+    }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
     if (lane == 0) red[warp] = x;
@@ -147,19 +176,23 @@ __global__ void __launch_bounds__(SEQ_THREADS) slim_sequential_kernel(const Para
     // pyx:266-304.  Within one sample the cells (i, s) are distinct from each other and from the cells (j, s')
     // except in symmetric mode where (i, j) and (j, i) coincide when both i and j are in the profile -- j never is
     // (it is a sampled negative), so the cell sets are disjoint and the order inside the sample is free.
-    for (int k = s + tid; k < e; k += SEQ_THREADS) {
-      const int sn = k == s + tid ? sn0 : p.indices[k];
-      if (sn != i) {
-        const size_t c = cell(p, i, sn); const float v = p.S[c]; p.S[c] = v + p.lr * (gi - p.li_reg * v);
-        if (p.exists) p.exists[c] = 1;
+    if constexpr (CELLS == DENSE_CELLS) {
+      for (int k = s + tid; k < e; k += SEQ_THREADS) {
+        const int sn = k == s + tid ? sn0 : p.indices[k];
+        if (sn != i) { const size_t c = cell(p, i, sn); const float v = p.S[c]; p.S[c] = v + p.lr * (gi - p.li_reg * v); }
+        if (sn != j) { const size_t c = cell(p, j, sn); const float v = p.S[c]; p.S[c] = v - p.lr * (gj - p.lj_reg * v); }
       }
-      if (sn != j) {
-        const size_t c = cell(p, j, sn); const float v = p.S[c]; p.S[c] = v - p.lr * (gj - p.lj_reg * v);
-        if (p.exists) p.exists[c] = 1;
+    } else {
+      for (long long q = base + tid; q < nbase; q += SEQ_THREADS) {
+        const long long a = q == base + tid ? ci0 : p.slot_i[q];
+        const long long b = q == base + tid ? cj0 : p.slot_j[q];
+        if (a >= 0) { const float v = p.val[a]; p.val[a] = v + p.lr * (gi - p.li_reg * v); }
+        { const float v = p.val[b]; p.val[b] = v - p.lr * (gj - p.lj_reg * v); }  // s != j: j is not in the profile
       }
     }
     if (p.sgd_mode == ADAM) { b1p *= (double)p.beta1; b2p *= (double)p.beta2; }  // per sample, pyx:309-312
     u = nu; i = ni; j = nj; s = ns; e = ne; sn0 = nsn0;
+    base = nbase; ci0 = nci0; cj0 = ncj0;
     nu = nnu; ni = nni; nj = nnj;
     SLIM_MARK(4);
     __syncthreads();
@@ -315,74 +348,228 @@ __global__ void slim_shard_state_kernel(const ShardParams sp, const float* __res
   }
 }
 
-// ---- tree mode: rebalance_tree(TopK) pyx:782-802 and the in-place selection inside get_scipy_csr(TopK) pyx:762-763, both
-// through topK_selection_from_list pyx:954-1031.  A row whose tree holds at least K cells keeps the K largest by value; the
-// reference sorts the column-ordered list with a stable qsort on the value, so among equal values the HIGHER columns
-// survive: key = (value bits << 32) | column, keep the K largest keys.  Cells that are dropped cease to exist and read as 0.
-// One CTA per row, 11-bit radix select over the 64-bit keys (the row is L2-resident across the six passes).
+// ---- tree mode (row-sparse).  The cells live in a row-sorted CSR: key[t] = (row << 32) | col, val[t], rowptr[n + 1].
+// Per segment: (1) structure: the cells kept so far plus every cell the segment touches (row i gains profile(u) \ {i}, row j
+// gains profile(u)) are radix-sorted and de-duplicated; kept cells keep their value, new ones start at 0 -- what a cell that
+// does not exist yet reads in the reference; (2) slot map: per update, in sample order, the index of its cell; (3) values:
+// slim_sequential_kernel<SLOT_CELLS>; (4) cut: rows holding more than K cells keep their K largest.
+typedef unsigned long long u64;
+__device__ __forceinline__ u64 tree_cell_key(int r, int c) { return ((u64)(unsigned)r << 32) | (u64)(unsigned)c; }
+
+// one warp per sample of the segment: 2 * len_u keys at 2 * (off[n] - off[first]).  The (i, i) update is never made (s == i),
+// so its place holds a second copy of (j, i), which the de-duplication removes.
+__global__ void __launch_bounds__(256) slim_tree_touch_kernel(const Params p, const long long* __restrict__ off, u64* out) {
+  const int lane = threadIdx.x & 31;
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  const long long off0 = off[p.first];
+  for (long long g = w; g < p.n_samples; g += n_warps) {
+    const long long n = p.first + g;
+    const int u = p.su[n], i = p.si[n], j = p.sj[n];
+    const int s = p.indptr[u], len = p.indptr[u + 1] - s;
+    u64* o = out + 2 * (off[n] - off0);
+    for (int k = lane; k < len; k += 32) {
+      const int sn = p.indices[s + k];
+      o[k] = sn == i ? tree_cell_key(j, sn) : tree_cell_key(i, sn);
+      o[len + k] = tree_cell_key(j, sn);
+    }
+  }
+}
+
+__global__ void slim_tree_diag_kernel(int n, u64* out) {  // get_S touches (r, r), pyx:349-350
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n) out[r] = tree_cell_key(r, r);
+}
+
+// rowptr of m sorted unique keys: the first cell of row r is the first key whose row is >= r
+__global__ void slim_tree_rowptr_kernel(const u64* __restrict__ key, long long m, int n, long long* rowptr) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t > m) return;
+  const int r = t < m ? (int)(key[t] >> 32) : n;
+  const int rp = t > 0 ? (int)(key[t - 1] >> 32) : -1;
+  for (int q = rp + 1; q <= r; ++q) rowptr[q] = t;
+}
+
+__device__ __forceinline__ long long tree_find(const u64* __restrict__ key, long long lo, long long hi, u64 k) {
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (key[mid] < k) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// the new structure's values: the old value of a cell that existed before, 0 for a new one
+__global__ void slim_tree_carry_kernel(const u64* __restrict__ key, long long m, const u64* __restrict__ old_key,
+                                       const float* __restrict__ old_val, const long long* __restrict__ old_rowptr, float* val) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  const u64 k = key[t];
+  const int r = (int)(k >> 32);
+  const long long lo = old_rowptr[r], hi = old_rowptr[r + 1];
+  const long long q = tree_find(old_key, lo, hi, k);
+  val[t] = q < hi && old_key[q] == k ? old_val[q] : 0.f;
+}
+
+// one warp per sample: the cells of its 2 * len_u updates in the new structure
+__global__ void __launch_bounds__(256) slim_tree_slot_kernel(const Params p, const long long* __restrict__ off, const u64* __restrict__ key,
+                                                             const long long* __restrict__ rowptr, long long* slot_i, long long* slot_j) {
+  const int lane = threadIdx.x & 31;
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  const long long off0 = off[p.first];
+  for (long long g = w; g < p.n_samples; g += n_warps) {
+    const long long n = p.first + g;
+    const int u = p.su[n], i = p.si[n], j = p.sj[n];
+    const int s = p.indptr[u], len = p.indptr[u + 1] - s;
+    const long long q0 = off[n] - off0;
+    const long long ilo = rowptr[i], ihi = rowptr[i + 1], jlo = rowptr[j], jhi = rowptr[j + 1];
+    for (int k = lane; k < len; k += 32) {
+      const int sn = p.indices[s + k];
+      slot_i[q0 + k] = sn == i ? -1 : tree_find(key, ilo, ihi, tree_cell_key(i, sn));
+      slot_j[q0 + k] = tree_find(key, jlo, jhi, tree_cell_key(j, sn));
+    }
+  }
+}
+
+// ---- the cut: rebalance_tree(TopK) pyx:782-802 and the in-place selection inside get_scipy_csr(TopK) pyx:762-763, both
+// through topK_selection_from_list pyx:954-1031.  A row holding more than K cells keeps the K largest by value; the reference
+// sorts the column-ordered list with a stable qsort on the value, so among equal values the HIGHER columns survive:
+// key = (orderable value << 32) | column, keep the K largest keys.  Dropped cells vanish from the structure (a later touch
+// creates them again with value 0).  One warp per row: 8-bit radix select over the 64-bit keys, read from the row in
+// global memory (L1/L2-resident across the passes), stopping at the first digit whose bin is kept whole.
 __device__ __forceinline__ unsigned tree_orderable(float v) {
   const unsigned b = __float_as_uint(v);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
-__global__ void __launch_bounds__(256) slim_tree_prune_kernel(float* S, unsigned char* exists, int n, int K, int touch_diagonal) {
-  typedef unsigned long long u64;
-  constexpr int BINS = 2048;
-  __shared__ int hist[BINS];
-  __shared__ int s_digit, s_need, s_m;
-  const int tid = threadIdx.x;
-  for (int row = blockIdx.x; row < n; row += gridDim.x) {
-    float* Sr = S + (size_t)row * n;
-    unsigned char* Er = exists + (size_t)row * n;
-    if (tid == 0) {
-      s_m = 0;
-      if (touch_diagonal) { Sr[row] = 0.f; Er[row] = 1; }  // get_S: add_value(index, index, -get_value(index, index)), pyx:349-350
+__device__ __forceinline__ u64 tree_cut_key(u64 cell, float v) { return ((u64)tree_orderable(v) << 32) | (cell & 0xFFFFFFFFull); }
+
+constexpr int CUT_THREADS = 256;
+// thr[r]: the row keeps the cells whose cut key is >= thr[r]; cnt[r]: how many
+__global__ void __launch_bounds__(CUT_THREADS) slim_tree_cut_select_kernel(const u64* __restrict__ key, const float* __restrict__ val,
+                                                                           const long long* __restrict__ rowptr, int n, int K, u64* thr,
+                                                                           long long* cnt) {
+  __shared__ unsigned hist[CUT_THREADS / 32][256];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  unsigned* h = hist[wib];
+  const int w = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int n_warps = (int)(((long long)gridDim.x * blockDim.x) >> 5);
+  for (int row = w; row < n; row += n_warps) {
+    const long long lo = rowptr[row], hi = rowptr[row + 1];
+    if (hi - lo <= K) {  // fewer than K cells: the list is returned as it is (pyx:977-978); exactly K: all stay
+      if (lane == 0) { thr[row] = 0ull; cnt[row] = hi - lo; }
+      continue;
     }
-    __syncthreads();
-    int m = 0;
-    for (int c = tid; c < n; c += 256) m += Er[c] != 0;
-    m = __reduce_add_sync(0xffffffffu, m);
-    if ((tid & 31) == 0 && m) atomicAdd(&s_m, m);
-    __syncthreads();
-    m = s_m;
-    __syncthreads();
-    if (K <= 0 || m <= K) continue;  // fewer than K cells: the list is returned as it is (pyx:977-978); exactly K: all stay
     u64 prefix = 0, mask = 0;
-    int need = K;
-    for (int shift = 53; ; shift -= 11) {
-      const int sh = max(shift, 0);
-      const int nb = shift >= 0 ? 11 : 11 + shift;
-      for (int i = tid; i < BINS; i += 256) hist[i] = 0;
-      __syncthreads();
-      for (int c = tid; c < n; c += 256) {
-        if (Er[c]) {
-          const u64 key = (((u64)tree_orderable(Sr[c])) << 32) | (u64)(unsigned)c;
-          if ((key & mask) == prefix) atomicAdd(&hist[(int)((key >> sh) & ((1u << nb) - 1))], 1);
+    unsigned need = (unsigned)K;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+      for (int b = lane; b < 256; b += 32) h[b] = 0u;
+      __syncwarp();
+      for (long long t = lo + lane; t < hi; t += 32) {
+        const u64 k = tree_cut_key(key[t], val[t]);
+        if ((k & mask) == prefix) atomicAdd(&h[(int)((k >> shift) & 255u)], 1u);
+      }
+      __syncwarp();
+      // the bin holding the need-th largest key: lane l owns bins [8l, 8l + 8)
+      unsigned loc = 0;
+#pragma unroll
+      for (int b = 0; b < 8; ++b) loc += h[lane * 8 + b];
+      unsigned incl = loc;  // sum over the lanes >= this one
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned v = __shfl_down_sync(0xffffffffu, incl, o);
+        if (lane + o < 32) incl += v;
+      }
+      const unsigned above = incl - loc;
+      const unsigned owner = __ffs(__ballot_sync(0xffffffffu, above < need && need <= incl)) - 1;
+      int digit = 0;
+      unsigned rest = 0, bin = 0;
+      if (lane == (int)owner) {
+        unsigned cum = above;
+        for (int b = 7; b >= 0; --b) {
+          const unsigned c = h[lane * 8 + b];
+          if (cum + c >= need) { digit = lane * 8 + b; rest = need - cum; bin = c; break; }
+          cum += c;
         }
       }
-      __syncthreads();
-      if (tid == 0) {  // the need-th largest digit
-        int cum = 0;
-        for (int b = (1 << nb) - 1; b >= 0; --b) {
-          const int cnt = hist[b];
-          if (cum + cnt >= need) { s_digit = b; s_need = need - cum; break; }
-          cum += cnt;
-        }
-      }
-      __syncthreads();
-      prefix |= ((u64)s_digit) << sh;
-      mask |= ((u64)((1u << nb) - 1)) << sh;
-      need = s_need;
-      __syncthreads();
-      if (shift <= 0) break;
+      digit = __shfl_sync(0xffffffffu, digit, owner);
+      rest = __shfl_sync(0xffffffffu, rest, owner);
+      bin = __shfl_sync(0xffffffffu, bin, owner);
+      __syncwarp();
+      prefix |= (u64)digit << shift;
+      mask |= 0xFFull << shift;
+      need = rest;
+      if (bin == need) break;  // every key of this bin is kept (the keys are distinct: at the last digit bin == need == 1)
     }
-    for (int c = tid; c < n; c += 256) {
-      if (Er[c]) {
-        const u64 key = (((u64)tree_orderable(Sr[c])) << 32) | (u64)(unsigned)c;
-        if (key < prefix) { Sr[c] = 0.f; Er[c] = 0; }
-      }
-    }
-    __syncthreads();
+    if (lane == 0) { thr[row] = prefix; cnt[row] = K; }  // keys are kept iff (key & mask) >= prefix, i.e. key >= prefix
   }
+}
+
+// the kept cells, in column order, into the new structure at rowptr_new
+__global__ void __launch_bounds__(CUT_THREADS) slim_tree_cut_compact_kernel(const u64* __restrict__ key, const float* __restrict__ val,
+                                                                            const long long* __restrict__ rowptr, int n,
+                                                                            const u64* __restrict__ thr, const long long* __restrict__ rowptr_new,
+                                                                            u64* key_new, float* val_new) {
+  const int lane = threadIdx.x & 31;
+  const int w = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int n_warps = (int)(((long long)gridDim.x * blockDim.x) >> 5);
+  for (int row = w; row < n; row += n_warps) {
+    const long long lo = rowptr[row], hi = rowptr[row + 1];
+    const u64 T = thr[row];
+    long long dst = rowptr_new[row];
+    for (long long b = lo; b < hi; b += 32) {
+      const long long t = b + lane;
+      u64 k = 0; float v = 0.f;
+      bool keep = false;
+      if (t < hi) { k = key[t]; v = val[t]; keep = tree_cut_key(k, v) >= T; }
+      const unsigned bal = __ballot_sync(0xffffffffu, keep);
+      if (keep) {
+        const long long d = dst + __popc(bal & ((1u << lane) - 1u));
+        key_new[d] = k; val_new[d] = v;
+      }
+      dst += __popc(bal);
+    }
+  }
+}
+
+// CSR export of the non-zero off-diagonal cells: per-row counts, then (after a scan) the fill
+__global__ void __launch_bounds__(256) slim_tree_export_kernel(const u64* __restrict__ key, const float* __restrict__ val,
+                                                               const long long* __restrict__ rowptr, int n, long long* cnt,
+                                                               const long long* __restrict__ out_ptr, int* out_idx, float* out_val) {
+  const int lane = threadIdx.x & 31;
+  const int w = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int n_warps = (int)(((long long)gridDim.x * blockDim.x) >> 5);
+  for (int row = w; row < n; row += n_warps) {
+    const long long lo = rowptr[row], hi = rowptr[row + 1];
+    long long dst = out_ptr ? out_ptr[row] : 0;
+    for (long long b = lo; b < hi; b += 32) {
+      const long long t = b + lane;
+      int c = 0; float v = 0.f;
+      bool keep = false;
+      if (t < hi) { c = (int)(unsigned)key[t]; v = val[t]; keep = v != 0.f && c != row; }
+      const unsigned bal = __ballot_sync(0xffffffffu, keep);
+      if (out_ptr && keep) {
+        const long long d = dst + __popc(bal & ((1u << lane) - 1u));
+        out_idx[d] = c; out_val[d] = v;
+      }
+      dst += __popc(bal);
+    }
+    if (!out_ptr && lane == 0) cnt[row] = dst;
+  }
+}
+
+// the raw tree state as the dense view get_S starts from (diagonal 0) into a zeroed n x n buffer
+__global__ void tree_len_kernel(const int* __restrict__ su, const int* __restrict__ indptr, long long n, long long* len) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n) { const int u = su[g]; len[g] = indptr[u + 1] - indptr[u]; }
+  else if (g == n) len[g] = 0;
+}
+
+__global__ void slim_tree_scatter_kernel(const u64* __restrict__ key, const float* __restrict__ val, long long m, int n, float* out) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  const u64 k = key[t];
+  const int r = (int)(k >> 32), c = (int)(unsigned)k;
+  if (r != c) out[(size_t)r * n + c] = val[t];
 }
 
 // expands the stored matrix into the full n x n view get_S returns before its top-K (diagonal zeroed, pyx:345-355;
@@ -444,6 +631,82 @@ __global__ void slim_sample_kernel(const int* __restrict__ indptr, const int* __
 
 using GlibcRand = GlibcRandHost;  // common.cuh
 
+// grows a scratch buffer to at least `count` elements (contents are not kept)
+template <typename T>
+void reserve(DevBuf<T>& b, size_t count) {
+  if (b.n < count) b.alloc(count + count / 4);
+}
+
+// the row-sparse tree state and the per-segment scratch
+struct TreeStore {
+  DevBuf<u64> key, key_new;            // row-sorted cells
+  DevBuf<float> val, val_new;
+  DevBuf<long long> rowptr, rowptr_new;  // n_items + 1
+  long long m = 0;                       // cells in the structure
+  DevBuf<u64> kin, kalt;                 // structure build: cells in, sorted
+  DevBuf<long long> slot_i, slot_j;      // slot map of the running segment
+  DevBuf<long long> len, off;            // per sample of the epoch: profile length and its exclusive prefix sum (n_users + 1)
+  DevBuf<u64> thr;                       // cut: per row, the smallest kept key
+  DevBuf<long long> cnt, count;          // cut / export: per-row counts (n_items + 1); de-duplicated key count
+  DevBuf<unsigned char> tmp;             // CUB scratch
+
+  void* scratch(size_t bytes) { reserve(tmp, std::max<size_t>(bytes, 1)); return tmp.get(); }
+
+  // rowptr_new from cnt[0, n) (cnt[n] = 0)
+  void scan_counts(int n, cudaStream_t st) {
+    size_t tb = 0;
+    B200_CUDA(cudaMemsetAsync(cnt.get() + n, 0, sizeof(long long), st));
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.get(), rowptr_new.get(), n + 1, st));
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(scratch(tb), tb, cnt.get(), rowptr_new.get(), n + 1, st));
+    count_launch();
+  }
+
+  // (1) the structure: the current cells merged with `extra` new keys that `emit` writes after them.  One host read.
+  template <typename Emit>
+  void build(int n, long long extra, cudaStream_t st, Emit emit) {
+    const long long total = m + extra;
+    reserve(kin, (size_t)total); reserve(kalt, (size_t)total); reserve(key_new, (size_t)total); reserve(val_new, (size_t)total);
+    if (m) B200_CUDA(cudaMemcpyAsync(kin.get(), key.get(), sizeof(u64) * (size_t)m, cudaMemcpyDeviceToDevice, st));
+    emit(kin.get() + m);
+    int bits = 1;
+    while ((1ll << bits) <= (long long)n) ++bits;
+    cub::DoubleBuffer<u64> db(kin.get(), kalt.get());
+    size_t tb = 0, tb2 = 0;
+    B200_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, db, total, 0, 32 + bits, st));
+    B200_CUDA(cub::DeviceSelect::Unique(nullptr, tb2, db.Current(), key_new.get(), count.get(), total, st));
+    void* t = scratch(std::max(tb, tb2));
+    B200_CUDA(cub::DeviceRadixSort::SortKeys(t, tb, db, total, 0, 32 + bits, st));
+    B200_CUDA(cub::DeviceSelect::Unique(t, tb2, db.Current(), key_new.get(), count.get(), total, st));
+    long long m_new = 0;
+    B200_CUDA(cudaMemcpyAsync(&m_new, count.get(), sizeof(long long), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    slim_tree_rowptr_kernel<<<div_up(m_new + 1, 256), 256, 0, st>>>(key_new.get(), m_new, n, rowptr_new.get());
+    if (m_new) slim_tree_carry_kernel<<<div_up(m_new, 256), 256, 0, st>>>(key_new.get(), m_new, key.get(), val.get(), rowptr.get(), val_new.get());
+    B200_CUDA(cudaGetLastError());
+    count_launch(4);
+    std::swap(key, key_new); std::swap(val, val_new); std::swap(rowptr, rowptr_new);
+    m = m_new;
+  }
+
+  // (4) rows holding more than K cells keep their K largest.  One host read.
+  void cut(int n, int K, cudaStream_t st) {
+    const int grid = std::min<int>(div_up(n, CUT_THREADS / 32), sm_count() * 16);
+    slim_tree_cut_select_kernel<<<grid, CUT_THREADS, 0, st>>>(key.get(), val.get(), rowptr.get(), n, K, thr.get(), cnt.get());
+    B200_CUDA(cudaGetLastError());
+    scan_counts(n, st);
+    long long m_new = 0;
+    B200_CUDA(cudaMemcpyAsync(&m_new, rowptr_new.get() + n, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    reserve(key_new, (size_t)std::max(m_new, 1ll)); reserve(val_new, (size_t)std::max(m_new, 1ll));
+    slim_tree_cut_compact_kernel<<<grid, CUT_THREADS, 0, st>>>(key.get(), val.get(), rowptr.get(), n, thr.get(), rowptr_new.get(),
+                                                                key_new.get(), val_new.get());
+    B200_CUDA(cudaGetLastError());
+    count_launch(2);
+    std::swap(key, key_new); std::swap(val, val_new); std::swap(rowptr, rowptr_new);
+    m = m_new;
+  }
+};
+
 }  // namespace slim
 }  // namespace b200
 
@@ -463,10 +726,72 @@ struct b200_slim_s {
   bool timed = false;
   int shard_lo = 0, shard_hi = 0;  // column-sharded handle (b200_slim_create_sharded): S is [n_items, shard_hi - shard_lo]
   long long drawn_epoch = -1;      // the epoch whose sample stream is in su / si / sj
-  DevBuf<unsigned char> exists;    // tree mode (b200_slim_enable_tree)
+  TreeStore ts;                    // tree mode (b200_slim_enable_tree)
   bool tree = false;
   int tree_topk = 0;
 };
+
+// the dense S of a non-tree handle, allocated (zeroed: pyx:122-125) by the first call that needs it
+static void ensure_dense_S(b200_slim_s* h, cudaStream_t st) {
+  if (h->S.get()) return;
+  const int n = h->p.n_items;
+  B200_REQUIRE((double)n * (double)n * 4.0 < 1.6e11, "b200_slim_create: dense S does not fit one GPU");
+  const size_t cells = (size_t)n * (size_t)n;
+  h->S.alloc(cells);
+  B200_CUDA(cudaMemsetAsync(h->S.get(), 0, cells * sizeof(float), st));
+  h->p.S = h->S.get();
+}
+
+// pyx:318-319: after sample n (n != 0) with `n % (n_users / 5) == 0` -- a float modulo under language_level=3 -- the rows
+// are cut back to their TopK; the epoch runs as the segments between those points, each on the structure built for it
+static void tree_epoch(b200_slim_s* h, cudaStream_t st) {
+  Params& p = h->p;
+  TreeStore& T = h->ts;
+  const long long n = p.n_users;
+  const int ni = p.n_items;
+  // off[g] = sum of the profile lengths of samples < g
+  tree_len_kernel<<<div_up(n + 1, 256), 256, 0, st>>>(p.su, p.indptr, n, T.len.get());
+  size_t tb = 0;
+  B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, T.len.get(), T.off.get(), n + 1, st));
+  B200_CUDA(cub::DeviceScan::ExclusiveSum(T.scratch(tb), tb, T.len.get(), T.off.get(), n + 1, st));
+  int launches = 2;
+  struct Seg { long long first, last; bool cut; };
+  std::vector<Seg> segs;
+  long long first = 0;
+  const double period = (double)p.n_users / 5.0;
+  for (long long g = 1; g <= n; ++g) {
+    const bool prune_here = g < n && fmod((double)g, period) == 0.0;
+    if (!prune_here && g != n) continue;
+    const long long last = g < n ? g : n - 1;  // the segment ends with sample `last`
+    segs.push_back({first, last, prune_here});
+    first = last + 1;
+    if (g == n) break;
+  }
+  std::vector<long long> bounds(segs.size() + 1);
+  for (size_t k = 0; k < segs.size(); ++k)
+    B200_CUDA(cudaMemcpyAsync(&bounds[k], T.off.get() + segs[k].first, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaMemcpyAsync(&bounds[segs.size()], T.off.get() + n, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaStreamSynchronize(st));
+  for (size_t k = 0; k < segs.size(); ++k) {
+    Params q = p;
+    q.first = segs[k].first; q.n_samples = segs[k].last - segs[k].first + 1; q.chain_pow = segs[k].first > 0;
+    const long long updates = bounds[k + 1] - bounds[k];
+    if (q.n_samples > 0) {  // every sampled profile is non-empty (pyx:443-447): updates > 0
+      const unsigned grid = std::min<long long>(div_up(q.n_samples, 8), (long long)sm_count() * 16);
+      T.build(ni, 2 * updates, st, [&](u64* out) {
+        slim_tree_touch_kernel<<<grid, 256, 0, st>>>(q, T.off.get(), out);
+      });
+      reserve(T.slot_i, (size_t)updates); reserve(T.slot_j, (size_t)updates);
+      slim_tree_slot_kernel<<<grid, 256, 0, st>>>(q, T.off.get(), T.key.get(), T.rowptr.get(), T.slot_i.get(), T.slot_j.get());
+      q.val = T.val.get(); q.slot_i = T.slot_i.get(); q.slot_j = T.slot_j.get();
+      slim_sequential_kernel<SLOT_CELLS><<<1, SEQ_THREADS, 0, st>>>(q);
+      B200_CUDA(cudaGetLastError());
+      launches += 3;
+    }
+    if (segs[k].cut && h->tree_topk > 0) T.cut(ni, h->tree_topk, st);
+  }
+  count_launch(launches - 1);  // the last one is counted by the caller
+}
 
 extern "C" {
 
@@ -479,7 +804,6 @@ int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t
     B200_REQUIRE(out && h_indptr && (nnz == 0 || h_indices), "b200_slim_create: NULL argument");
     B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_slim_create: bad shape");
     B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_slim_create: unknown sgd_mode %d", sgd_mode);
-    B200_REQUIRE((double)n_items * (double)n_items * 4.0 < 1.6e11, "b200_slim_create: dense S does not fit one GPU");
     h = new b200_slim_s();
     Params& p = h->p;
     p.n_users = (int)n_users; p.n_items = (int)n_items; p.symmetric = symmetric != 0; p.sgd_mode = sgd_mode;
@@ -495,10 +819,8 @@ int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t
     B200_CUDA(cudaMemcpy(h->d_indptr.get(), h_indptr, sizeof(int) * ((size_t)n_users + 1), cudaMemcpyHostToDevice));
     if (nnz) B200_CUDA(cudaMemcpy(h->d_indices.get(), h_indices, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice));
     p.indptr = h->d_indptr.get(); p.indices = h->d_indices.get();
-    const size_t cells = (size_t)n_items * (size_t)n_items;
-    h->S.alloc(cells);
-    B200_CUDA(cudaMemset(h->S.get(), 0, cells * sizeof(float)));  // S starts at zero (pyx:122-125)
-    p.S = h->S.get();
+    // S starts at zero (pyx:122-125): a dense S is allocated by the first call that needs it (ensure_dense_S), so a handle
+    // that becomes a tree handle (b200_slim_enable_tree) never holds one
     if (sgd_mode == ADAGRAD || sgd_mode == RMSPROP) {
       h->c.alloc((size_t)n_items); B200_CUDA(cudaMemset(h->c.get(), 0, sizeof(float) * (size_t)n_items)); p.c = h->c.get();
     } else if (sgd_mode == ADAM) {
@@ -665,32 +987,14 @@ int b200_slim_epoch(b200_slim_t h, void* stream) {
                                                         h->su.get(), h->si.get(), h->sj.get());
       count_launch();
     }
+    if (!h->tree) ensure_dense_S(h, st);
     if (h->hogwild) {
       slim_hogwild_kernel<<<sm_count() * 8, 256, 0, st>>>(p);
       if (p.sgd_mode == ADAM) { p.b1_pow *= pow((double)p.beta1, (double)n); p.b2_pow *= pow((double)p.beta2, (double)n); }
     } else if (h->tree) {
-      // pyx:318-319: after sample n (n != 0) with `n % (n_users / 5) == 0` -- a float modulo under language_level=3 -- the rows
-      // are cut back to their TopK; the epoch runs as the segments between those points
-      long long first = 0;
-      int launches = 0;
-      const double period = (double)p.n_users / 5.0;
-      for (long long g = 1; g <= n; ++g) {
-        const bool prune_here = g < n && fmod((double)g, period) == 0.0;
-        if (!prune_here && g != n) continue;
-        const long long last = g < n ? g : n - 1;  // the segment ends with sample `last`
-        Params q = p;
-        q.first = first; q.n_samples = last - first + 1; q.chain_pow = first > 0;
-        if (q.n_samples > 0) { slim_sequential_kernel<<<1, SEQ_THREADS, 0, st>>>(q); ++launches; }
-        if (prune_here && h->tree_topk > 0) {
-          slim_tree_prune_kernel<<<std::min(p.n_items, sm_count() * 8), 256, 0, st>>>(p.S, p.exists, p.n_items, h->tree_topk, 0);
-          ++launches;
-        }
-        first = last + 1;
-        if (g == n) break;
-      }
-      if (launches > 1) count_launch(launches - 1);  // the last one is counted below
+      tree_epoch(h, st);
     } else {
-      slim_sequential_kernel<<<1, SEQ_THREADS, 0, st>>>(p);
+      slim_sequential_kernel<DENSE_CELLS><<<1, SEQ_THREADS, 0, st>>>(p);
     }
     B200_CUDA(cudaGetLastError());
     count_launch();
@@ -715,23 +1019,78 @@ int b200_slim_enable_tree(b200_slim_t h, int topK) {
                  "b200_slim_enable_tree: the tree mode is sequential, non-symmetric (pyx:111-112) and single-GPU");
     B200_REQUIRE(h->epoch == 0 && !h->tree, "b200_slim_enable_tree: call once, before the first epoch");
     B200_REQUIRE(topK >= 0, "b200_slim_enable_tree: topK must be >= 0 (0 = False: rows are never cut)");
-    const size_t cells = (size_t)h->p.n_items * (size_t)h->p.n_items;
-    h->exists.alloc(cells);
-    B200_CUDA(cudaMemset(h->exists.get(), 0, cells));
-    h->p.exists = h->exists.get();
+    const int n = h->p.n_items;
+    TreeStore& T = h->ts;
+    T.rowptr.alloc((size_t)n + 1); T.rowptr_new.alloc((size_t)n + 1);
+    B200_CUDA(cudaMemset(T.rowptr.get(), 0, sizeof(long long) * ((size_t)n + 1)));  // no cells yet
+    T.cnt.alloc((size_t)n + 1); T.thr.alloc((size_t)n); T.count.alloc(1);
+    T.len.alloc((size_t)h->p.n_users + 1); T.off.alloc((size_t)h->p.n_users + 1);
     h->tree = true;
-    h->tree_topk = std::min(topK, h->p.n_items);
+    h->tree_topk = std::min(topK, n);
   });
 }
 
 int b200_slim_tree_prune(b200_slim_t h, int touch_diagonal, void* stream) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr && h->tree, "b200_slim_tree_prune: not a tree-mode handle");
+    cudaStream_t st = (cudaStream_t)stream;
     const int n = h->p.n_items;
-    slim_tree_prune_kernel<<<std::min(n, sm_count() * 8), 256, 0, (cudaStream_t)stream>>>(h->p.S, h->p.exists, n, h->tree_topk,
-                                                                                           touch_diagonal != 0);
+    TreeStore& T = h->ts;
+    if (touch_diagonal)  // get_S: add_value(index, index, -get_value(index, index)), pyx:349-350 (the diagonal is never written)
+      T.build(n, n, st, [&](u64* out) { slim_tree_diag_kernel<<<div_up(n, 256), 256, 0, st>>>(n, out); });
+    if (h->tree_topk > 0) T.cut(n, h->tree_topk, st);
+    B200_CUDA(cudaGetLastError());
+  });
+}
+
+int b200_slim_tree_csr_nnz(b200_slim_t h, int64_t* nnz) {
+  return guarded([&] {
+    B200_REQUIRE(h && nnz && h->tree, "b200_slim_tree_csr_nnz: not a tree-mode handle");
+    const int n = h->p.n_items;
+    TreeStore& T = h->ts;
+    B200_CUDA(cudaDeviceSynchronize());  // no stream argument: the epoch may still run on the caller's stream
+    slim_tree_export_kernel<<<std::min<int>(div_up(n, 8), sm_count() * 16), 256>>>(T.key.get(), T.val.get(), T.rowptr.get(), n,
+                                                                                 T.cnt.get(), nullptr, nullptr, nullptr);
     B200_CUDA(cudaGetLastError());
     count_launch();
+    T.scan_counts(n, 0);
+    long long c = 0;
+    B200_CUDA(cudaMemcpy(&c, T.rowptr_new.get() + n, sizeof(long long), cudaMemcpyDeviceToHost));
+    *nnz = c;
+  });
+}
+
+int b200_slim_tree_csr(b200_slim_t h, int64_t* indptr, int32_t* indices, float* data) {
+  return guarded([&] {
+    B200_REQUIRE(h && indptr && h->tree, "b200_slim_tree_csr: not a tree-mode handle");
+    const int n = h->p.n_items;
+    TreeStore& T = h->ts;
+    const int grid = std::min<int>(div_up(n, 8), sm_count() * 16);
+    B200_CUDA(cudaDeviceSynchronize());
+    slim_tree_export_kernel<<<grid, 256>>>(T.key.get(), T.val.get(), T.rowptr.get(), n, T.cnt.get(), nullptr, nullptr, nullptr);
+    B200_CUDA(cudaGetLastError());
+    T.scan_counts(n, 0);
+    long long c = 0;
+    B200_CUDA(cudaMemcpy(&c, T.rowptr_new.get() + n, sizeof(long long), cudaMemcpyDeviceToHost));
+    B200_REQUIRE(c == 0 || (indices && data), "b200_slim_tree_csr: NULL argument");
+    DevBuf<int> d_idx((size_t)std::max(c, 1ll));
+    DevBuf<float> d_val((size_t)std::max(c, 1ll));
+    slim_tree_export_kernel<<<grid, 256>>>(T.key.get(), T.val.get(), T.rowptr.get(), n, nullptr, T.rowptr_new.get(), d_idx.get(),
+                                           d_val.get());
+    B200_CUDA(cudaGetLastError());
+    count_launch(3);
+    B200_CUDA(cudaMemcpy(indptr, T.rowptr_new.get(), sizeof(long long) * ((size_t)n + 1), cudaMemcpyDeviceToHost));
+    if (c) {
+      B200_CUDA(cudaMemcpy(indices, d_idx.get(), sizeof(int) * (size_t)c, cudaMemcpyDeviceToHost));
+      B200_CUDA(cudaMemcpy(data, d_val.get(), sizeof(float) * (size_t)c, cudaMemcpyDeviceToHost));
+    }
+  });
+}
+
+int b200_slim_tree_cells(b200_slim_t h, int64_t* cells) {
+  return guarded([&] {
+    B200_REQUIRE(h && cells && h->tree, "b200_slim_tree_cells: not a tree-mode handle");
+    *cells = h->ts.m;
   });
 }
 
@@ -755,10 +1114,16 @@ int b200_slim_get_S_dense(b200_slim_t h, float* h_out, float* d_out) {
     DevBuf<float> tmp;
     float* dst = d_out;
     if (!dst) { tmp.alloc(cells); dst = tmp.get(); }
+    if (!h->tree) ensure_dense_S(h, 0);
     // the epoch kernels run on the caller's stream (possibly a non-blocking one) and need not have finished: this entry
     // point has no stream argument, so it waits for the whole device before it reads S on the default stream
     B200_CUDA(cudaDeviceSynchronize());
-    slim_full_kernel<<<div_up((long long)cells, 256), 256>>>(h->p.S, n, h->p.symmetric, dst);
+    if (h->tree) {  // the cells scattered into the zeroed view
+      B200_CUDA(cudaMemset(dst, 0, cells * sizeof(float)));
+      if (h->ts.m) slim_tree_scatter_kernel<<<div_up(h->ts.m, 256), 256>>>(h->ts.key.get(), h->ts.val.get(), h->ts.m, n, dst);
+    } else {
+      slim_full_kernel<<<div_up((long long)cells, 256), 256>>>(h->p.S, n, h->p.symmetric, dst);
+    }
     B200_CUDA(cudaGetLastError());
     count_launch();
     if (h_out) B200_CUDA(cudaMemcpy(h_out, dst, cells * sizeof(float), cudaMemcpyDeviceToHost));

@@ -533,14 +533,19 @@ class SLIMElasticNetRecommender(BaseItemSimilarityMatrixRecommender):
 
 
 class SLIM_BPR_Cython(BaseItemSimilarityMatrixRecommender, Incremental_Training_Early_Stopping):
-    """SLIM_BPR/Cython/SLIM_BPR_Cython.py:48-183 with S dense on the device.  `train_with_sparse_weights=None` (the reference's
-    RAM-based auto selection, :85-103) resolves to the dense mode; True runs the tree mode's semantics (slim_bpr_epoch.py)."""
+    """SLIM_BPR/Cython/SLIM_BPR_Cython.py:48-183 with S on the device: dense, or row-sparse in the tree mode
+    (train_with_sparse_weights=True, slim_bpr_epoch.py).  `train_with_sparse_weights=None` is the device counterpart of the
+    reference's RAM-based auto selection (:85-103): the tree mode when the dense mode's 8 * n_items^2 bytes exceed the free
+    device memory (slim_bpr_epoch.sparse_weights_for_device), the dense mode otherwise."""
     RECOMMENDER_NAME = "SLIM_BPR_Recommender"
 
     def fit(self, epochs=300, positive_threshold_BPR=None, train_with_sparse_weights=None, symmetric=True, random_seed=None,
             lambda_i=0.0, lambda_j=0.0, learning_rate=1e-4, topK=200, sgd_mode="adagrad", gamma=0.995, beta_1=0.9,
             beta_2=0.999, sampler="glibc", hogwild=False, **earlystopping_kwargs):
-        from .slim_bpr_epoch import SLIM_BPR_Cython_Epoch, similarityMatrixTopK
+        import torch
+        from .slim_bpr_epoch import SLIM_BPR_Cython_Epoch, similarityMatrixTopK, sparse_weights_for_device
+        if train_with_sparse_weights is None:
+            train_with_sparse_weights = sparse_weights_for_device(None, self.n_items, torch.cuda.mem_get_info()[0], symmetric)
         self.symmetric, self.train_with_sparse_weights = symmetric, bool(train_with_sparse_weights)
         URM_train_positive = self.URM_train.copy()
         if positive_threshold_BPR is not None:  # SLIM_BPR_Cython.py:112-116

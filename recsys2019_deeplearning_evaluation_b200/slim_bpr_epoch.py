@@ -3,9 +3,10 @@ equivalent of Base/Recommender_utils.py:55-122 `similarityMatrixTopK` for dense 
 
 Same constructor signature as pyx:88-94, `epochIteration_Cython()`, `get_S()`, `_dealloc()`.  Extra keywords:
 sampler="glibc"|"philox", hogwild=False (see mf_epoch.py).  S is dense fp32 in HBM, optionally symmetric (lower-triangular
-addressing).  `train_with_sparse_weights=True` (Sparse_Matrix_Tree_CSR, pyx:579-1031) keeps the SEMANTICS of the tree mode on
-the dense array -- which cells exist, the periodic rebalance_tree(TopK) during the epoch (pyx:318-319), the in-place top-K
-of get_S (pyx:762-763) -- not its memory footprint (for catalogues whose dense S does not fit: dist.ShardedSLIM_BPR)."""
+addressing).  `train_with_sparse_weights=True` (Sparse_Matrix_Tree_CSR, pyx:579-1031) is the tree mode with its semantics --
+which cells exist, the periodic rebalance_tree(TopK) during the epoch (pyx:318-319), the in-place top-K of get_S
+(pyx:762-763) -- and its memory footprint: S is row-sparse on the device, its size follows the cells the rows hold, so a
+catalogue whose dense S does not fit trains on one GPU."""
 import ctypes
 
 import numpy as np
@@ -48,6 +49,16 @@ def similarityMatrixTopK(item_weights, k=100, verbose=False):
     assert t.shape[0] == t.shape[1], "selectTopK: ItemWeights is not a square matrix"
     t = t.to(device="cuda", dtype=torch.float32).contiguous()
     return dense_topk_to_sparse(t, t.shape[0], k, along_columns=True, mode=0).tocsc()
+
+
+def sparse_weights_for_device(train_with_sparse_weights, n_items, free_bytes, symmetric=True):
+    """The `train_with_sparse_weights` an epoch object gets.  True / False are kept; None (SLIM_BPR_Cython.py:85-103, where
+    the reference picks the tree mode when the dense S would not fit in RAM) is the device counterpart of that rule, with a
+    different threshold: the dense mode needs S (n_items^2 fp32, allocated in full even when symmetric) plus get_S's
+    n_items^2 fp32 buffer, so the tree mode is picked when 8 * n_items^2 bytes exceed the free device memory."""
+    if train_with_sparse_weights is not None:
+        return bool(train_with_sparse_weights)
+    return 8 * int(n_items) * int(n_items) > int(free_bytes)
 
 
 class SLIM_BPR_Cython_Epoch:
@@ -100,20 +111,30 @@ class SLIM_BPR_Cython_Epoch:
         _lib.check(self._lib.b200_slim_get_S_dense(self._h, _lib.ptr(out), None))
         return out
 
+    def tree_cells(self):
+        """Tree mode: the cells the row-sparse structure holds now (12 bytes of device memory each)."""
+        c = ctypes.c_int64()
+        _lib.check(self._lib.b200_slim_tree_cells(self._h, ctypes.byref(c)))
+        return int(c.value)
+
     def get_S(self):
         """pyx:340-388: diagonal zeroed, then per ROW top-K -- symmetric: K largest over all cells, zeros dropped
         (Triangular_Matrix.get_scipy_csr, pyx:1335-1415); dense: similarityMatrixTopK(S.T).T (pyx:371,386)."""
         import torch
         n = self.n_items
-        d = torch.empty((n, n), dtype=torch.float32, device="cuda")
         if self.train_with_sparse_weights:
-            # pyx:349-350 touches the diagonal cells, get_scipy_csr(TopK) (pyx:737-778) cuts every row that holds >= TopK cells
-            # IN PLACE and emits the non-zero cells that are left; topK=False emits them all
+            # pyx:349-350 touches the diagonal cells, get_scipy_csr(TopK) (pyx:737-778) cuts every row that holds more than
+            # TopK cells IN PLACE and emits the non-zero cells that are left; topK=False emits them all.  No n x n buffer.
             _lib.check(self._lib.b200_slim_tree_prune(self._h, 1, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
-            _lib.check(self._lib.b200_slim_get_S_dense(self._h, None, d.data_ptr()))
-            if self.topK:  # every row now holds <= topK non-zero cells: the top-K kernel emits exactly them, CSR built on the device
-                return dense_topk_to_sparse(d, n, self.topK, along_columns=False, mode=0).astype(np.float64)
-            return sps.csr_matrix(d.cpu().numpy().astype(np.float64))
+            nnz = ctypes.c_int64()
+            _lib.check(self._lib.b200_slim_tree_csr_nnz(self._h, ctypes.byref(nnz)))
+            indptr = np.empty(n + 1, np.int64)
+            indices = np.empty(max(nnz.value, 1), np.int32)
+            data = np.empty(max(nnz.value, 1), np.float32)
+            _lib.check(self._lib.b200_slim_tree_csr(self._h, _lib.ptr(indptr), _lib.ptr(indices), _lib.ptr(data)))
+            nz = nnz.value
+            return sps.csr_matrix((data[:nz].astype(np.float64), indices[:nz], indptr), shape=(n, n))
+        d = torch.empty((n, n), dtype=torch.float32, device="cuda")
         _lib.check(self._lib.b200_slim_get_S_dense(self._h, None, d.data_ptr()))
         if self.topK is False:
             if self.symmetric or self.final_model_sparse_weights:

@@ -1,7 +1,8 @@
 """Timings of the SURVEY.md 8(f).4 trainers at BASELINE shapes, one JSON object per line, with the CPU side timed beside them
 on a bounded sample (the oracle port for the SGD trainers, scikit-learn's ElasticNet -- what the reference calls -- for SLIM
 ElasticNet).
-    python tools/next_rows_bench.py [--no-c4]
+    python tools/next_rows_bench.py [--no-c4] [--no-c5] [--only-slim-tree]
+--only-slim-tree runs the SLIM-BPR tree-mode legs alone (C2, then the C5 shape unless --no-c5).
 """
 import json, os, sys, time, warnings
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -28,6 +29,64 @@ nu, ni = X2.shape
 emit(bench="URM C2", shape=list(X2.shape), nnz=int(X2.nnz))
 
 only_asy = "--only-asy" in sys.argv
+only_tree = "--only-slim-tree" in sys.argv
+
+
+def gpu_info():
+    import subprocess
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                              text=True, timeout=30).stdout.strip()
+    except Exception as ex:  # noqa
+        return repr(ex)
+
+
+def slim_tree_c2():
+    # ---- SLIM-BPR tree mode, C2 (adagrad, topK 200: the reference's configs[1] hyper-parameters, sparse-weights mode)
+    kws = dict(train_with_sparse_weights=True, learning_rate=1e-4, li_reg=0.0, lj_reg=0.0, topK=200, sgd_mode="adagrad", random_seed=42)
+    g = SLIM_BPR_Cython_Epoch(sps.csr_matrix(X2), **kws)
+    g.epochIteration_Cython(); sync()
+    ts = []
+    for _ in range(5):
+        t = time.perf_counter(); g.epochIteration_Cython(); sync(); ts.append(time.perf_counter() - t)
+    t = time.perf_counter(); S = g.get_S(); t_get = time.perf_counter() - t
+    emit(bench="SLIM-BPR tree mode epoch C2", samples=nu, seconds_median=float(np.median(ts)), samples_per_s=nu / float(np.median(ts)), get_S_s=t_get,
+         nnz=int(S.nnz), cuts_per_epoch=4, epochs_s=ts, gpu=gpu_info())
+    g._dealloc()
+
+
+def slim_tree_c5():
+    # ---- SLIM-BPR tree mode at the C5 shape (1 M users x 200 K items, K = 200, adagrad): the dense S would be 160 GB.  One
+    # epoch timed plain, one under torch.profiler for the split: structure build (key emission, sort, unique, rowptr, value
+    # carry, slot map) / the sequential kernel / the cuts
+    X5 = synth_config("C5", values="ratings")
+    kws = dict(train_with_sparse_weights=True, learning_rate=1e-4, topK=200, sgd_mode="adagrad", random_seed=42)
+    g = SLIM_BPR_Cython_Epoch(sps.csr_matrix(X5), **kws)
+    sync(); t = time.perf_counter(); g.epochIteration_Cython(); sync(); t_epoch = time.perf_counter() - t
+    cells_epoch = g.tree_cells()
+    from torch.profiler import profile, ProfilerActivity
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        t = time.perf_counter(); g.epochIteration_Cython(); sync(); t_prof = time.perf_counter() - t
+    split = {"build": 0.0, "sequential": 0.0, "cut": 0.0}
+    for ev in prof.key_averages():
+        us = ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
+        if us <= 0:
+            continue
+        key = "sequential" if "slim_sequential_kernel" in ev.key else ("cut" if "slim_tree_cut" in ev.key else "build")
+        split[key] += us * 1e-6
+    t = time.perf_counter(); S = g.get_S(); t_get = time.perf_counter() - t
+    emit(bench="SLIM-BPR tree mode epoch C5 shape", shape=list(X5.shape), nnz_urm=int(X5.nnz), samples=int(X5.shape[0]), epoch_s=t_epoch,
+         epoch_profiled_s=t_prof, device_s_build=split["build"], device_s_sequential=split["sequential"], device_s_cut=split["cut"],
+         get_S_s=t_get, cells_after_epoch=cells_epoch, cells_after_get_S=g.tree_cells(), structure_bytes_after_epoch=12 * cells_epoch,
+         nnz=int(S.nnz), gpu=gpu_info())
+    g._dealloc()
+
+
+if only_tree:
+    slim_tree_c2()
+    if "--no-c5" not in sys.argv:
+        slim_tree_c5()
+    sys.exit(0)
 if only_asy:
     for mode in ("sgd", "adagrad", "adam"):
         for f in (32, 128):
@@ -90,17 +149,9 @@ o = MFOracle(Xs, n_factors=32, algorithm_name="ASY_SVD", batch_size=1, learning_
 t = time.perf_counter(); n = o.epochIteration_Cython(); dt = time.perf_counter() - t
 emit(bench="AsySVD C port of the reference loop (CPU, 1 thread), 600 users of C2", samples=int(n), seconds=dt, samples_per_s=n / dt)
 
-# ---- SLIM-BPR tree mode, C2 (adagrad, topK 200: the reference's configs[1] hyper-parameters, sparse-weights mode)
-kws = dict(train_with_sparse_weights=True, learning_rate=1e-4, li_reg=0.0, lj_reg=0.0, topK=200, sgd_mode="adagrad", random_seed=42)
-g = SLIM_BPR_Cython_Epoch(sps.csr_matrix(X2), **kws)
-g.epochIteration_Cython(); sync()
-ts = []
-for _ in range(5):
-    t = time.perf_counter(); g.epochIteration_Cython(); sync(); ts.append(time.perf_counter() - t)
-t = time.perf_counter(); S = g.get_S(); t_get = time.perf_counter() - t
-emit(bench="SLIM-BPR tree mode epoch C2", samples=nu, seconds_median=float(np.median(ts)), samples_per_s=nu / float(np.median(ts)), get_S_s=t_get, nnz=int(S.nnz),
-     cuts_per_epoch=4)
-g._dealloc()
+slim_tree_c2()
+if "--no-c5" not in sys.argv:
+    slim_tree_c5()
 
 # ---- SLIM ElasticNet, C4 (480 K x 17.7 K): the Gram matrix is the EASE_R one; 3 * n * 4 bytes = 208 KB of shared memory per CTA
 if "--no-c4" not in sys.argv:
