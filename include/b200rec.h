@@ -324,7 +324,8 @@ int b200_score_mf_device(const int32_t* d_users, int n_users_block, const float*
 /* -inf on items outside d_items_keep (nullable, n_items bytes) and on the seen items of each user (nullable URM) */
 int b200_score_mask_device(const int32_t* d_users, int n_users_block, const int32_t* d_urm_ptr, const int32_t* d_urm_idx,
                            const unsigned char* d_items_keep, int n_items, float* d_scores, void* stream);
-/* per row the `cutoff` (<= 1024) best items, best first, ties by ascending item index: [n_rows, cutoff] tables */
+/* per row the `cutoff` (<= 1024) best items in the order of np.lexsort((arange, -s)): +inf, finite scores descending,
+ * -inf, then NaN; ties (-0 == +0) by ascending item index.  [n_rows, cutoff] tables; past the end of a row -1 / -inf */
 int b200_score_topn_device(const float* d_scores, int n_rows, int n_items, int cutoff, int32_t* d_items,
                            float* d_item_scores, void* stream);
 
@@ -390,8 +391,10 @@ int b200_feature_weighting_device(int mode, int n_users, int n_items, int64_t nn
  * Evaluation inner loop on the device  (SURVEY.md 8(f).1)
  * replaces  Base/Evaluation/Evaluator.py:305-388 _compute_metrics_on_recommendation_list and the per-user metric
  *           functions of Base/Evaluation/metrics.py (:65-287, :615-716) for one block of users.
- * d_rec_items / d_rec_scores: the [n_block, max_cutoff] tables of b200_score_topn_device (a -inf score ends a list);
- * test URM in CSR with sorted indices; d_cutoffs: n_cutoffs ascending list lengths; d_idcg: [n_users, n_cutoffs] ideal
+ * d_rec_items / d_rec_scores: the [n_block, max_cutoff] tables of b200_score_topn_device; entries whose score is not
+ * finite (+inf, -inf, NaN) are skipped, and the finite ones, in table order, form the list (BaseRecommender.py:203-207);
+ * test URM in CSR with sorted indices; d_cutoffs: n_cutoffs >= 1 list lengths in any order, no cap on their number (each
+ * above max_cutoff counts the whole list); d_idcg: [n_users, n_cutoffs] ideal
  * DCG of every user (metrics.py:268); d_item_novelty / d_item_pop_norm: the per-item terms of Novelty (:651) and
  * AveragePopularity (:686).  Accumulates (atomically, across calls) into d_acc [n_cutoffs, B200_EVAL_NACC] doubles
  * and the per-item counters d_rec_count / d_hit_count [n_cutoffs, n_items] (times recommended / recommended and

@@ -7,11 +7,12 @@
 // AveragePopularity :670, and the per-item recommendation counters every global-distribution metric is a function of
 // (_Global_Item_Distribution_Counter :289, Coverage_Item_HIT :346, Diversity_MeanInterList :778).
 //
-// Input: the [n_block, max_cutoff] item table of b200_score_topn_device (a -inf score ends the list, BaseRecommender.py
-// :203-207 drops those entries) and the test URM in CSR on the device.  One warp per user: the hit flag / gain of every
-// list position is found by a binary search in the user's sorted test row, hits are prefix-summed with ballots, then
-// every cutoff reduces its prefix of the list.  Sums go to fp64 accumulators with atomics; nothing returns to the host
-// until the evaluation ends.  HBM-bound on the list table (4 B per position) and the test rows.
+// Input: the [n_block, max_cutoff] item table of b200_score_topn_device (entries whose score is not finite are not
+// recommendations, BaseRecommender.py:203-207 drops them) and the test URM in CSR on the device.  One warp per user: the
+// hit flag / gain of every recommendation is found by a binary search in the user's sorted test row, hits are
+// prefix-summed with ballots, then every cutoff (any number, any order) reduces its prefix of the list.  Sums go to fp64
+// accumulators with atomics; nothing returns to the host until the evaluation ends.  HBM-bound on the list table (4 B per
+// position) and the test rows.
 #include "common.cuh"
 
 namespace b200 {
@@ -36,15 +37,14 @@ __global__ void __launch_bounds__(WARPS * 32) metrics_kernel(
   const int n_test = te - ts;
   const int* row = rec + (size_t)b * max_cutoff;
   const float* srow = rec_score + (size_t)b * max_cutoff;
-  // ---- phase 1: hit / gain per position, running hit count, list length (valid entries form a prefix)
+  // ---- phase 1: hit / gain per recommendation, running hit count, list length.  Only entries with a finite score are
+  // recommendations (BaseRecommender.py:203-207 drops the rest from the first max_cutoff positions); they are compacted
+  // to positions 0..len-1 in table order, so +inf entries before them and NaN / -inf entries among them take no position.
   int carry = 0, len = 0;
   for (int p0 = 0; p0 < max_cutoff; p0 += 32) {
     const int p = p0 + lane;
     int item = -1;
-    if (p < max_cutoff) {
-      item = row[p];
-      if (!(srow[p] > -3.0e38f)) item = -1;  // -inf score: not a recommendation (BaseRecommender.py:203-207)
-    }
+    if (p < max_cutoff && isfinite(srow[p])) item = row[p];
     int hit = 0;
     float gain = 0.f;
     if (item >= 0) {
@@ -57,12 +57,13 @@ __global__ void __launch_bounds__(WARPS * 32) metrics_kernel(
     }
     const unsigned valid_mask = __ballot_sync(0xffffffffu, item >= 0);
     const unsigned hit_mask = __ballot_sync(0xffffffffu, hit);
-    len += __popc(valid_mask);
-    if (p < max_cutoff) {
-      s_item[w][p] = item;
-      s_gain[w][p] = gain;
-      s_cum[w][p] = (unsigned short)(carry + __popc(hit_mask & (0xffffffffu >> (31 - lane))));
+    if (item >= 0) {
+      const int q = len + __popc(valid_mask & ((1u << lane) - 1u));  // position among the recommendations
+      s_item[w][q] = item;
+      s_gain[w][q] = gain;
+      s_cum[w][q] = (unsigned short)(carry + __popc(hit_mask & (0xffffffffu >> (31 - lane))));
     }
+    len += __popc(valid_mask);
     carry += __popc(hit_mask);
   }
   __syncwarp();
@@ -142,7 +143,7 @@ int b200_eval_accumulate_device(const int32_t* d_users, int n_block, const int32
                      d_item_novelty && d_item_pop_norm && d_acc && d_rec_count && d_hit_count,
                  "b200_eval_accumulate: NULL argument");
     B200_REQUIRE(max_cutoff >= 1 && max_cutoff <= eval::MAXCUT, "b200_eval_accumulate: max_cutoff must be in [1, %d]", eval::MAXCUT);
-    B200_REQUIRE(n_cutoffs >= 1 && n_cutoffs <= 16 && n_items > 0 && n_block >= 0, "b200_eval_accumulate: bad shape");
+    B200_REQUIRE(n_cutoffs >= 1 && n_items > 0 && n_block >= 0, "b200_eval_accumulate: bad shape");
     if (n_block == 0) return;
     eval::metrics_kernel<<<div_up(n_block, eval::WARPS), eval::WARPS * 32, 0, (cudaStream_t)stream>>>(
         d_users, n_block, d_rec_items, d_rec_scores, max_cutoff, d_test_ptr, d_test_idx, d_test_val, d_cutoffs, n_cutoffs, d_idcg,

@@ -76,15 +76,19 @@ __global__ void __launch_bounds__(256) mf_scores_kernel(const int* __restrict__ 
   }
 }
 
+// 32 x 32 tiles; the row tiles are walked grid-stride along y, whose grid size is capped at 65 535
 __global__ void transpose_kernel(const float* __restrict__ in, int rows, int cols, float* out) {
   __shared__ float tile[32][33];
-  const int x = blockIdx.x * 32 + threadIdx.x, y0 = blockIdx.y * 32;
-  for (int k = threadIdx.y; k < 32; k += blockDim.y)
-    if (x < cols && y0 + k < rows) tile[k][threadIdx.x] = in[(size_t)(y0 + k) * cols + x];
-  __syncthreads();
-  const int ox = blockIdx.y * 32 + threadIdx.x, oy0 = blockIdx.x * 32;
-  for (int k = threadIdx.y; k < 32; k += blockDim.y)
-    if (ox < rows && oy0 + k < cols) out[(size_t)(oy0 + k) * rows + ox] = tile[threadIdx.x][k];
+  const int x = blockIdx.x * 32 + threadIdx.x, oy0 = blockIdx.x * 32;
+  for (int y0 = blockIdx.y * 32; y0 < rows; y0 += gridDim.y * 32) {
+    for (int k = threadIdx.y; k < 32; k += blockDim.y)
+      if (x < cols && y0 + k < rows) tile[k][threadIdx.x] = in[(size_t)(y0 + k) * cols + x];
+    __syncthreads();
+    const int ox = y0 + threadIdx.x;
+    for (int k = threadIdx.y; k < 32; k += blockDim.y)
+      if (ox < rows && oy0 + k < cols) out[(size_t)(oy0 + k) * rows + ox] = tile[threadIdx.x][k];
+    __syncthreads();
+  }
 }
 
 // scores[b, seen items of users[b]] = -inf (BaseRecommender.py:164-169); one warp per user
@@ -103,9 +107,12 @@ __global__ void mask_items_kernel(const unsigned char* __restrict__ keep, int n_
   if (!keep[g % n_items]) scores[g] = -INFINITY;
 }
 
+// Unsigned key in the order of np.lexsort((arange, -s)), the host ranking (BaseRecommender.py:189-196): +inf, finite
+// values descending, -inf, then NaN of either sign (key 0, below -inf's 0x007FFFFF).  -0 and +0 are one value, so they
+// tie and fall back to the item index.
 __device__ __forceinline__ unsigned orderable(float v) {
-  const unsigned b = __float_as_uint(v);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+  const unsigned b = __float_as_uint(v == 0.f ? 0.f : v);
+  return v != v ? 0u : (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
 // per row the `cutoff` best items, best first (BaseRecommender.py:189-196); ties -> ascending item index.
@@ -204,7 +211,8 @@ int b200_score_spmm_device(const int32_t* d_users, int n_users_block, const int3
 int b200_transpose_device(const float* d_in, int rows, int cols, float* d_out, void* stream) {
   return guarded([&] {
     B200_REQUIRE(d_in && d_out && rows > 0 && cols > 0, "b200_transpose: bad argument");
-    transpose_kernel<<<dim3(div_up(cols, 32), div_up(rows, 32)), dim3(32, 8), 0, (cudaStream_t)stream>>>(d_in, rows, cols, d_out);
+    transpose_kernel<<<dim3(div_up(cols, 32), std::min(div_up(rows, 32), 65535u)), dim3(32, 8), 0, (cudaStream_t)stream>>>(
+        d_in, rows, cols, d_out);
     B200_CUDA(cudaGetLastError());
     count_launch();
   });
@@ -221,10 +229,16 @@ int b200_score_mf_device(const int32_t* d_users, int n_users_block, const float*
     if (n_users_block == 0) return;
     const size_t smem = (size_t)UT * n_factors * sizeof(float);
     B200_REQUIRE(smem <= 48 * 1024, "b200_score_mf: n_factors=%d too large", n_factors);
-    mf_scores_kernel<<<dim3(div_up(n_items, 256), div_up(n_users_block, UT)), 256, smem, (cudaStream_t)stream>>>(
-        d_users, n_users_block, d_user_factors, d_item_factors_T, n_factors, n_items, d_user_bias, d_item_bias, d_global_bias, d_out);
-    B200_CUDA(cudaGetLastError());
-    count_launch();
+    // gridDim.y (UT users per block) is capped at 65 535: larger user arrays take several launches
+    const int per_launch = 65535 * UT;
+    for (int b0 = 0; b0 < n_users_block; b0 += per_launch) {
+      const int nb = std::min(per_launch, n_users_block - b0);
+      mf_scores_kernel<<<dim3(div_up(n_items, 256), div_up(nb, UT)), 256, smem, (cudaStream_t)stream>>>(
+          d_users + b0, nb, d_user_factors, d_item_factors_T, n_factors, n_items, d_user_bias, d_item_bias, d_global_bias,
+          d_out + (size_t)b0 * n_items);
+      B200_CUDA(cudaGetLastError());
+      count_launch();
+    }
   });
 }
 

@@ -155,8 +155,9 @@ class BaseRecommender(object):
         return scores
 
     def _topn_device(self, scores, cutoff):
-        """[B, cutoff] int32 items / float32 scores CUDA tensors, best first, ties by ascending item id (cutoff <= 1024);
-        lists end where the score is -inf."""
+        """[B, cutoff] int32 items / float32 scores CUDA tensors (cutoff <= 1024) in the order of
+        np.lexsort((arange, -s)): +inf, finite scores descending, -inf, NaN, ties by ascending item id.  Entries whose
+        score is not finite are not recommendations."""
         import torch
         items = torch.empty((scores.shape[0], cutoff), dtype=torch.int32, device=scores.device)
         vals = torch.empty((scores.shape[0], cutoff), dtype=torch.float32, device=scores.device)
