@@ -26,6 +26,7 @@ extern "C" {
 #define B200_E_CUDA (-2)    /* CUDA runtime / launch failure (RuntimeError) */
 #define B200_E_NOMEM (-3)   /* device or host allocation failed */
 #define B200_E_UNSUPPORTED (-4)
+#define B200_E_SINGULAR (-5)    /* the matrix to invert is exactly singular (np.linalg.LinAlgError) */
 
 const char* b200_last_error(void);
 int b200_version(void);
@@ -347,9 +348,24 @@ int b200_slim_enet_device(const float* d_G, const float* d_diag, int n_items, in
  * replaces  EASE_R/EASE_R_Recommender.py:55-69
  * ------------------------------------------------------------------------------------------------ */
 /* In-place inverse of a symmetric positive definite matrix on the device through a blocked Cholesky factorisation
- * (replaces np.linalg.inv, EASE_R_Recommender.py:65).  d_A: [n_pad, n_pad] row-major fp32, n_pad a multiple of 128
- * (pad with an identity block); d_work: 2 * n_pad * n_pad floats. */
+ * (replaces np.linalg.inv, EASE_R_Recommender.py:65, for positive definite Grams).  d_A: [n_pad, n_pad] row-major fp32,
+ * n_pad a multiple of 128 (pad with an identity block); d_work: 2 * n_pad * n_pad floats.  A matrix that is not positive
+ * definite is an error (B200_E_INVALID). */
 int b200_spd_inverse_device(float* d_A, int n_pad, float* d_work, void* stream);
+/* In-place inverse of a general non-singular matrix on the device in fp64 (np.linalg.inv: LAPACK dgetrf + dgetri):
+ * blocked LU with partial pivoting (largest |a|, lowest row on ties), then A^-1 = U^-1 L^-1 P, every O(n^3) step on the
+ * FP64 tensor cores; about 2 n^3 flops.  d_A: [n_pad, n_pad] row-major fp64, n_pad a multiple of 128 (pad with an identity
+ * block; it stays an identity block); d_work: 2 * n_pad * n_pad doubles.  An exactly zero pivot returns B200_E_SINGULAR
+ * ("singular matrix (zero pivot at column j)", j 0-based), the condition under which LAPACK reports info > 0. */
+int b200_lu_inverse_device(double* d_A, int n_pad, double* d_work, void* stream);
+/* TEST HOOK: the fp64 tensor-core GEMM of the LU inverse (row-major device pointers, lda / ldb / ldc even, 16-byte aligned):
+ * kind 0: C = alpha A B + beta C (A [M,K], B [K,N]);
+ * kind 1: batched, M / 128 products C_b = alpha A_b B_b + beta C_b of A_b = rows [128 b, 128 b + 128) of A, B_b = rows
+ *         [K b, K b + K) of B (B has M / 128 * K rows) and C_b = rows [128 b, 128 b + 128) of C;
+ * kind 2: C = alpha A B + beta C with k >= max(row block, column block) only (M == N == K; the U^-1 L^-1 product).
+ * M, N multiples of 128, K a multiple of 16. */
+int b200_debug_dgemm_device(int kind, int M, int N, int K, double alpha, const double* d_A, int lda, const double* d_B, int ldb,
+                            double beta, double* d_C, int ldc, void* stream);
 /* TEST HOOK: one GEMM of the blocked inverse through tensor-core GEMM version 1 (the default, gemm_tc.cuh) or 2
  * (gemm_tc2.cuh: pre-packed hi/lo TF32 operands fed by cp.async.bulk, opt-in via B200REC_GEMM=2).
  * kind 0: C = alpha A B^T + beta C (A [M,K], B [N,K]); kind 1: C = alpha A B + beta C (B [K,N]);
@@ -359,7 +375,11 @@ int b200_debug_gemm_device(int version, int kind, int M, int N, int K, float alp
                            const float* d_B, int ldb, float beta, float* d_C, int ldc, void* stream);
 /* d_G: dense [n_items, n_items] Gram block X^T X (b200_sim_compute_dense_device with normalize=0, shrink=0); the
  * diagonal is replaced by item popularity (stored-entry count per column of the URM, :62-63) + l2_norm, the matrix is
- * inverted, and B[i, j] = P[i, j] / (-P[j, j]), B[j, j] = 0 is written to h_B (host) and/or d_B (device). */
+ * inverted, and B[i, j] = P[i, j] / (-P[j, j]), B[j, j] = 0 is written to h_B (host) and/or d_B (device).
+ * The inverse is the fp32 blocked Cholesky of b200_spd_inverse_device; when that meets a non-positive pivot (explicit
+ * ratings: the popularity diagonal is below sum r^2, so G + diag can be indefinite) the fp32 workspaces are freed and the
+ * same matrix is inverted by b200_lu_inverse_device in fp64, B computed in fp64 and rounded once to fp32.  Device memory of
+ * that path: 3 * 8 * n_pad^2 bytes besides d_G and d_B.  A singular matrix returns B200_E_SINGULAR. */
 int b200_ease_from_gram_device(const float* d_G, int n_items, const int32_t* d_urm_indices, int64_t nnz, float l2_norm,
                                float* h_B, float* d_B, void* stream);
 

@@ -99,6 +99,9 @@ SIGNATURES = {
     "b200_spd_inverse_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void]),
     "b200_debug_gemm_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_void,
                                               ctypes.c_int, c_void, ctypes.c_int, ctypes.c_float, c_void, ctypes.c_int, c_void]),
+    "b200_lu_inverse_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void]),
+    "b200_debug_dgemm_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, c_void,
+                                               ctypes.c_int, c_void, ctypes.c_int, ctypes.c_double, c_void, ctypes.c_int, c_void]),
     "b200_ease_from_gram_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, ctypes.c_int64, ctypes.c_float, c_void, c_void, c_void]),
     "b200_feature_weighting_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int64, c_void, c_void, c_void,
                                                      ctypes.c_float, ctypes.c_float, c_void]),
@@ -140,6 +143,8 @@ def check(rc):
         raise ValueError(msg)
     if rc == -3:
         raise MemoryError(msg)
+    if rc == -5:
+        raise np.linalg.LinAlgError(msg)
     raise B200Error("libb200rec error %d: %s" % (rc, msg))
 
 

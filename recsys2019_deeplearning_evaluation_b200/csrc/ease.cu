@@ -2,17 +2,20 @@
 //
 // Replaces EASE_R/EASE_R_Recommender.py:55-69:  G = X^T X (through Compute_Similarity, shrink 0, normalize False,
 // topK = n_items), G[diag] = item_popularity + l2_norm (nnz count per column, :62-63), P = inv(G) (np.linalg.inv on
-// float32 -> LAPACK sgetrf/sgetri), B = P / (-diag P) (column j divided by -P_jj), B[diag] = 0.
+// float32: LAPACK dgetrf/dgetri in float64, rounded to float32), B = P / (-diag P) (column j divided by -P_jj), B[diag] = 0.
 //
-// The Gram matrix comes from the dense mode of the similarity kernel (csrc/sim_topk.cu).  G is symmetric positive
-// definite (l2_norm > 0), so the inverse is formed through a blocked Cholesky factorisation instead of LU:
+// The Gram matrix comes from the dense mode of the similarity kernel (csrc/sim_topk.cu).  When G is symmetric positive
+// definite (binary data, or a large enough l2_norm) the inverse is formed through a blocked Cholesky factorisation:
 //   1. right-looking blocked Cholesky, NB = 128: diagonal block factor + its inverse in one CTA (shared memory),
 //      panel L21 = A21 inv(L11)^T and trailing update A22 -= L21 L21^T as GEMMs;
 //   2. inverse of the factor block column by block column, one batched GEMM pair per block diagonal;
 //   3. P = Linv^T Linv with the K range of every tile clipped to the non-zero (lower-triangular) part.
 // All three are O(n^3) GEMM work and run on the tensor cores: gemm_tc2.cuh / gemm_tc.cuh (wgmma .tf32 with a 3xTF32 operand
-// split for fp32-level accuracy -- the reference inverts in fp32 LAPACK -- accumulators in registers).  Only the 128 x 128
-// diagonal-block factorisations stay on the CUDA cores (one CTA each, O(n * NB^2) work in total).
+// split for fp32-level accuracy, accumulators in registers).  Only the 128 x 128 diagonal-block factorisations stay on the
+// CUDA cores (one CTA each, O(n * NB^2) work in total).
+// The popularity diagonal is a count, below sum r^2 on explicit ratings, so there G can be indefinite.  When the Cholesky
+// meets a non-positive pivot, G is inverted again in fp64 by the pivoted LU of lu_inverse.cu (what np.linalg.inv does);
+// an fp32 LU of these systems (cond up to ~1e7) would be far from the reference.
 #include <algorithm>
 #include <vector>
 
@@ -88,6 +91,24 @@ __global__ void ease_finish_kernel(const float* __restrict__ P, int ldp, int n, 
   Bout[g] = i == j ? 0.f : P[(long long)i * ldp + j] / (-P[(long long)j * ldp + j]);
 }
 
+// fp64 copy of G padded to n_pad with the diagonal set_diag_kernel writes (the fp32 values, widened): input of the LU path
+__global__ void widen_gram_kernel(const float* __restrict__ G, int n, int n_pad, const int* __restrict__ csc_cnt, float l2, double* A) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (long long)n_pad * n_pad) return;
+  const int i = (int)(g / n_pad), j = (int)(g % n_pad);
+  float v = i == j ? 1.0f : 0.0f;
+  if (i < n && j < n) v = i == j ? (float)csc_cnt[j] + l2 : G[(long long)i * n + j];
+  A[g] = (double)v;
+}
+
+// ease_finish_kernel on the fp64 inverse: the quotient in fp64, rounded once to fp32
+__global__ void ease_finish64_kernel(const double* __restrict__ P, int ldp, int n, float* Bout) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (long long)n * n) return;
+  const int i = (int)(g / n), j = (int)(g % n);
+  Bout[g] = i == j ? 0.f : (float)(P[(long long)i * ldp + j] / (-P[(long long)j * ldp + j]));
+}
+
 __global__ void copy_block_kernel(const float* __restrict__ src, int lds, float* dst, int ldd, int rows, int cols) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= (long long)rows * cols) return;
@@ -155,6 +176,63 @@ void gemm(cudaStream_t st, int M, int N, int K, float alpha, const float* A, int
   count_launch();
 }
 
+// In-place inverse of a symmetric positive definite n_pad x n_pad matrix (n_pad multiple of 128, row-major, device).
+// Returns 0 with A^{-1} (full symmetric matrix) in d_A, or the 1-based position of the first non-positive pivot inside a
+// diagonal block (the factorisation runs to the end, no inverse is formed).  d_work: 2 * n_pad * n_pad floats.
+int spd_inverse(float* d_A, int n_pad, float* d_work, cudaStream_t st) {
+  const int nblk = n_pad / NB;
+  const long long nn = (long long)n_pad * n_pad;
+  float* Linv = d_work;        // n_pad x n_pad
+  float* panel = d_work + nn;  // n_pad x NB  (first part of the second workspace)
+  DevBuf<float> inv_blocks((size_t)nblk * NB * NB);
+  DevBuf<int> info(1);
+  B200_CUDA(cudaMemsetAsync(info.get(), 0, sizeof(int), st));
+  B200_CUDA(cudaFuncSetAttribute(potrf_inv_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, NB * (NB + 1) * 4));
+  // ---- 1. blocked Cholesky (lower), A = L L^T
+  for (int k = 0; k < nblk; ++k) {
+    float* Akk = d_A + (long long)k * NB * n_pad + (long long)k * NB;
+    potrf_inv_block_kernel<<<1, 256, NB * (NB + 1) * 4, st>>>(Akk, n_pad, inv_blocks.get() + (size_t)k * NB * NB, info.get());
+    count_launch();
+    const int rem = n_pad - (k + 1) * NB;
+    if (rem > 0) {
+      float* A21 = Akk + (long long)NB * n_pad;
+      // panel = A21 * inv(L11)^T
+      gemm<false, true, false>(st, rem, NB, NB, 1.f, A21, n_pad, 0, inv_blocks.get() + (size_t)k * NB * NB, NB, 0, 0.f, panel, NB, 0, 1);
+      copy_block_kernel<<<div_up((long long)rem * NB, 256), 256, 0, st>>>(panel, NB, A21, n_pad, rem, NB);
+      count_launch();
+      // A22 -= L21 * L21^T
+      float* A22 = A21 + NB;
+      gemm<false, true, false>(st, rem, rem, NB, -1.f, A21, n_pad, 0, A21, n_pad, 0, 1.f, A22, n_pad, 0, 1);
+    }
+  }
+  int h_info = 0;
+  B200_CUDA(cudaMemcpyAsync(&h_info, info.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaStreamSynchronize(st));
+  if (h_info != 0) return h_info;
+  // ---- 2. Linv = L^{-1}: diagonal blocks, then one block diagonal at a time
+  B200_CUDA(cudaMemsetAsync(Linv, 0, sizeof(float) * (size_t)nn, st));
+  for (int k = 0; k < nblk; ++k) {
+    copy_block_kernel<<<div_up((long long)NB * NB, 256), 256, 0, st>>>(inv_blocks.get() + (size_t)k * NB * NB, NB,
+                                                                       Linv + (long long)k * NB * n_pad + (long long)k * NB, n_pad, NB, NB);
+  }
+  count_launch(nblk);
+  const long long diag_stride = (long long)NB * n_pad + NB;  // from block (k, k) to block (k+1, k+1)
+  float* T = panel;                                          // nblk blocks of NB x NB
+  for (int d = 1; d < nblk; ++d) {
+    const int batch = nblk - d;
+    // T_k = L[k+d, k .. k+d-1] * Linv[k .. k+d-1, k]      (NB x d*NB) * (d*NB x NB)
+    gemm<false, false, false>(st, NB, NB, d * NB, 1.f, d_A + (long long)d * NB * n_pad, n_pad, diag_stride, Linv, n_pad, diag_stride, 0.f,
+                              T, NB, (long long)NB * NB, batch);
+    // Linv[k+d, k] = -inv(L[k+d, k+d]) * T_k
+    gemm<false, false, false>(st, NB, NB, NB, -1.f, inv_blocks.get() + (size_t)d * NB * NB, NB, (long long)NB * NB, T, NB,
+                              (long long)NB * NB, 0.f, Linv + (long long)d * NB * n_pad, n_pad, diag_stride, batch);
+  }
+  // ---- 3. A^{-1} = Linv^T * Linv  (k >= max(i, j) only)
+  gemm<true, false, true>(st, n_pad, n_pad, n_pad, 1.f, Linv, n_pad, 0, Linv, n_pad, 0, 0.f, d_A, n_pad, 0, 1);
+  B200_CUDA(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace ease
 }  // namespace b200
 
@@ -168,57 +246,8 @@ extern "C" {
 int b200_spd_inverse_device(float* d_A, int n_pad, float* d_work, void* stream) {
   return guarded([&] {
     B200_REQUIRE(d_A && d_work && n_pad > 0 && n_pad % NB == 0, "b200_spd_inverse: n_pad must be a positive multiple of %d", NB);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int nblk = n_pad / NB;
-    const long long nn = (long long)n_pad * n_pad;
-    float* Linv = d_work;        // n_pad x n_pad
-    float* panel = d_work + nn;  // n_pad x NB  (first part of the second workspace)
-    DevBuf<float> inv_blocks((size_t)nblk * NB * NB);
-    DevBuf<int> info(1);
-    B200_CUDA(cudaMemsetAsync(info.get(), 0, sizeof(int), st));
-    B200_CUDA(cudaFuncSetAttribute(potrf_inv_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, NB * (NB + 1) * 4));
-    // ---- 1. blocked Cholesky (lower), A = L L^T
-    for (int k = 0; k < nblk; ++k) {
-      float* Akk = d_A + (long long)k * NB * n_pad + (long long)k * NB;
-      potrf_inv_block_kernel<<<1, 256, NB * (NB + 1) * 4, st>>>(Akk, n_pad, inv_blocks.get() + (size_t)k * NB * NB, info.get());
-      count_launch();
-      const int rem = n_pad - (k + 1) * NB;
-      if (rem > 0) {
-        float* A21 = Akk + (long long)NB * n_pad;
-        // panel = A21 * inv(L11)^T
-        gemm<false, true, false>(st, rem, NB, NB, 1.f, A21, n_pad, 0, inv_blocks.get() + (size_t)k * NB * NB, NB, 0, 0.f, panel, NB, 0, 1);
-        copy_block_kernel<<<div_up((long long)rem * NB, 256), 256, 0, st>>>(panel, NB, A21, n_pad, rem, NB);
-        count_launch();
-        // A22 -= L21 * L21^T
-        float* A22 = A21 + NB;
-        gemm<false, true, false>(st, rem, rem, NB, -1.f, A21, n_pad, 0, A21, n_pad, 0, 1.f, A22, n_pad, 0, 1);
-      }
-    }
-    int h_info = 0;
-    B200_CUDA(cudaMemcpyAsync(&h_info, info.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    B200_REQUIRE(h_info == 0, "b200_spd_inverse: matrix is not positive definite (pivot %d of a diagonal block)", h_info);
-    // ---- 2. Linv = L^{-1}: diagonal blocks, then one block diagonal at a time
-    B200_CUDA(cudaMemsetAsync(Linv, 0, sizeof(float) * (size_t)nn, st));
-    for (int k = 0; k < nblk; ++k) {
-      copy_block_kernel<<<div_up((long long)NB * NB, 256), 256, 0, st>>>(inv_blocks.get() + (size_t)k * NB * NB, NB,
-                                                                         Linv + (long long)k * NB * n_pad + (long long)k * NB, n_pad, NB, NB);
-    }
-    count_launch(nblk);
-    const long long diag_stride = (long long)NB * n_pad + NB;  // from block (k, k) to block (k+1, k+1)
-    float* T = panel;                                          // nblk blocks of NB x NB
-    for (int d = 1; d < nblk; ++d) {
-      const int batch = nblk - d;
-      // T_k = L[k+d, k .. k+d-1] * Linv[k .. k+d-1, k]      (NB x d*NB) * (d*NB x NB)
-      gemm<false, false, false>(st, NB, NB, d * NB, 1.f, d_A + (long long)d * NB * n_pad, n_pad, diag_stride, Linv, n_pad, diag_stride, 0.f,
-                                T, NB, (long long)NB * NB, batch);
-      // Linv[k+d, k] = -inv(L[k+d, k+d]) * T_k
-      gemm<false, false, false>(st, NB, NB, NB, -1.f, inv_blocks.get() + (size_t)d * NB * NB, NB, (long long)NB * NB, T, NB,
-                                (long long)NB * NB, 0.f, Linv + (long long)d * NB * n_pad, n_pad, diag_stride, batch);
-    }
-    // ---- 3. A^{-1} = Linv^T * Linv  (k >= max(i, j) only)
-    gemm<true, false, true>(st, n_pad, n_pad, n_pad, 1.f, Linv, n_pad, 0, Linv, n_pad, 0, 0.f, d_A, n_pad, 0, 1);
-    B200_CUDA(cudaGetLastError());
+    const int info = spd_inverse(d_A, n_pad, d_work, (cudaStream_t)stream);
+    B200_REQUIRE(info == 0, "b200_spd_inverse: matrix is not positive definite (pivot %d of a diagonal block)", info);
   });
 }
 
@@ -269,12 +298,29 @@ int b200_ease_from_gram_device(const float* d_G, int n_items, const int32_t* d_u
     if (nnz > 0) { col_count_kernel<<<sm_count() * 8, 256, 0, st>>>(d_urm_indices, nnz, cnt.get()); count_launch(); }
     set_diag_kernel<<<div_up(n_pad, 256), 256, 0, st>>>(A.get(), n, n_pad, cnt.get(), l2_norm);
     count_launch();
-    int rc = b200_spd_inverse_device(A.get(), n_pad, work.get(), stream);
-    if (rc != B200_OK) throw CudaFail{rc};
+    const bool spd = spd_inverse(A.get(), n_pad, work.get(), st) == 0;
+    DevBuf<double> A64, work64;
+    if (!spd) {
+      // G + diag is not positive definite (explicit ratings: the popularity diagonal is below sum r^2): invert it as the
+      // reference does, by LU with partial pivoting, in fp64 (np.linalg.inv computes in float64 for a float32 input)
+      A.release();
+      work.release();
+      B200_CUDA(cudaStreamSynchronize(st));  // the Cholesky's GEMMs may still read the packed-operand workspaces
+      g_pack_a.release();
+      g_pack_b.release();
+      A64.alloc((size_t)nn);
+      work64.alloc((size_t)2 * nn);
+      widen_gram_kernel<<<div_up(nn, 256), 256, 0, st>>>(d_G, n, n_pad, cnt.get(), l2_norm, A64.get());
+      count_launch();
+      const int rc = b200_lu_inverse_device(A64.get(), n_pad, work64.get(), stream);
+      if (rc != B200_OK) throw CudaFail{rc};
+      work64.release();
+    }
     DevBuf<float> tmpB;
     float* out = d_B;
     if (!out) { tmpB.alloc((size_t)n * n); out = tmpB.get(); }
-    ease_finish_kernel<<<div_up((long long)n * n, 256), 256, 0, st>>>(A.get(), n_pad, n, out);
+    if (spd) ease_finish_kernel<<<div_up((long long)n * n, 256), 256, 0, st>>>(A.get(), n_pad, n, out);
+    else ease_finish64_kernel<<<div_up((long long)n * n, 256), 256, 0, st>>>(A64.get(), n_pad, n, out);
     count_launch();
     B200_CUDA(cudaGetLastError());
     if (h_B) B200_CUDA(cudaMemcpyAsync(h_B, out, sizeof(float) * (size_t)n * n, cudaMemcpyDeviceToHost, st));

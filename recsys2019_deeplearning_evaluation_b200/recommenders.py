@@ -586,8 +586,10 @@ class SLIM_BPR_Cython(BaseItemSimilarityMatrixRecommender, Incremental_Training_
 
 
 class EASE_R_Recommender(BaseItemSimilarityMatrixRecommender):
-    """EASE_R/EASE_R_Recommender.py:36-106.  Gram through the dense mode of the similarity kernel, SPD inverse through
-    the blocked-Cholesky kernels of csrc/ease.cu; `topK=None` keeps the dense B on the device for scoring."""
+    """EASE_R/EASE_R_Recommender.py:36-106.  Gram through the dense mode of the similarity kernel, inverse through the
+    fp32 blocked-Cholesky kernels of csrc/ease.cu, or -- when G + diag is not positive definite, as on explicit ratings at
+    small l2_norm -- through the fp64 pivoted LU of csrc/lu_inverse.cu; `topK=None` keeps the dense B on the device for
+    scoring.  A singular G raises np.linalg.LinAlgError("Singular matrix") like the reference's np.linalg.inv."""
     RECOMMENDER_NAME = "EASE_R_Recommender"
 
     def fit(self, topK=None, l2_norm=1e3, normalize_matrix=False, verbose=True):
@@ -604,8 +606,11 @@ class EASE_R_Recommender(BaseItemSimilarityMatrixRecommender):
         G = self._gram_device()
         _, d_idx, _ = self._urm_device()
         B = torch.empty((n, n), dtype=torch.float32, device=G.device)
-        _lib.check(self._lib.b200_ease_from_gram_device(G.data_ptr(), n, d_idx.data_ptr(), self.URM_train.nnz, float(l2_norm), None,
-                                                        B.data_ptr(), _stream()))
+        try:
+            _lib.check(self._lib.b200_ease_from_gram_device(G.data_ptr(), n, d_idx.data_ptr(), self.URM_train.nnz, float(l2_norm),
+                                                            None, B.data_ptr(), _stream()))
+        except np.linalg.LinAlgError as e:
+            raise np.linalg.LinAlgError("Singular matrix") from e
         del G
         if topK is None:  # :75-78: dense W, scores = URM[users] . W
             self._d_B = B
