@@ -329,6 +329,33 @@ int b200_score_mask_device(const int32_t* d_users, int n_users_block, const int3
  * -inf, then NaN; ties (-0 == +0) by ascending item index.  [n_rows, cutoff] tables; past the end of a row -1 / -inf */
 int b200_score_topn_device(const float* d_scores, int n_rows, int n_items, int cutoff, int32_t* d_items,
                            float* d_item_scores, void* stream);
+/* Candidate lists (EvaluatorNegativeItemSample, Evaluator.py:466-578): row b of a block of n_block users is d_users[b]'s
+ * list d_cand_idx[d_cand_ptr[b] .. d_cand_ptr[b+1]) of strictly ascending item ids (d_cand_ptr may point into a larger
+ * CSR: offsets stay absolute).  Per-candidate arrays are ragged fp32 [d_cand_ptr[n_block] - d_cand_ptr[0]], entry k at
+ * k - d_cand_ptr[0].
+ * sparse: score(b, c) = sum_j A[u, j] * B[j, c] with A CSR (row u = d_users[b]) and column c of B given as row c of
+ *   (d_b_ptr, d_b_idx, d_b_val), sorted indices: item-based A = URM, B = W (rows of W^T); user-based A = W, B = URM (CSC) */
+int b200_cand_score_sparse_device(const int32_t* d_users, int n_block, const int32_t* d_a_ptr, const int32_t* d_a_idx,
+                                  const float* d_a_val, const int32_t* d_b_ptr, const int32_t* d_b_idx, const float* d_b_val,
+                                  const int32_t* d_cand_ptr, const int32_t* d_cand_idx, float* d_out, void* stream);
+/* dense: score(b, c) = sum over (j, r) in row u of CSR A of r * B[j, c], B row-major [*, n_items] (EASE_R's dense W) */
+int b200_cand_score_dense_device(const int32_t* d_users, int n_block, const int32_t* d_a_ptr, const int32_t* d_a_idx,
+                                 const float* d_a_val, const float* d_B, int n_items, const int32_t* d_cand_ptr,
+                                 const int32_t* d_cand_idx, float* d_out, void* stream);
+/* MF: score(b, c) = U[u, :] . V[c, :] (+ global + user + item bias when the three pointers are non-NULL), V row-major
+ * [n_items, n_factors]; bitwise equal to the same entry of b200_score_mf_device's block */
+int b200_cand_score_mf_device(const int32_t* d_users, int n_block, const float* d_user_factors, const float* d_item_factors,
+                              int n_factors, const float* d_user_bias, const float* d_item_bias, const float* d_global_bias,
+                              const int32_t* d_cand_ptr, const int32_t* d_cand_idx, float* d_out, void* stream);
+/* d_out[k] = d_scores[b, candidate k of row b] from a dense row-major [n_block, n_items] score block */
+int b200_cand_gather_device(int n_block, const float* d_scores, int n_items, const int32_t* d_cand_ptr, const int32_t* d_cand_idx,
+                            float* d_out, void* stream);
+/* Per row the `cutoff` (<= 1024) best candidates, in the [n_block, cutoff] table format of b200_score_topn_device, after
+ * seen items (sorted CSR rows of d_users[b] in d_seen_ptr / d_seen_idx, both NULL for none) and items with
+ * d_ignore[item] != 0 (nullable, n_items bytes) are set to -inf.  d_cand_scores is overwritten with the masked scores. */
+int b200_cand_topn_device(const int32_t* d_users, int n_block, const int32_t* d_cand_ptr, const int32_t* d_cand_idx,
+                          float* d_cand_scores, const int32_t* d_seen_ptr, const int32_t* d_seen_idx, const unsigned char* d_ignore,
+                          int cutoff, int32_t* d_items, float* d_item_scores, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K7: SLIM ElasticNet  (SURVEY.md 8(f).4)

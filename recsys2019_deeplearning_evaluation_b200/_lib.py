@@ -96,6 +96,15 @@ SIGNATURES = {
     "b200_score_mf_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void, c_void, c_void]),
     "b200_score_mask_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, ctypes.c_int, c_void, c_void]),
     "b200_score_topn_device": (ctypes.c_int, [c_void, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void]),
+    "b200_cand_score_sparse_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, c_void, c_void, c_void, c_void,
+                                                     c_void, c_void]),
+    "b200_cand_score_dense_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, ctypes.c_int, c_void, c_void,
+                                                    c_void, c_void]),
+    "b200_cand_score_mf_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, ctypes.c_int, c_void, c_void, c_void, c_void, c_void,
+                                                 c_void, c_void]),
+    "b200_cand_gather_device": (ctypes.c_int, [ctypes.c_int, c_void, ctypes.c_int, c_void, c_void, c_void, c_void]),
+    "b200_cand_topn_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, c_void, c_void, ctypes.c_int, c_void,
+                                             c_void, c_void]),
     "b200_spd_inverse_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void]),
     "b200_debug_gemm_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_void,
                                               ctypes.c_int, c_void, ctypes.c_int, ctypes.c_float, c_void, ctypes.c_int, c_void]),

@@ -8,6 +8,8 @@
 // Outputs are dense [B, n_items] fp32 blocks (the Evaluator asks for B <= 1000 users at a time,
 // Base/Evaluation/Evaluator.py:422).  Roofline: HBM, dominated by the B*n_items*4 bytes written (+ read back by the
 // mask / top-N passes) and, for the sparse product, 8 bytes per gathered (j, w) pair of W.
+// The cand_* kernels score and rank per-user candidate lists instead (Evaluator.py:466-578, test items plus sampled
+// negatives, ~100 per user): the work is proportional to the candidates, not to B * n_items.
 #include <algorithm>
 
 #include "common.cuh"
@@ -115,74 +117,283 @@ __device__ __forceinline__ unsigned orderable(float v) {
   return v != v ? 0u : (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
-// per row the `cutoff` best items, best first (BaseRecommender.py:189-196); ties -> ascending item index.
-// One CTA per row: MSB radix select of the cutoff-th key over 64-bit keys (score bits, ~index), then the survivors
-// are ranked by counting (cutoff is small: <= 1024).
+// The `cutoff` best of the n scores L[0..n) of one row, best first (BaseRecommender.py:189-196); ties -> ascending
+// position.  Position q is item q, or items[q] when a (strictly ascending) item map is given, so that ties go to the
+// ascending item either way.  Called by all TOPN_THREADS threads of a CTA: MSB radix select of the cutoff-th key over
+// 64-bit keys (score bits, ~position), then the survivors are ranked by counting (cutoff is small: <= 1024).
+// out_items / out_scores: this row's `cutoff` slots; past the end of the row -1 / -inf.
 constexpr int TOPN_THREADS = 256;
 constexpr int TOPN_MAX = 1024;
+struct TopnSmem {
+  int hist[2048];
+  int digit, need, cnt;
+  u64 cand[TOPN_MAX];
+};
+__device__ __forceinline__ void topn_row(const float* L, int n, int cutoff, const int* items, int* out_items, float* out_scores,
+                                         TopnSmem& sm) {
+  const int tid = threadIdx.x;
+  const int keep = min(cutoff, n);
+  u64 prefix = 0, mask = 0;
+  int need = keep;
+  if (keep < n) {
+    for (int shift = 53;; shift -= 11) {
+      const int sh = max(shift, 0), nb = shift >= 0 ? 11 : 11 + shift;
+      for (int i = tid; i < 2048; i += TOPN_THREADS) sm.hist[i] = 0;
+      __syncthreads();
+      for (int q = tid; q < n; q += TOPN_THREADS) {
+        const u64 key = (((u64)orderable(L[q])) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
+        if ((key & mask) == prefix) atomicAdd(&sm.hist[(int)((key >> sh) & ((1u << nb) - 1))], 1);
+      }
+      __syncthreads();
+      if (tid < 32) {
+        int local = 0;
+        for (int b = 0; b < 64; ++b) local += sm.hist[tid * 64 + b];
+        int incl = local;
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+          const int t = __shfl_down_sync(0xffffffffu, incl, off);
+          if (tid + off < 32) incl += t;
+        }
+        int cum = incl - local;
+        for (int b = 63; b >= 0; --b) {
+          const int c = sm.hist[tid * 64 + b];
+          if (cum < need && cum + c >= need) { sm.digit = tid * 64 + b; sm.need = need - cum; }
+          cum += c;
+        }
+      }
+      __syncthreads();
+      prefix |= ((u64)sm.digit) << sh;
+      mask |= ((u64)((1u << nb) - 1)) << sh;
+      need = sm.need;
+      __syncthreads();
+      if (shift <= 0) break;
+    }
+  }
+  if (tid == 0) sm.cnt = 0;
+  __syncthreads();
+  for (int q = tid; q < n; q += TOPN_THREADS) {
+    const u64 key = (((u64)orderable(L[q])) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
+    if (key >= prefix) sm.cand[atomicAdd(&sm.cnt, 1)] = key;
+  }
+  __syncthreads();
+  const int m = sm.cnt;  // == keep
+  for (int t = tid; t < m; t += TOPN_THREADS) {
+    const u64 k = sm.cand[t];
+    int rank = 0;
+    for (int q = 0; q < m; ++q) rank += sm.cand[q] > k;
+    const int q = (int)(0xFFFFFFFFu - (unsigned)k);
+    out_items[rank] = items ? items[q] : q;
+    out_scores[rank] = L[q];
+  }
+  for (int t = m + tid; t < cutoff; t += TOPN_THREADS) { out_items[t] = -1; out_scores[t] = -INFINITY; }
+  __syncthreads();
+}
+
+// per row of a dense [n_rows, n_items] block the `cutoff` best items; one CTA per row
 __global__ void __launch_bounds__(TOPN_THREADS) topn_rows_kernel(const float* __restrict__ scores, int n_rows, int n_items,
                                                                 int cutoff, int* out_items, float* out_scores) {
-  __shared__ int hist[2048];
-  __shared__ int s_digit, s_need, s_cnt;
-  __shared__ u64 cand[TOPN_MAX];
-  const int tid = threadIdx.x;
-  for (int row = blockIdx.x; row < n_rows; row += gridDim.x) {
-    const float* L = scores + (size_t)row * n_items;
-    const int keep = min(cutoff, n_items);
-    u64 prefix = 0, mask = 0;
-    int need = keep;
-    if (keep < n_items) {
-      for (int shift = 53;; shift -= 11) {
-        const int sh = max(shift, 0), nb = shift >= 0 ? 11 : 11 + shift;
-        for (int i = tid; i < 2048; i += TOPN_THREADS) hist[i] = 0;
-        __syncthreads();
-        for (int q = tid; q < n_items; q += TOPN_THREADS) {
-          const u64 key = (((u64)orderable(L[q])) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
-          if ((key & mask) == prefix) atomicAdd(&hist[(int)((key >> sh) & ((1u << nb) - 1))], 1);
-        }
-        __syncthreads();
-        if (tid < 32) {
-          int local = 0;
-          for (int b = 0; b < 64; ++b) local += hist[tid * 64 + b];
-          int incl = local;
-#pragma unroll
-          for (int off = 1; off < 32; off <<= 1) {
-            const int t = __shfl_down_sync(0xffffffffu, incl, off);
-            if (tid + off < 32) incl += t;
-          }
-          int cum = incl - local;
-          for (int b = 63; b >= 0; --b) {
-            const int c = hist[tid * 64 + b];
-            if (cum < need && cum + c >= need) { s_digit = tid * 64 + b; s_need = need - cum; }
-            cum += c;
-          }
-        }
-        __syncthreads();
-        prefix |= ((u64)s_digit) << sh;
-        mask |= ((u64)((1u << nb) - 1)) << sh;
-        need = s_need;
-        __syncthreads();
-        if (shift <= 0) break;
+  __shared__ TopnSmem sm;
+  for (int row = blockIdx.x; row < n_rows; row += gridDim.x)
+    topn_row(scores + (size_t)row * n_items, n_items, cutoff, nullptr, out_items + (size_t)row * cutoff,
+             out_scores + (size_t)row * cutoff, sm);
+}
+
+// ---- candidate lists (EvaluatorNegativeItemSample, Evaluator.py:466-578): every user is ranked over her own sorted list
+// of candidate items only.  Row b of a block holds cand_idx[cand_ptr[b] .. cand_ptr[b + 1]); a per-candidate array is
+// ragged, [cand_ptr[n_block] - cand_ptr[0]], entry k of the block at k - cand_ptr[0].  Every other item of the catalogue
+// scores -inf on the full-catalogue path, so ranking the candidates alone gives the same +inf / finite prefix.
+constexpr int CAND_THREADS = 256;
+constexpr int CAND_STAGE = 2048;  // left-row entries staged in shared memory (16 KB); longer rows are read from global
+
+__device__ __forceinline__ int lower_bound(const int* a, int n, int x) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (a[mid] < x) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// score(b, c) = sum over j in row users[b] of A and column c of B of A[u, j] * B[j, c], column c of B being row c of
+// (b_ptr, b_idx, b_val) with sorted indices: item-based A = URM, B rows = rows of W^T; user-based A = W, B rows = URM
+// columns (CSC).  One CTA per user, the row of A staged in shared memory, one warp per candidate: the lanes walk the
+// shorter of the two sorted lists and binary-search the longer one.
+__global__ void __launch_bounds__(CAND_THREADS) cand_sparse_kernel(const int* __restrict__ users, const int* __restrict__ a_ptr,
+                                                                  const int* __restrict__ a_idx, const float* __restrict__ a_val,
+                                                                  const int* __restrict__ b_ptr, const int* __restrict__ b_idx,
+                                                                  const float* __restrict__ b_val, const int* __restrict__ cand_ptr,
+                                                                  const int* __restrict__ cand_idx, float* __restrict__ out) {
+  __shared__ int s_idx[CAND_STAGE];
+  __shared__ float s_val[CAND_STAGE];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+  const int b = blockIdx.x, u = users[b];
+  const int as = a_ptr[u], na = a_ptr[u + 1] - as;
+  const int* ri = a_idx + as;
+  const float* rv = a_val + as;
+  if (na <= CAND_STAGE) {
+    for (int t = tid; t < na; t += blockDim.x) { s_idx[t] = ri[t]; s_val[t] = rv[t]; }
+    ri = s_idx;
+    rv = s_val;
+  }
+  __syncthreads();
+  const int base = cand_ptr[0], ce = cand_ptr[b + 1];
+  for (int k = cand_ptr[b] + warp; k < ce; k += nwarps) {
+    const int c = cand_idx[k];
+    const int bs = b_ptr[c], nb = b_ptr[c + 1] - bs;
+    const int* ci = b_idx + bs;
+    const float* cv = b_val + bs;
+    float acc = 0.f;
+    if (nb <= na) {
+      for (int q = lane; q < nb; q += 32) {
+        const int j = ci[q], p = lower_bound(ri, na, j);
+        if (p < na && ri[p] == j) acc += rv[p] * cv[q];
+      }
+    } else {
+      for (int p = lane; p < na; p += 32) {
+        const int j = ri[p], q = lower_bound(ci, nb, j);
+        if (q < nb && ci[q] == j) acc += rv[p] * cv[q];
       }
     }
-    if (tid == 0) s_cnt = 0;
-    __syncthreads();
-    for (int q = tid; q < n_items; q += TOPN_THREADS) {
-      const u64 key = (((u64)orderable(L[q])) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
-      if (key >= prefix) cand[atomicAdd(&s_cnt, 1)] = key;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+    if (lane == 0) out[k - base] = acc;
+  }
+}
+
+// score(b, c) = sum over (j, r) in row users[b] of A of r * B[j, c], B dense row-major [*, n_items] (EASE_R's dense W).
+// One CTA per user, the row of A staged in shared memory, one thread per candidate summing in profile order.
+__global__ void __launch_bounds__(CAND_THREADS) cand_dense_kernel(const int* __restrict__ users, const int* __restrict__ a_ptr,
+                                                                 const int* __restrict__ a_idx, const float* __restrict__ a_val,
+                                                                 const float* __restrict__ B, int n_items,
+                                                                 const int* __restrict__ cand_ptr, const int* __restrict__ cand_idx,
+                                                                 float* __restrict__ out) {
+  __shared__ int s_idx[CAND_STAGE];
+  __shared__ float s_val[CAND_STAGE];
+  const int tid = threadIdx.x;
+  const int b = blockIdx.x, u = users[b];
+  const int as = a_ptr[u], na = a_ptr[u + 1] - as;
+  const int* ri = a_idx + as;
+  const float* rv = a_val + as;
+  if (na <= CAND_STAGE) {
+    for (int t = tid; t < na; t += blockDim.x) { s_idx[t] = ri[t]; s_val[t] = rv[t]; }
+    ri = s_idx;
+    rv = s_val;
+  }
+  __syncthreads();
+  const int base = cand_ptr[0], ce = cand_ptr[b + 1];
+  for (int k = cand_ptr[b] + tid; k < ce; k += blockDim.x) {
+    const int c = cand_idx[k];
+    float acc = 0.f;
+    for (int p = 0; p < na; ++p) acc += rv[p] * B[(size_t)ri[p] * n_items + c];
+    out[k - base] = acc;
+  }
+}
+
+// score(b, c) = U[users[b], :] . V[c, :] (+ biases), one thread per (user, candidate) in the fp32 operation order of
+// mf_scores_kernel (a sequential fused sum over the factors, then + (mu + bi) + bu), so the scores are bitwise those of the
+// dense block.  One CTA per user, its factor row in shared memory; V row-major [n_items, f].
+__global__ void __launch_bounds__(CAND_THREADS) cand_mf_kernel(const int* __restrict__ users, const float* __restrict__ U,
+                                                              const float* __restrict__ V, int f, const float* __restrict__ bu,
+                                                              const float* __restrict__ bi, const float* __restrict__ mu,
+                                                              const int* __restrict__ cand_ptr, const int* __restrict__ cand_idx,
+                                                              float* __restrict__ out) {
+  extern __shared__ float us[];  // [f]
+  const int tid = threadIdx.x;
+  const int b = blockIdx.x, u = users[b];
+  for (int t = tid; t < f; t += blockDim.x) us[t] = U[(size_t)u * f + t];
+  __syncthreads();
+  const int base = cand_ptr[0], ce = cand_ptr[b + 1];
+  for (int k = cand_ptr[b] + tid; k < ce; k += blockDim.x) {
+    const int c = cand_idx[k];
+    const float* v = V + (size_t)c * f;
+    float acc = 0.f;
+    for (int q = 0; q < f; ++q) acc += us[q] * v[q];
+    const float bias = mu ? mu[0] + bi[c] : 0.f;
+    out[k - base] = acc + bias + (mu ? bu[u] : 0.f);
+  }
+}
+
+// out[k] = scores[b, cand_idx[k]] from a dense [n_block, n_items] block; one warp per row
+__global__ void cand_gather_kernel(int n_block, const float* __restrict__ scores, int n_items, const int* __restrict__ cand_ptr,
+                                   const int* __restrict__ cand_idx, float* __restrict__ out) {
+  const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (b >= n_block) return;
+  const int base = cand_ptr[0], ce = cand_ptr[b + 1];
+  for (int k = cand_ptr[b] + lane; k < ce; k += 32) out[k - base] = scores[(size_t)b * n_items + cand_idx[k]];
+}
+
+// BaseRecommender.py:164-169, :192-193: a seen candidate (binary search in the user's sorted train row) or an ignored one
+// scores -inf
+__device__ __forceinline__ float cand_masked(float v, int item, const int* seen, int n_seen, const unsigned char* ignore) {
+  if (ignore && ignore[item]) return -INFINITY;
+  if (n_seen > 0) {
+    const int p = lower_bound(seen, n_seen, item);
+    if (p < n_seen && seen[p] == item) return -INFINITY;
+  }
+  return v;
+}
+
+// candidate top-N, lists of up to CAND_WARP_LIST: one warp per user, keys in shared memory, rank by counting
+constexpr int CAND_WARP_LIST = 256;
+constexpr int CAND_TOPN_WARPS = 8;
+__global__ void __launch_bounds__(CAND_TOPN_WARPS * 32) cand_topn_warp_kernel(
+    const int* __restrict__ users, int n_block, const int* __restrict__ cand_ptr, const int* __restrict__ cand_idx,
+    const float* __restrict__ scores, const int* __restrict__ seen_ptr, const int* __restrict__ seen_idx,
+    const unsigned char* __restrict__ ignore, int cutoff, int* out_items, float* out_scores) {
+  __shared__ u64 s_key[CAND_TOPN_WARPS][CAND_WARP_LIST];
+  __shared__ float s_val[CAND_TOPN_WARPS][CAND_WARP_LIST];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int b = blockIdx.x * CAND_TOPN_WARPS + w;
+  if (b >= n_block) return;
+  const int cs = cand_ptr[b], n = cand_ptr[b + 1] - cs;
+  if (n > CAND_WARP_LIST) return;  // cand_topn_cta_kernel's row
+  const float* L = scores + (cs - cand_ptr[0]);
+  const int* items = cand_idx + cs;
+  const int* seen = nullptr;
+  int n_seen = 0;
+  if (seen_ptr) {
+    const int u = users[b];
+    seen = seen_idx + seen_ptr[u];
+    n_seen = seen_ptr[u + 1] - seen_ptr[u];
+  }
+  for (int q = lane; q < n; q += 32) {
+    const float v = cand_masked(L[q], items[q], seen, n_seen, ignore);
+    s_val[w][q] = v;
+    s_key[w][q] = (((u64)orderable(v)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
+  }
+  __syncwarp();
+  int* oi = out_items + (size_t)b * cutoff;
+  float* os = out_scores + (size_t)b * cutoff;
+  for (int q = lane; q < n; q += 32) {
+    const u64 k = s_key[w][q];
+    int rank = 0;
+    for (int t = 0; t < n; ++t) rank += s_key[w][t] > k;
+    if (rank < cutoff) { oi[rank] = items[q]; os[rank] = s_val[w][q]; }
+  }
+  for (int t = n + lane; t < cutoff; t += 32) { oi[t] = -1; os[t] = -INFINITY; }
+}
+
+// candidate top-N, lists longer than CAND_WARP_LIST: one CTA per user masks the scores in place, then topn_row
+__global__ void __launch_bounds__(TOPN_THREADS) cand_topn_cta_kernel(
+    const int* __restrict__ users, int n_block, const int* __restrict__ cand_ptr, const int* __restrict__ cand_idx,
+    float* scores, const int* __restrict__ seen_ptr, const int* __restrict__ seen_idx, const unsigned char* __restrict__ ignore,
+    int cutoff, int* out_items, float* out_scores) {
+  __shared__ TopnSmem sm;
+  for (int b = blockIdx.x; b < n_block; b += gridDim.x) {
+    const int cs = cand_ptr[b], n = cand_ptr[b + 1] - cs;
+    if (n <= CAND_WARP_LIST) continue;
+    float* L = scores + (cs - cand_ptr[0]);
+    const int* items = cand_idx + cs;
+    const int* seen = nullptr;
+    int n_seen = 0;
+    if (seen_ptr) {
+      const int u = users[b];
+      seen = seen_idx + seen_ptr[u];
+      n_seen = seen_ptr[u + 1] - seen_ptr[u];
     }
+    for (int q = threadIdx.x; q < n; q += TOPN_THREADS) L[q] = cand_masked(L[q], items[q], seen, n_seen, ignore);
     __syncthreads();
-    const int n = s_cnt;  // == keep
-    for (int t = tid; t < n; t += TOPN_THREADS) {
-      const u64 k = cand[t];
-      int rank = 0;
-      for (int q = 0; q < n; ++q) rank += cand[q] > k;
-      const int item = (int)(0xFFFFFFFFu - (unsigned)k);
-      out_items[(size_t)row * cutoff + rank] = item;
-      out_scores[(size_t)row * cutoff + rank] = L[item];
-    }
-    for (int t = n + tid; t < cutoff; t += TOPN_THREADS) { out_items[(size_t)row * cutoff + t] = -1; out_scores[(size_t)row * cutoff + t] = -INFINITY; }
-    __syncthreads();
+    topn_row(L, n, cutoff, items, out_items + (size_t)b * cutoff, out_scores + (size_t)b * cutoff, sm);
   }
 }
 
@@ -270,6 +481,89 @@ int b200_score_topn_device(const float* d_scores, int n_rows, int n_items, int c
                                                                                                   d_items, d_item_scores);
     B200_CUDA(cudaGetLastError());
     count_launch();
+  });
+}
+
+int b200_cand_score_sparse_device(const int32_t* d_users, int n_block, const int32_t* d_a_ptr, const int32_t* d_a_idx,
+                                  const float* d_a_val, const int32_t* d_b_ptr, const int32_t* d_b_idx, const float* d_b_val,
+                                  const int32_t* d_cand_ptr, const int32_t* d_cand_idx, float* d_out, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(d_users && d_a_ptr && d_a_idx && d_a_val && d_b_ptr && d_b_idx && d_b_val && d_cand_ptr && d_cand_idx && d_out,
+                 "b200_cand_score_sparse: NULL argument");
+    B200_REQUIRE(n_block >= 0, "b200_cand_score_sparse: bad shape");
+    if (n_block == 0) return;
+    cand_sparse_kernel<<<n_block, CAND_THREADS, 0, (cudaStream_t)stream>>>(d_users, d_a_ptr, d_a_idx, d_a_val, d_b_ptr, d_b_idx,
+                                                                            d_b_val, d_cand_ptr, d_cand_idx, d_out);
+    B200_CUDA(cudaGetLastError());
+    count_launch();
+  });
+}
+
+int b200_cand_score_dense_device(const int32_t* d_users, int n_block, const int32_t* d_a_ptr, const int32_t* d_a_idx,
+                                 const float* d_a_val, const float* d_B, int n_items, const int32_t* d_cand_ptr,
+                                 const int32_t* d_cand_idx, float* d_out, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(d_users && d_a_ptr && d_a_idx && d_a_val && d_B && d_cand_ptr && d_cand_idx && d_out,
+                 "b200_cand_score_dense: NULL argument");
+    B200_REQUIRE(n_block >= 0 && n_items > 0, "b200_cand_score_dense: bad shape");
+    if (n_block == 0) return;
+    cand_dense_kernel<<<n_block, CAND_THREADS, 0, (cudaStream_t)stream>>>(d_users, d_a_ptr, d_a_idx, d_a_val, d_B, n_items,
+                                                                           d_cand_ptr, d_cand_idx, d_out);
+    B200_CUDA(cudaGetLastError());
+    count_launch();
+  });
+}
+
+int b200_cand_score_mf_device(const int32_t* d_users, int n_block, const float* d_user_factors, const float* d_item_factors,
+                              int n_factors, const float* d_user_bias, const float* d_item_bias, const float* d_global_bias,
+                              const int32_t* d_cand_ptr, const int32_t* d_cand_idx, float* d_out, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(d_users && d_user_factors && d_item_factors && d_cand_ptr && d_cand_idx && d_out, "b200_cand_score_mf: NULL argument");
+    B200_REQUIRE(n_factors >= 1 && n_block >= 0, "b200_cand_score_mf: bad shape");
+    B200_REQUIRE((d_global_bias == nullptr) == (d_user_bias == nullptr) && (d_user_bias == nullptr) == (d_item_bias == nullptr),
+                 "b200_cand_score_mf: biases must be all given or all NULL");
+    const size_t smem = (size_t)n_factors * sizeof(float);
+    B200_REQUIRE(smem <= 48 * 1024, "b200_cand_score_mf: n_factors=%d too large", n_factors);
+    if (n_block == 0) return;
+    cand_mf_kernel<<<n_block, CAND_THREADS, smem, (cudaStream_t)stream>>>(d_users, d_user_factors, d_item_factors, n_factors,
+                                                                           d_user_bias, d_item_bias, d_global_bias, d_cand_ptr,
+                                                                           d_cand_idx, d_out);
+    B200_CUDA(cudaGetLastError());
+    count_launch();
+  });
+}
+
+int b200_cand_gather_device(int n_block, const float* d_scores, int n_items, const int32_t* d_cand_ptr, const int32_t* d_cand_idx,
+                            float* d_out, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(d_scores && d_cand_ptr && d_cand_idx && d_out, "b200_cand_gather: NULL argument");
+    B200_REQUIRE(n_block >= 0 && n_items > 0, "b200_cand_gather: bad shape");
+    if (n_block == 0) return;
+    cand_gather_kernel<<<div_up((long long)n_block * 32, 256), 256, 0, (cudaStream_t)stream>>>(n_block, d_scores, n_items, d_cand_ptr,
+                                                                                             d_cand_idx, d_out);
+    B200_CUDA(cudaGetLastError());
+    count_launch();
+  });
+}
+
+int b200_cand_topn_device(const int32_t* d_users, int n_block, const int32_t* d_cand_ptr, const int32_t* d_cand_idx,
+                          float* d_cand_scores, const int32_t* d_seen_ptr, const int32_t* d_seen_idx, const unsigned char* d_ignore,
+                          int cutoff, int32_t* d_items, float* d_item_scores, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(d_cand_ptr && d_cand_idx && d_cand_scores && d_items && d_item_scores, "b200_cand_topn: NULL argument");
+    B200_REQUIRE((d_seen_ptr == nullptr) == (d_seen_idx == nullptr) && (d_seen_ptr == nullptr || d_users),
+                 "b200_cand_topn: the seen-item filter needs d_users, d_seen_ptr and d_seen_idx");
+    B200_REQUIRE(cutoff >= 1 && cutoff <= TOPN_MAX, "b200_cand_topn: cutoff must be in [1, %d]", TOPN_MAX);
+    B200_REQUIRE(n_block >= 0, "b200_cand_topn: bad shape");
+    if (n_block == 0) return;
+    cudaStream_t st = (cudaStream_t)stream;
+    cand_topn_warp_kernel<<<div_up(n_block, CAND_TOPN_WARPS), CAND_TOPN_WARPS * 32, 0, st>>>(
+        d_users, n_block, d_cand_ptr, d_cand_idx, d_cand_scores, d_seen_ptr, d_seen_idx, d_ignore, cutoff, d_items, d_item_scores);
+    B200_CUDA(cudaGetLastError());
+    cand_topn_cta_kernel<<<std::min(n_block, sm_count() * 4), TOPN_THREADS, 0, st>>>(
+        d_users, n_block, d_cand_ptr, d_cand_idx, d_cand_scores, d_seen_ptr, d_seen_idx, d_ignore, cutoff, d_items, d_item_scores);
+    B200_CUDA(cudaGetLastError());
+    count_launch(2);
   });
 }
 

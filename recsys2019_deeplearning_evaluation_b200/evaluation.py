@@ -9,8 +9,8 @@ and its top-`max_cutoff` table stay on the device (recommenders.BaseRecommender.
 and `b200_eval_accumulate_device` (csrc/eval.cu) reduces all per-user metrics of :336-366 into device accumulators;
 the host only combines the final sums and the per-item recommendation counters (O(n_items) once per evaluation).
 
-`EvaluatorNegativeItemSample` (Evaluator.py:466-578) is the same pipeline with one user per step and the user's candidate set
-(test items + sampled negatives) passed through the items_to_compute mask.
+`EvaluatorNegativeItemSample` (Evaluator.py:466-578) walks the same blocks of users, but scores and ranks only each user's
+candidate list (test items + sampled negatives) with the csrc/score.cu candidate kernels before the same accumulate kernel.
 Not mirrored: `diversity_object` (DIVERSITY_SIMILARITY needs an item-similarity matrix, metrics.py:719-775).
 """
 import ctypes
@@ -137,33 +137,34 @@ class EvaluatorHoldout(object):
             hit=torch.zeros((len(self.cutoff_list), self.n_items), dtype=torch.int32, device=dev))
         return st
 
-    def _blocks(self, users, block_size):
-        """(user ids of one block, items_to_compute or None): hold-out evaluation scores whole blocks of users (:426-455)."""
+    def _accumulate(self, st, d_users, items, vals, cutoff):
+        """Adds one block's [B, cutoff] top-N table to the device accumulators (csrc/eval.cu)."""
+        import torch
+        _lib.check(self._lib.b200_eval_accumulate_device(
+            d_users.data_ptr(), d_users.shape[0], items.data_ptr(), vals.data_ptr(), cutoff, st["ptr"].data_ptr(),
+            st["idx"].data_ptr(), st["val"].data_ptr(), st["cut"].data_ptr(), len(self.cutoff_list), st["idcg"].data_ptr(),
+            st["nov"].data_ptr(), st["pop"].data_ptr(), self.n_items, st["acc"].data_ptr(), st["rec"].data_ptr(),
+            st["hit"].data_ptr(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+
+    def _evaluate_blocks(self, recommender_object, users, block_size, st):
+        """Hold-out evaluation scores whole blocks of users (:426-455)."""
+        cutoff = int(min(self.max_cutoff, self.n_items))
         for b0 in range(0, len(users), block_size):
-            yield users[b0:b0 + block_size], None
+            d_users = recommender_object._users_tensor(users[b0:b0 + block_size])
+            scores = recommender_object._masked_scores_device(d_users, remove_seen_flag=self.exclude_seen, items_to_compute=None,
+                                                              remove_custom_items_flag=self.ignore_items_flag)
+            items, vals = recommender_object._topn_device(scores, cutoff)
+            self._accumulate(st, d_users, items, vals, cutoff)
 
     def evaluateRecommender(self, recommender_object, block_size=None):
         """Evaluator.py:240-288 + :413-461."""
-        import torch
         if self.ignore_items_flag:
             recommender_object.set_items_to_ignore(self.ignore_items_ID)
         users = np.asarray(self.users_to_evaluate, dtype=np.int64)
         if block_size is None:  # :422
             block_size = min([1000, int(4 * 1e9 * 8 / 64 / self.n_items), max(len(users), 1)])
         st = self._device_state(recommender_object.get_URM_train())
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        cutoff = int(min(self.max_cutoff, self.n_items))
-        for block_users, items_to_compute in self._blocks(users, block_size):
-            d_users = recommender_object._users_tensor(block_users)
-            scores = recommender_object._masked_scores_device(d_users, remove_seen_flag=self.exclude_seen,
-                                                              items_to_compute=items_to_compute,
-                                                              remove_custom_items_flag=self.ignore_items_flag)
-            items, vals = recommender_object._topn_device(scores, cutoff)
-            _lib.check(self._lib.b200_eval_accumulate_device(
-                d_users.data_ptr(), d_users.shape[0], items.data_ptr(), vals.data_ptr(), cutoff, st["ptr"].data_ptr(),
-                st["idx"].data_ptr(), st["val"].data_ptr(), st["cut"].data_ptr(), len(self.cutoff_list), st["idcg"].data_ptr(),
-                st["nov"].data_ptr(), st["pop"].data_ptr(), self.n_items, st["acc"].data_ptr(), st["rec"].data_ptr(),
-                st["hit"].data_ptr(), stream))
+        self._evaluate_blocks(recommender_object, users, block_size, st)
         acc, rec, hit = st["acc"].cpu().numpy(), st["rec"].cpu().numpy().astype(np.float64), st["hit"].cpu().numpy().astype(np.float64)
         n_eval = len(users)
         results_dict = {}
@@ -211,8 +212,11 @@ class EvaluatorHoldout(object):
 
 class EvaluatorNegativeItemSample(EvaluatorHoldout):
     """Base/Evaluation/Evaluator.py:466-578: every user is ranked over HER test items plus her sampled negative items only
-    (the protocol of the NeuMF-style experiments).  Same device pipeline as the hold-out evaluator, one user per step like
-    the reference (:553-571), the per-user candidate set going through the items_to_compute mask of the score block."""
+    (the protocol of the NeuMF-style experiments).  The reference scores one user at a time (:553-571) over the whole
+    catalogue with the other items masked; here blocks of users score and rank their candidates only, on the device:
+    `rec._candidate_scores_device` (a ragged array aligned with the candidate CSR) -> `b200_cand_topn_device` (seen and
+    ignored candidates -> -inf, the [B, max_cutoff] table of the hold-out path) -> the same accumulate kernel.  Every
+    non-candidate scores -inf in the reference's ranking, so its finite prefix -- the recommendation list -- is the same."""
     EVALUATOR_NAME = "EvaluatorNegativeItemSample"
 
     def __init__(self, URM_test_list, URM_test_negative, cutoff_list, min_ratings_per_user=1, exclude_seen=True,
@@ -224,12 +228,53 @@ class EvaluatorNegativeItemSample(EvaluatorHoldout):
         rank.eliminate_zeros()
         rank.sort_indices()
         self.URM_items_to_rank = rank
+        # the candidate lists in users_to_evaluate order, so that a block of users is a contiguous slice
+        cand = rank[np.asarray(self.users_to_evaluate, dtype=np.int64)]
+        if cand.nnz >= 2 ** 31:
+            raise ValueError("EvaluatorNegativeItemSample: more than 2^31 - 1 candidate items in total")
+        self._cand_ptr = np.ascontiguousarray(cand.indptr, np.int32)
+        self._cand_idx = np.ascontiguousarray(cand.indices, np.int32)
+        self._d_cand = None
 
     def _get_user_specific_items_to_compute(self, user_id):
         r = self.URM_items_to_rank
         return r.indices[r.indptr[user_id]:r.indptr[user_id + 1]]
 
-    def _blocks(self, users, block_size):
-        for u in users:
-            yield np.atleast_1d(u), self._get_user_specific_items_to_compute(int(u))
+    def _cand_device(self, dev):
+        """(users, candidate pointer, candidate items) on the device, uploaded once per evaluator."""
+        import torch
+        if self._d_cand is None or self._d_cand[0].device != dev:
+            users = np.asarray(self.users_to_evaluate, dtype=np.int32)
+            self._d_cand = tuple(torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in (users, self._cand_ptr, self._cand_idx))
+        return self._d_cand
+
+    def _evaluate_blocks(self, recommender_object, users, block_size, st):
+        import torch
+        n = len(users)
+        if n == 0:
+            return
+        dev = st["ptr"].device
+        d_users, d_ptr, d_idx = self._cand_device(dev)
+        cutoff = int(min(self.max_cutoff, self.n_items))
+        starts = np.arange(0, n, block_size)
+        longest = int(np.max(self._cand_ptr[np.minimum(starts + block_size, n)] - self._cand_ptr[starts]))
+        scores = torch.empty(max(longest, 1), dtype=torch.float32, device=dev)
+        items = torch.empty((min(block_size, n), cutoff), dtype=torch.int32, device=dev)
+        vals = torch.empty((min(block_size, n), cutoff), dtype=torch.float32, device=dev)
+        seen_ptr = seen_idx = ignore = None
+        if self.exclude_seen:
+            seen_ptr, seen_idx, _ = (t.data_ptr() for t in recommender_object._urm_device())
+        if self.ignore_items_flag and len(recommender_object.items_to_ignore_ID):  # BaseRecommender.py:192-193
+            mask = np.zeros(self.n_items, np.uint8)
+            mask[recommender_object.items_to_ignore_ID] = 1
+            ignore = torch.from_numpy(mask).to(dev)
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        for b0 in starts.tolist():
+            nb = min(block_size, n - b0)
+            b_users, b_ptr = d_users[b0:b0 + nb], d_ptr[b0:b0 + nb + 1]
+            recommender_object._candidate_scores_device(b_users, b_ptr, d_idx, scores)
+            _lib.check(self._lib.b200_cand_topn_device(
+                b_users.data_ptr(), nb, b_ptr.data_ptr(), d_idx.data_ptr(), scores.data_ptr(), seen_ptr, seen_idx,
+                ignore.data_ptr() if ignore is not None else None, cutoff, items.data_ptr(), vals.data_ptr(), stream))
+            self._accumulate(st, b_users, items[:nb], vals[:nb], cutoff)
 

@@ -154,6 +154,23 @@ class BaseRecommender(object):
             scores[:, torch.from_numpy(self.items_to_ignore_ID).to(scores.device)] = float("-inf")
         return scores
 
+    def _candidate_scores_device(self, d_users, d_cand_ptr, d_cand_idx, out):
+        """Raw scores of each user's candidate items (EvaluatorNegativeItemSample): d_cand_ptr [B + 1] int32 (absolute
+        offsets, a slice of a larger CSR), d_cand_idx the candidate items, out the ragged fp32 CUDA tensor, entry k at
+        k - d_cand_ptr[0].  A model family's own kernel is used only when `_scores_device` is that family's method, so a
+        subclass that overrides `_scores_device` is always scored through it (`_candidate_scores_by_block`)."""
+        kernel = _CANDIDATE_KERNELS.get(type(self)._scores_device)
+        if kernel is None:
+            return self._candidate_scores_by_block(d_users, d_cand_ptr, d_cand_idx, out)
+        return kernel(self, d_users, d_cand_ptr, d_cand_idx, out)
+
+    def _candidate_scores_by_block(self, d_users, d_cand_ptr, d_cand_idx, out):
+        """The dense [B, n_items] block of `_scores_device`, then its candidates' entries."""
+        scores = self._scores_device(d_users)
+        _lib.check(self._lib.b200_cand_gather_device(d_users.shape[0], scores.data_ptr(), self.n_items, d_cand_ptr.data_ptr(),
+                                                     d_cand_idx.data_ptr(), out.data_ptr(), _stream()))
+        return out
+
     def _topn_device(self, scores, cutoff):
         """[B, cutoff] int32 items / float32 scores CUDA tensors (cutoff <= 1024) in the order of
         np.lexsort((arange, -s)): +inf, finite scores descending, -inf, NaN, ties by ascending item id.  Entries whose
@@ -203,6 +220,15 @@ class BaseItemSimilarityMatrixRecommender(BaseRecommender):
             self._d_w_src = self.W_sparse
         return self._d_w
 
+    def _wt_device(self):
+        """W_sparse^T in CSR (the columns of W as rows), cached by the identity of W_sparse like _w_device."""
+        if getattr(self, "_d_wt_src", None) is not self.W_sparse:
+            WT = sps.csr_matrix(sps.csc_matrix(self.W_sparse, dtype=np.float32).T)
+            WT.sum_duplicates()
+            self._d_wt = _dev_csr(WT)
+            self._d_wt_src = self.W_sparse
+        return self._d_wt
+
     def _scores_device(self, d_users, items_to_compute=None):
         import torch
         a_ptr, a_idx, a_val = self._urm_device()
@@ -211,6 +237,15 @@ class BaseItemSimilarityMatrixRecommender(BaseRecommender):
         _lib.check(self._lib.b200_score_spmm_device(d_users.data_ptr(), d_users.shape[0], a_ptr.data_ptr(), a_idx.data_ptr(),
                                                     a_val.data_ptr(), b_ptr.data_ptr(), b_idx.data_ptr(), b_val.data_ptr(),
                                                     self.n_items, out.data_ptr(), _stream()))
+        return out
+
+    def _candidate_scores_kernel(self, d_users, d_cand_ptr, d_cand_idx, out):
+        """score(u, c) = URM[u, :] . W[:, c] over the candidates only."""
+        a_ptr, a_idx, a_val = self._urm_device()
+        b_ptr, b_idx, b_val = self._wt_device()
+        _lib.check(self._lib.b200_cand_score_sparse_device(
+            d_users.data_ptr(), d_users.shape[0], a_ptr.data_ptr(), a_idx.data_ptr(), a_val.data_ptr(), b_ptr.data_ptr(),
+            b_idx.data_ptr(), b_val.data_ptr(), d_cand_ptr.data_ptr(), d_cand_idx.data_ptr(), out.data_ptr(), _stream()))
         return out
 
 
@@ -231,6 +266,26 @@ class BaseUserSimilarityMatrixRecommender(BaseRecommender):
         _lib.check(self._lib.b200_score_spmm_device(d_users.data_ptr(), d_users.shape[0], a_ptr.data_ptr(), a_idx.data_ptr(),
                                                     a_val.data_ptr(), b_ptr.data_ptr(), b_idx.data_ptr(), b_val.data_ptr(),
                                                     self.n_items, out.data_ptr(), _stream()))
+        return out
+
+    def _urm_csc_device(self):
+        """URM_train in CSC (its columns as rows), rebuilt whenever the CSR device copy of the profiles is."""
+        d_urm = self._urm_device()
+        if getattr(self, "_d_urm_csc_src", None) is not d_urm:
+            self._d_urm_csc = _dev_csr(sps.csr_matrix(sps.csc_matrix(self.URM_train, dtype=np.float32).T))
+            self._d_urm_csc_src = d_urm
+        return self._d_urm_csc
+
+    def _candidate_scores_kernel(self, d_users, d_cand_ptr, d_cand_idx, out):
+        """score(u, c) = W[u, :] . URM[:, c] over the candidates only."""
+        if getattr(self, "_d_w_src", None) is not self.W_sparse:
+            self._d_w = _dev_csr(self.W_sparse)
+            self._d_w_src = self.W_sparse
+        a_ptr, a_idx, a_val = self._d_w
+        b_ptr, b_idx, b_val = self._urm_csc_device()
+        _lib.check(self._lib.b200_cand_score_sparse_device(
+            d_users.data_ptr(), d_users.shape[0], a_ptr.data_ptr(), a_idx.data_ptr(), a_val.data_ptr(), b_ptr.data_ptr(),
+            b_idx.data_ptr(), b_val.data_ptr(), d_cand_ptr.data_ptr(), d_cand_idx.data_ptr(), out.data_ptr(), _stream()))
         return out
 
 
@@ -375,18 +430,30 @@ class BaseMatrixFactorizationRecommender(BaseRecommender):
             if self.use_bias:
                 biases = tuple(torch.from_numpy(np.ascontiguousarray(np.atleast_1d(b), np.float32)).to(dev)
                                for b in (self.USER_bias, self.ITEM_bias, self.GLOBAL_bias))
-            self._d_f, self._d_f_src = (U, VT, biases), (self.USER_factors, self.ITEM_factors)
+            # V itself is kept for the candidate scorer, which reads one item's factors per thread
+            self._d_f, self._d_f_src = (U, V, VT, biases), (self.USER_factors, self.ITEM_factors)
         return self._d_f
 
     def _scores_device(self, d_users, items_to_compute=None):
         import torch
-        U, VT, biases = self._factors_device()
+        U, _, VT, biases = self._factors_device()
         out = torch.empty((d_users.shape[0], self.n_items), dtype=torch.float32, device=d_users.device)
         bu = bi = mu = None
         if biases is not None:
             bu, bi, mu = (b.data_ptr() for b in biases)
         _lib.check(self._lib.b200_score_mf_device(d_users.data_ptr(), d_users.shape[0], U.data_ptr(), VT.data_ptr(), U.shape[1],
                                                   self.n_items, bu, bi, mu, out.data_ptr(), _stream()))
+        return out
+
+    def _candidate_scores_kernel(self, d_users, d_cand_ptr, d_cand_idx, out):
+        """score(u, c) = U[u] . V[c] (+ biases) over the candidates only, bitwise equal to the dense block's entry."""
+        U, V, _, biases = self._factors_device()
+        bu = bi = mu = None
+        if biases is not None:
+            bu, bi, mu = (b.data_ptr() for b in biases)
+        _lib.check(self._lib.b200_cand_score_mf_device(d_users.data_ptr(), d_users.shape[0], U.data_ptr(), V.data_ptr(), U.shape[1],
+                                                       bu, bi, mu, d_cand_ptr.data_ptr(), d_cand_idx.data_ptr(), out.data_ptr(),
+                                                       _stream()))
         return out
 
 
@@ -649,6 +716,16 @@ class EASE_R_Recommender(BaseItemSimilarityMatrixRecommender):
                                                     out.data_ptr(), _stream()))
         return out
 
+    def _candidate_scores_kernel(self, d_users, d_cand_ptr, d_cand_idx, out):
+        """score(u, c) = sum over the user's (j, r) of r * B[j, c] with the dense B, else the sparse item-based kernel."""
+        if getattr(self, "_d_B", None) is None:
+            return super(EASE_R_Recommender, self)._candidate_scores_kernel(d_users, d_cand_ptr, d_cand_idx, out)
+        a_ptr, a_idx, a_val = self._urm_device()
+        _lib.check(self._lib.b200_cand_score_dense_device(
+            d_users.data_ptr(), d_users.shape[0], a_ptr.data_ptr(), a_idx.data_ptr(), a_val.data_ptr(), self._d_B.data_ptr(),
+            self.n_items, d_cand_ptr.data_ptr(), d_cand_idx.data_ptr(), out.data_ptr(), _stream()))
+        return out
+
 
 class IALSRecommender(BaseMatrixFactorizationRecommender, Incremental_Training_Early_Stopping):
     """MatrixFactorization/IALSRecommender.py:19-213.  Factors live on the device in fp64; one `_run_epoch` is two calls
@@ -704,3 +781,13 @@ class IALSRecommender(BaseMatrixFactorizationRecommender, Incremental_Training_E
     def _update_best_model(self):
         self._prepare_model_for_validation()
         self.USER_factors_best, self.ITEM_factors_best = self.USER_factors.copy(), self.ITEM_factors.copy()
+
+
+# `_scores_device` of a model family -> its candidate scorer (BaseRecommender._candidate_scores_device).  Keyed by the
+# function itself: a class that overrides `_scores_device` finds no entry and is scored through its own block.
+_CANDIDATE_KERNELS = {
+    BaseItemSimilarityMatrixRecommender._scores_device: BaseItemSimilarityMatrixRecommender._candidate_scores_kernel,
+    BaseUserSimilarityMatrixRecommender._scores_device: BaseUserSimilarityMatrixRecommender._candidate_scores_kernel,
+    EASE_R_Recommender._scores_device: EASE_R_Recommender._candidate_scores_kernel,
+    BaseMatrixFactorizationRecommender._scores_device: BaseMatrixFactorizationRecommender._candidate_scores_kernel,
+}
