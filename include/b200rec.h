@@ -425,6 +425,33 @@ int b200_ials_half_epoch_device(const int32_t* d_rows, int n_solve, const int32_
                                 double* d_X, double* d_YtY_work, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * K8: non-negative matrix factorisation
+ * replaces  MatrixFactorization/NMFRecommender.py:33-60 -- sklearn NMF(init="random", alpha_W=0, shuffle=False).fit(URM) and
+ *           .transform(URM), i.e. _fit_multiplicative_update / _fit_coordinate_descent of sklearn/decomposition/_nmf.py
+ * One call runs one whole solve from the factors the caller put in d_W ([n_users, n_factors] row-major fp32) and d_Ht
+ * (H^T, [n_items, n_factors] row-major fp32), and leaves the result there:
+ *   update_h != 0: fit (W and H alternate; X^T is given as the CSR d_xt_* of the [n_items, n_users] transpose);
+ *   update_h == 0: transform (H fixed, d_xt_* may be NULL).
+ * X: the URM as CSR with sorted indices and no explicit zeros.  1 <= n_factors <= 512.  Every product accumulates in fp64.
+ * Stopping rules are sklearn's: mu tests sqrt(2 D(X, WH)) every 10 iterations when tol > 0 (tol == 0: exactly max_iter
+ * iterations, no test), cd stops when violation / violation_init <= tol or violation_init == 0.  *n_iter receives the
+ * iterations run, *last_error the last error evaluated (mu; 0 when tol == 0) or the last violation (cd).  Device workspace
+ * is allocated inside the call: about 4 * max(n_users, n_items) * n_factors bytes plus a few n_factors^2 doubles.
+ * The host reads one double per stopping test and nothing else during the iterations. */
+enum b200_nmf_solver { B200_NMF_MU = 0, B200_NMF_CD = 1 };
+enum b200_nmf_loss { B200_NMF_FROBENIUS = 0, B200_NMF_KL = 1 };
+int b200_nmf_solve_device(int solver, int beta_loss, int update_h, int n_users, int n_items, int n_factors, const int32_t* d_x_ptr,
+                          const int32_t* d_x_idx, const float* d_x_val, const int32_t* d_xt_ptr, const int32_t* d_xt_idx,
+                          const float* d_xt_val, float* d_W, float* d_Ht, int max_iter, double tol, int32_t* n_iter,
+                          double* last_error, void* stream);
+/* TEST HOOK for the two building blocks of the solve (M: [n_rows, n_factors] row-major fp32 on the device):
+ * op 0: d_out (fp32 [n_rows, n_factors]) = CSR (d_ptr, d_idx, d_val) with n_rows rows times M (M has as many rows as the
+ *       CSR has columns);
+ * op 1: d_out (fp64 [n_factors, n_factors]) = M^T M over the n_rows rows of M (CSR pointers unused). */
+int b200_nmf_debug_device(int op, int n_rows, int n_factors, const int32_t* d_ptr, const int32_t* d_idx, const float* d_val,
+                          const float* d_M, void* d_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * URM feature weighting in front of the KNN similarity  (SURVEY.md 8(f).3)
  * replaces  Base/IR_feature_weighting.py:13-51 okapi_BM_25 and :56-78 TF_IDF as KNN/ItemKNNCFRecommender.py:42-50 and
  *           KNN/UserKNNCFRecommender.py:43-51 apply them: weighting(URM.T).T -- items are the documents, users the terms.

@@ -118,6 +118,11 @@ SIGNATURES = {
                                                    ctypes.c_int, c_void, c_void, c_void, ctypes.c_int, c_void, c_void, c_void, c_void]),
     "b200_ials_half_epoch_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, ctypes.c_int, ctypes.c_int,
                                                    ctypes.c_double, c_void, c_void, c_void]),
+    "b200_nmf_solve_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                             c_void, c_void, c_void, c_void, c_void, c_void, c_void, c_void, ctypes.c_int,
+                                             ctypes.c_double, c_int_p, ctypes.POINTER(ctypes.c_double), c_void]),
+    "b200_nmf_debug_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void, c_void, c_void,
+                                             c_void]),
 }
 
 _lib = None

@@ -783,6 +783,95 @@ class IALSRecommender(BaseMatrixFactorizationRecommender, Incremental_Training_E
         self.USER_factors_best, self.ITEM_factors_best = self.USER_factors.copy(), self.ITEM_factors.copy()
 
 
+def nmf_random_init(X, n_components, random_state):
+    """W, H of sklearn's _initialize_nmf(X, n_components, init="random", random_state=random_state) (sklearn 1.9,
+    decomposition/_nmf.py), by the same numpy expressions: H is drawn first, then W, from check_random_state(random_state)
+    (None: numpy's global RandomState)."""
+    avg = np.sqrt(X.mean() / n_components)
+    if random_state is None:
+        rng = np.random.mtrand._rand
+    elif isinstance(random_state, np.random.RandomState):
+        rng = random_state
+    else:
+        rng = np.random.RandomState(random_state)
+    H = avg * rng.standard_normal(size=(n_components, X.shape[1])).astype(X.dtype, copy=False)
+    W = avg * rng.standard_normal(size=(X.shape[0], n_components)).astype(X.dtype, copy=False)
+    np.abs(H, out=H)
+    np.abs(W, out=W)
+    return W, H
+
+
+class NMFRecommender(BaseMatrixFactorizationRecommender):
+    """MatrixFactorization/NMFRecommender.py:15-60: sklearn NMF(init=init_type, solver=..., beta_loss=...).fit(URM_train), then
+    ITEM_factors = components_.T and USER_factors = transform(URM_train) -- a second solve with H fixed.  Both solves run on the
+    device (csrc/nmf.cu) as scikit-learn >= 1.2 runs them: alpha_W = 0, so l1_ratio is validated and stored only, max_iter
+    200, tol 1e-4, cd in component order.  init_type="random" is drawn on the host exactly like _initialize_nmf;
+    "nndsvda" needs a truncated SVD of the URM and is refused.  n_iter_ / n_iter_transform_ are the iterations of the solves."""
+    RECOMMENDER_NAME = "NMFRecommender"
+    SOLVER_VALUES = {"multiplicative_update": "mu", "coordinate_descent": "cd"}
+    INIT_VALUES = ["random", "nndsvda"]
+    BETA_LOSS_VALUES = ["frobenius", "kullback-leibler"]
+    MAX_ITER, TOL = 200, 1e-4
+
+    def fit(self, num_factors=100, l1_ratio=0.5, solver="multiplicative_update", init_type="random", beta_loss="frobenius",
+            verbose=False, random_seed=None):
+        assert l1_ratio >= 0 and l1_ratio <= 1, "{}: l1_ratio must be between 0 and 1, provided value was {}".format(
+            self.RECOMMENDER_NAME, l1_ratio)
+        if solver not in self.SOLVER_VALUES:
+            raise ValueError("Value for 'solver' not recognized. Acceptable values are {}, provided was '{}'".format(
+                self.SOLVER_VALUES.keys(), solver))
+        if init_type not in self.INIT_VALUES:
+            raise ValueError("Value for 'init_type' not recognized. Acceptable values are {}, provided was '{}'".format(
+                self.INIT_VALUES, init_type))
+        if beta_loss not in self.BETA_LOSS_VALUES:
+            raise ValueError("Value for 'beta_loss' not recognized. Acceptable values are {}, provided was '{}'".format(
+                self.BETA_LOSS_VALUES, beta_loss))
+        if self.SOLVER_VALUES[solver] == "cd" and beta_loss != "frobenius":  # NMF._check_params
+            raise ValueError("Invalid beta_loss parameter: solver 'cd' does not handle beta_loss = {!r}".format(beta_loss))
+        if init_type == "nndsvda":
+            raise NotImplementedError("NMFRecommender: init_type='nndsvda' is not on the CUDA path (it needs a truncated SVD of "
+                                      "the URM)")
+        self.num_factors, self.l1_ratio, self.solver, self.init_type, self.beta_loss = num_factors, l1_ratio, solver, init_type, beta_loss
+        self._print("Computing NMF decomposition...")
+        W, H = nmf_random_init(self.URM_train, num_factors, random_seed)
+        self.n_iter_, _ = self._solve(W, np.ascontiguousarray(H.T), update_h=True)
+        self.ITEM_factors = self._d_nmf_Ht.cpu().numpy()
+        # transform: BaseNMF._check_w_h(update_H=False) starts mu from avg and cd from zeros
+        if self.SOLVER_VALUES[solver] == "mu":
+            W0 = np.full((self.n_users, num_factors), np.sqrt(self.URM_train.mean() / num_factors), dtype=np.float32)
+        else:
+            W0 = np.zeros((self.n_users, num_factors), dtype=np.float32)
+        self.n_iter_transform_, _ = self._solve(W0, self.ITEM_factors, update_h=False)
+        self.USER_factors = self._d_nmf_W.cpu().numpy()
+        del self._d_nmf_W, self._d_nmf_Ht
+        self._print("Computing NMF decomposition... Done!")
+
+    def _solve(self, W, Ht, update_h, max_iter=None, tol=None):
+        """One sklearn solve (_fit_transform, update_H=update_h) on the device from the host factors W [n_users, f] and
+        Ht = H^T [n_items, f]; the results stay in self._d_nmf_W / self._d_nmf_Ht.  Returns (n_iter, last error or
+        violation)."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        d_xt = _dev_csr(self.URM_train.T) if update_h else None  # X^T as CSR, read by the H step only
+        self._d_nmf_W = torch.from_numpy(np.ascontiguousarray(W, np.float32)).to(dev)
+        self._d_nmf_Ht = torch.from_numpy(np.ascontiguousarray(Ht, np.float32)).to(dev)
+        return self._solve_device(d_xt, update_h, max_iter, tol)
+
+    def _solve_device(self, d_xt, update_h, max_iter=None, tol=None):
+        """The C call of _solve on the factors already in self._d_nmf_W / self._d_nmf_Ht (d_xt: X^T as device CSR, or
+        None for a transform)."""
+        x_ptr, x_idx, x_val = self._urm_device()
+        xt = tuple(t.data_ptr() for t in d_xt) if update_h else (None, None, None)
+        n_iter, last = ctypes.c_int32(), ctypes.c_double()
+        _lib.check(self._lib.b200_nmf_solve_device(
+            {"mu": 0, "cd": 1}[self.SOLVER_VALUES[self.solver]], {"frobenius": 0, "kullback-leibler": 1}[self.beta_loss],
+            int(update_h), self.n_users, self.n_items, self._d_nmf_W.shape[1], x_ptr.data_ptr(), x_idx.data_ptr(),
+            x_val.data_ptr(), xt[0], xt[1], xt[2], self._d_nmf_W.data_ptr(), self._d_nmf_Ht.data_ptr(),
+            int(self.MAX_ITER if max_iter is None else max_iter), float(self.TOL if tol is None else tol), ctypes.byref(n_iter),
+            ctypes.byref(last), _stream()))
+        return int(n_iter.value), float(last.value)
+
+
 # `_scores_device` of a model family -> its candidate scorer (BaseRecommender._candidate_scores_device).  Keyed by the
 # function itself: a class that overrides `_scores_device` finds no entry and is scored through its own block.
 _CANDIDATE_KERNELS = {
