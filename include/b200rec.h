@@ -452,6 +452,34 @@ int b200_nmf_debug_device(int op, int n_rows, int n_factors, const int32_t* d_pt
                           const float* d_M, void* d_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * K9: PureSVD -- scikit-learn's randomized truncated SVD
+ * replaces  MatrixFactorization/PureSVDRecommender.py:36-55 -- sklearn.utils.extmath.randomized_svd(URM, n_components=k,
+ *           random_state=seed) (n_oversamples 10, n_iter "auto", power_iteration_normalizer "auto", transpose "auto",
+ *           svd_flip), USER_factors = U, ITEM_factors = V diag(s).
+ * The host draws Omega (d_omega, [min(n_users, n_items), n_random] row-major fp32, n_random = k + 10 <= 512) and picks
+ * n_iter and transpose (n_users < n_items) by scikit-learn's rules; the call runs the rest.  It needs the URM as CSR
+ * (d_x_*) and the CSR of its transpose (d_xt_*, [n_items, n_users]).  It writes k' = min(k, n_users, n_items) components:
+ * d_user [n_users, k'] and d_item [n_items, k'] row-major fp32, d_s [k'] fp64, descending.  The power steps and the final
+ * basis are orthonormalised with SVQB (the same spans as scikit-learn's LU and QR), and B B^T's eigenpairs come from a
+ * parallel cyclic Jacobi method in fp64.  Device workspace: about 4 * (n_users + n_items) * n_random bytes plus a few
+ * n_random^2 doubles. */
+int b200_puresvd_device(int n_users, int n_items, const int32_t* d_x_ptr, const int32_t* d_x_idx, const float* d_x_val,
+                        const int32_t* d_xt_ptr, const int32_t* d_xt_idx, const float* d_xt_val, const float* d_omega, int n_random,
+                        int k, int n_iter, int transpose, float* d_user, float* d_item, double* d_s, void* stream);
+/* The CSR of the transpose of an [n_rows, n_cols] CSR on the device: d_out_ptr [n_cols + 1], d_out_idx / d_out_val [nnz].
+ * A stable radix sort of the column ids, so every output row lists its column ids in increasing order (scipy's
+ * .T.tocsr()).  Synchronises the stream before it returns. */
+int b200_csr_transpose_device(int n_rows, int n_cols, int64_t nnz, const int32_t* d_ptr, const int32_t* d_idx, const float* d_val,
+                              int32_t* d_out_ptr, int32_t* d_out_idx, float* d_out_val, void* stream);
+/* TEST HOOK for the building blocks of b200_puresvd_device (n_cols <= 512):
+ * op 0: d_a (fp32 [n_rows, n_cols]) is replaced by an orthonormal basis of its column span, SVQB with `arg` passes;
+ *       dropped directions are zero columns;
+ * op 1: d_a (fp64 [n_cols, n_cols], symmetric, n_rows == n_cols) -> d_b (fp64): the eigenvalues in descending order, then
+ *       the [n_cols, n_cols] row-major matrix whose column j is the eigenvector of eigenvalue j;
+ * op 2: svd_flip of d_a (fp32 [n_rows, n_cols], the side that decides) and d_b (fp32 [arg, n_cols]), both in place. */
+int b200_svd_debug_device(int op, int n_rows, int n_cols, int arg, void* d_a, void* d_b, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * URM feature weighting in front of the KNN similarity  (SURVEY.md 8(f).3)
  * replaces  Base/IR_feature_weighting.py:13-51 okapi_BM_25 and :56-78 TF_IDF as KNN/ItemKNNCFRecommender.py:42-50 and
  *           KNN/UserKNNCFRecommender.py:43-51 apply them: weighting(URM.T).T -- items are the documents, users the terms.

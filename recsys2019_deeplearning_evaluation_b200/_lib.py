@@ -123,6 +123,11 @@ SIGNATURES = {
                                              ctypes.c_double, c_int_p, ctypes.POINTER(ctypes.c_double), c_void]),
     "b200_nmf_debug_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void, c_void, c_void,
                                              c_void]),
+    "b200_puresvd_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, c_void, c_void, c_void, c_void, c_void, c_void, c_void,
+                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void, c_void]),
+    "b200_csr_transpose_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int64, c_void, c_void, c_void, c_void, c_void,
+                                                 c_void, c_void]),
+    "b200_svd_debug_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void]),
 }
 
 _lib = None

@@ -872,6 +872,70 @@ class NMFRecommender(BaseMatrixFactorizationRecommender):
         return int(n_iter.value), float(last.value)
 
 
+PURESVD_MAX_FACTORS = 502  # n_random = num_factors + 10 columns of the device sketch, at most 512
+
+
+def randomized_svd_sketch(shape, n_components, random_state):
+    """(transpose, n_iter, n_random, Omega) of sklearn's _randomized_svd(M, n_components, random_state=random_state) on a
+    float32 M of this shape (sklearn 1.9, utils/extmath.py), by the same rules and the same draw: n_random = n_components + 10,
+    n_iter = 7 if n_components < 0.1 min(shape) else 4, transpose = n_rows < n_cols, and Omega [min(shape), n_random] =
+    check_random_state(random_state).normal(...) cast to float32 (None: numpy's global RandomState).  The whole draw is
+    consumed, so the generator advances exactly as scikit-learn's does."""
+    n_random = n_components + 10
+    n_iter = 7 if n_components < 0.1 * min(shape) else 4
+    transpose = shape[0] < shape[1]
+    if random_state is None:
+        rng = np.random.mtrand._rand
+    elif isinstance(random_state, np.random.RandomState):
+        rng = random_state
+    else:
+        rng = np.random.RandomState(random_state)
+    omega = rng.normal(size=(min(shape), n_random)).astype(np.float32, copy=False)
+    return transpose, n_iter, n_random, np.ascontiguousarray(omega)
+
+
+class PureSVDRecommender(BaseMatrixFactorizationRecommender):
+    """MatrixFactorization/PureSVDRecommender.py:23-55: U, Sigma, VT = randomized_svd(URM_train, n_components=num_factors,
+    random_state=random_seed); USER_factors = U, ITEM_factors = (diag(Sigma) VT)^T.  The sketch is drawn on the host exactly
+    like scikit-learn's (randomized_svd_sketch); the range finder, the small SVD and svd_flip run on the device
+    (csrc/puresvd.cu).  min(num_factors, n_users, n_items) components are kept, as scikit-learn's slicing keeps them."""
+    RECOMMENDER_NAME = "PureSVDRecommender"
+
+    def fit(self, num_factors=100, random_seed=None):
+        if not 1 <= num_factors <= PURESVD_MAX_FACTORS:
+            raise ValueError("{}: num_factors must be between 1 and {} (the device sketch has at most 512 columns), provided "
+                             "was {}".format(self.RECOMMENDER_NAME, PURESVD_MAX_FACTORS, num_factors))
+        self._print("Computing SVD decomposition...")
+        self.USER_factors, self.ITEM_factors, _ = self._randomized_svd_device(num_factors, random_seed)
+        self.num_factors = num_factors
+        self._print("Computing SVD decomposition... Done!")
+
+    def _randomized_svd_device(self, num_factors, random_seed):
+        """(U [n_users, k'], V diag(s) [n_items, k'], s [k'] fp64) of randomized_svd(URM_train, num_factors, random_state=random_seed),
+        k' = min(num_factors, n_users, n_items); only the sketch is drawn on the host."""
+        import torch
+        transpose, n_iter, n_random, omega = randomized_svd_sketch(self.URM_train.shape, num_factors, random_seed)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        x_ptr, x_idx, x_val = self._urm_device()
+        nnz = int(self.URM_train.nnz)
+        xt_ptr = torch.empty(self.n_items + 1, dtype=torch.int32, device=dev)
+        xt_idx = torch.empty(nnz, dtype=torch.int32, device=dev)
+        xt_val = torch.empty(nnz, dtype=torch.float32, device=dev)
+        _lib.check(self._lib.b200_csr_transpose_device(self.n_users, self.n_items, nnz, x_ptr.data_ptr(), x_idx.data_ptr(),
+                                                       x_val.data_ptr(), xt_ptr.data_ptr(), xt_idx.data_ptr(), xt_val.data_ptr(),
+                                                       _stream()))
+        k = min(num_factors, self.n_users, self.n_items)
+        d_omega = torch.from_numpy(omega).to(dev)
+        U = torch.empty((self.n_users, k), dtype=torch.float32, device=dev)
+        V = torch.empty((self.n_items, k), dtype=torch.float32, device=dev)
+        s = torch.empty(k, dtype=torch.float64, device=dev)
+        _lib.check(self._lib.b200_puresvd_device(
+            self.n_users, self.n_items, x_ptr.data_ptr(), x_idx.data_ptr(), x_val.data_ptr(), xt_ptr.data_ptr(), xt_idx.data_ptr(),
+            xt_val.data_ptr(), d_omega.data_ptr(), n_random, num_factors, n_iter, int(transpose), U.data_ptr(), V.data_ptr(),
+            s.data_ptr(), _stream()))
+        return U.cpu().numpy(), V.cpu().numpy(), s.cpu().numpy()
+
+
 # `_scores_device` of a model family -> its candidate scorer (BaseRecommender._candidate_scores_device).  Keyed by the
 # function itself: a class that overrides `_scores_device` finds no entry and is scored through its own block.
 _CANDIDATE_KERNELS = {
