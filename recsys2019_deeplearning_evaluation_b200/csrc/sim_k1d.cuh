@@ -411,8 +411,12 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
 // Pair path: every co-occurrence count C[i][j] = C[j][i] is gathered once.
 //
 // The kernel above builds C[i][j] in pass i and again in pass j: it streams the whole row of every user of column i.  On a
-// call that covers every column, the upper pass streams only the part of each row after i (rows are sorted by the new
-// index), so pass i counts the neighbours j > i: half the gathered entries and half the shared atomics.  It writes column
+// call that covers every column, the upper pass counts each pair once, in a cyclic half window: pass i counts neighbour j
+// iff d = (j - i) mod n lies in [1, h], h = (n - 1) / 2, and, when n is even, the antipodal d = n / 2 for i < n / 2 only
+// (k1d_window_size).  Half the gathered entries and half the shared atomics, and -- unlike the j > i split, which gives
+// column 0 every neighbour and the last column none -- every pass needs at most n / 2 counters and gathers about half of
+// each of its rows.  Each user's row is stored twice, back to back (the indices, then the same indices + n), so that the
+// window of a CSC entry is one range of the doubled row.  It writes column
 // i's cells with count >= 3 as one contiguous own list and counts them into deg[j]; the exchange copies each cell into the
 // mirror list of j, so column c's candidates are its own list plus its mirror list, and the select kernel (one warp per
 // column) applies the rule of the kernel above to them: with at least K positive keys
@@ -421,13 +425,36 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
 // and norm terms, so the output is the same.  Every other column (fewer
 // than K candidates, count-2 / count-1 cells that matter, more than S_CAP candidates) is appended to a device
 // redo list that the kernel above then computes in full.  A counter overflow in the upper pass (the nibble checksum over
-// the suffix increments) or a full list sets a flag on the device, and the select kernel then hands EVERY column to
+// the window increments) or a full list sets a flag on the device, and the select kernel then hands EVERY column to
 // the kernel above: exactness never depends on the pair path.  Whether a handle takes the path at all is decided at create
 // time from the norm terms and the column lengths (k1d_pair_gate in sim_topk.cu): a column handed back costs a full pass
 // on top of the upper pass, so the path only pays when the select kernel can decide nearly every column.
 
-constexpr int U_STAGE = 2048;  // count >= 3 cells of one column staged in shared memory before one global reservation
-constexpr int U_STEPS = 1;     // loads of 32 chunks in flight per warp (more spill at 64 registers)
+// Launch shape of the upper pass: U_CTAS CTAs of U_THREADS threads per SM (half-window counters: 50 KB at 200 K columns),
+// so that several columns per SM are in different phases, and U_STEPS loads of 32 chunks in flight per warp.  The -D
+// overrides are for A/B builds (tools/build_variant.py).
+#ifndef B200_U_THREADS
+#define B200_U_THREADS 256
+#endif
+#ifndef B200_U_CTAS
+#define B200_U_CTAS 4
+#endif
+#ifndef B200_U_STEPS
+#define B200_U_STEPS 4
+#endif
+#ifndef B200_U_STAGE
+#define B200_U_STAGE 1024
+#endif
+constexpr int U_THREADS = B200_U_THREADS;
+constexpr int U_WARPS = U_THREADS / 32;
+constexpr int U_CTAS = B200_U_CTAS;
+constexpr int U_STEPS = B200_U_STEPS;
+constexpr int U_STAGE = B200_U_STAGE;  // count >= 3 cells of one column staged in shared memory before one global reservation
+
+// cells of pass c's window (see above); at most n / 2
+__host__ __device__ __forceinline__ int k1d_window_size(int n, int c) { return ((n - 1) >> 1) + ((n & 1) == 0 && c < (n >> 1) ? 1 : 0); }
+// counter words of the upper pass: every window, rounded to whole 16-byte vectors
+__host__ __device__ __forceinline__ int k1d_upper_words(int n) { return (((n >> 1) + 7) / 8 + 3) / 4 * 4; }
 // own_n flag: the column's cells overflowed its stage; the cells past it went to the loose list, so its own list is
 // incomplete and the select kernel hands the column to the redo list (it has more than S_CAP candidates anyway)
 constexpr int OWN_SPILLED = (int)0x80000000u;
@@ -437,15 +464,15 @@ struct K1DUpShared {
   unsigned long long base;
 };
 
-__global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KParams p) {
+__global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const KParams p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ K1DUpShared us;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int W = p.bm_words;
-  const int Wr = (p.n_cols + 7) >> 3;
+  const int n = p.n_cols;
+  const int W = k1d_upper_words(n);
   unsigned* acc = reinterpret_cast<unsigned*>(smem_raw);
   unsigned* stage = acc + W;
-  for (int i = tid; i < W; i += D_THREADS) acc[i] = 0u;
+  for (int i = tid; i < W; i += U_THREADS) acc[i] = 0u;
   if (blockIdx.x == 0 && tid == 0 && p.fail_every > 0) atomicExch(p.pair_fail, 1);  // test hook: exercises the fallback
   long long prof_t = p.prof ? clock64() : 0;
 
@@ -461,17 +488,19 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
     if (item >= p.n_range) break;
     const int4 wi = __ldg(p.worklist_up + item);
     const int col = wi.x, cs = wi.z, ce = wi.w;
+    const int size_c = k1d_window_size(n, col);
 
-    // ---------------- gather over the row suffixes: chunks that start at or before `col` are masked by j > col.  A suffix
-    // is half a row on average (C5: ~13 chunks), so one row per warp load would leave most lanes idle and issue as many
-    // loads and atomic instructions as the whole row; instead the 32 suffixes of a batch are one stream of chunks, every
+    // ---------------- gather over the row windows: cell t = j' - col - 1 of doubled-row index j', counted iff t < size_c,
+    // which masks the entries of the first and last chunk outside the window and the padding (INT_MAX).  A window is half a
+    // row on average (C5: ~13 chunks), so one row per warp load would leave most lanes idle and issue as many
+    // loads and atomic instructions as the whole row; instead the 32 windows of a batch are one stream of chunks, every
     // lane of every load busy.  Rows with chunks sit compacted in the low lanes; lane r holds row r's [beg, end) in the
     // stream, and the row of stream position f is the number of rows that end at or before f.
     int expect = 0;
-    for (int k0 = cs + warp * 32; k0 < ce; k0 += D_WARPS * 32) {
+    for (int k0 = cs + warp * 32; k0 < ce; k0 += U_WARPS * 32) {
       const int nrows = min(32, ce - k0);
       int2 seg = make_int2(0, 0);
-      if (lane < nrows) seg = __ldg(p.csc_suf + k0 + lane);
+      if (lane < nrows) seg = __ldg(p.csc_win + k0 + lane);
       expect += 4 * (seg.y >> 3) - (seg.y & 7);
       const unsigned nz = __ballot_sync(0xffffffffu, (seg.y >> 3) > 0);
       const int nr = __popc(nz);
@@ -504,8 +533,8 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
             const int jj[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
-              const int j = jj[c];
-              if (j < p.n_cols && j > col) atomicAdd(&acc[j >> 3], 1u << ((j & 7) << 2));
+              const unsigned t = (unsigned)(jj[c] - col - 1);
+              if (t < (unsigned)size_c) atomicAdd(&acc[t >> 3], 1u << ((t & 7) << 2));
             }
           }
         }
@@ -516,12 +545,12 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
     __syncthreads();
     PROF_MARK(8);
 
-    // ---------------- sweep of the words that hold j > col: checksum, count >= 3 cells into the stage (past it: the loose
-    // list), clear; every cell counts into deg[j] (fire-and-forget)
+    // ---------------- sweep of the window's words: checksum, count >= 3 cells into the stage (past it: the loose list), clear;
+    // every cell counts into deg[j] (fire-and-forget)
     {
       int ns = 0;
       uint4* acc4 = reinterpret_cast<uint4*>(acc);
-      for (int i4 = (((col + 1) >> 3) >> 2) + tid; i4 < ((Wr + 3) >> 2); i4 += D_THREADS) {
+      for (int i4 = tid; i4 < ((((size_c + 7) >> 3) + 3) >> 2); i4 += U_THREADS) {
         const uint4 w4 = acc4[i4];
         if (!(w4.x | w4.y | w4.z | w4.w)) continue;
         acc4[i4] = make_uint4(0u, 0u, 0u, 0u);
@@ -548,7 +577,8 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
             while (mm) {
               const int q = (__ffs(mm) - 1) >> 2;
               mm &= mm - 1;
-              const int j = (i4 * 4 + e) * 8 + q;
+              int j = col + 1 + (i4 * 4 + e) * 8 + q;
+              if (j >= n) j -= n;
               const unsigned cd = ((unsigned)j << 4) | ((ww[e] >> (q << 2)) & 15u);
               if (staged) {
                 stage[pos++] = cd;
@@ -577,7 +607,7 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_upper_kernel(const KPara
     __syncthreads();
     const unsigned long long base = us.base;
     if (base + nst <= (unsigned long long)p.pair_cap)
-      for (int t = tid; t < nst; t += D_THREADS) {
+      for (int t = tid; t < nst; t += U_THREADS) {
         const unsigned cd = stage[t];
         p.own[base + t] = cd;
         atomicAdd(p.deg + (cd >> 4), 1);
@@ -755,41 +785,57 @@ __global__ void k1d_tile_bounds_kernel(const int2* __restrict__ BN, int n_cols, 
   tb[t] = __int_as_float(BN[min(t << D_TILE_LOG2, n_cols - 1)].x);
 }
 
-// csc_seg[q] = where the padded single-window row of CSC entry q's user lives: x = start in 16-byte chunks,
-// y = chunks << 2 | padding entries in the last chunk (0..3)
-__global__ void k1d_csc_seg_kernel(const int* __restrict__ csc_idx, const int* __restrict__ split1, const int* __restrict__ csr_ptr,
-                                   long long nnz, int2* seg) {
-  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < nnz; q += (long long)gridDim.x * blockDim.x) {
-    const int u = csc_idx[q];
-    const int s = split1[2 * (size_t)u], e = split1[2 * (size_t)u + 1];
-    const int len = csr_ptr[u + 1] - csr_ptr[u];
-    seg[q] = make_int2(s >> 2, (((e - s) >> 2) << 2) | ((e - s) - len));
-  }
+// The K1-D row layout: every user's sorted row `copies` times back to back (copies = 2: the indices, then the same indices
+// + n_cols, so that the upper pass's cyclic window of an entry is one range of positions), padded to 16-byte chunks with
+// INT_MAX, which no window or neighbour test accepts.  len4[u] = the padded length; idx1 from its exclusive scan poff.
+__global__ void k1d_row_len_kernel(const int* __restrict__ csr_ptr, int n_rows, int copies, int* len4) {
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u < n_rows) len4[u] = (copies * (csr_ptr[u + 1] - csr_ptr[u]) + 3) & ~3;
 }
 
-// csc_suf[q] = the suffix of CSC entry q's padded row after the entry's column c, for the upper pass (csc_pos[q] = the
-// entry's position in the CSR, so its place in the user's row is csc_pos[q] - csr_ptr[u]).  x = start in 16-byte chunks of the chunk that holds the next
-// position, y = chunks << 3 | entries of those chunks that produce no increment (the ones at or before c, and the padding;
-// 0..6).  suf_work[c] = the increments of all of column c's suffixes, the work of its upper pass (sort key of the upper
-// pass's longest-first order, with iota[c] = c as the value).  One warp per column.
-__global__ void k1d_csc_suffix_kernel(const int* __restrict__ csc_ptr, const int* __restrict__ csc_idx, const int* __restrict__ csr_ptr,
-                                      const int* __restrict__ csc_pos, const int* __restrict__ split1, int n_cols, int2* suf,
-                                      unsigned long long* suf_work, int* iota) {
+__global__ void k1d_row_fill_kernel(const int* __restrict__ csr_ptr, const int* __restrict__ csr_idx, const int* __restrict__ poff,
+                                    int n_rows, int copies, int n_cols, int* idx1) {
+  const int u = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 3);  // 8 lanes per row
+  if (u >= n_rows) return;
+  const int r0 = csr_ptr[u], len = csr_ptr[u + 1] - r0, s = poff[u], n4 = poff[u + 1] - s;
+  for (int t = (threadIdx.x & 7); t < n4; t += 8)
+    idx1[s + t] = t < len ? csr_idx[r0 + t] : (t < copies * len ? csr_idx[r0 + t - len] + n_cols : INT_MAX);
+}
+
+// Per CSC entry q (user u, column c; csc_pos[q] = its position in the CSR, so its place in u's row is k = csc_pos[q] - r0):
+// csc_seg[q] = u's whole row for the K1-D kernel: x = start in 16-byte chunks, y = chunks << 2 | entries of the last chunk
+// past the row (0..3; second-copy entries or padding).  With a doubled layout (win != nullptr) also win[q] = the entry's
+// window for the upper pass, positions k + 1 .. (last one <= c + size_c) of the doubled row: x = start in 16-byte chunks,
+// y = chunks << 3 | entries of those chunks that produce no increment (0..6), and win_work[c] = the increments of all of
+// column c's windows (sort key of the upper pass's longest-first order, with iota[c] = c as the value).  One warp per column.
+__global__ void k1d_csc_rows_kernel(const int* __restrict__ csc_ptr, const int* __restrict__ csc_idx, const int* __restrict__ csr_ptr,
+                                    const int* __restrict__ csc_pos, const int* __restrict__ poff, const int* __restrict__ idx1,
+                                    int n_cols, int2* seg, int2* win, unsigned long long* win_work, int* iota) {
   const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (c >= n_cols) return;
+  const int bound = c + k1d_window_size(n_cols, c);
   unsigned long long w = 0;
   for (int q = csc_ptr[c] + lane; q < csc_ptr[c + 1]; q += 32) {
     const int u = csc_idx[q];
-    const int r0 = csr_ptr[u], len = csr_ptr[u + 1] - r0;
-    const int next = csc_pos[q] - r0 + 1;
-    const int s = split1[2 * (size_t)u], e = split1[2 * (size_t)u + 1];
-    const int nch = ((e - s) >> 2) - (next >> 2);
-    suf[q] = make_int2((s >> 2) + (next >> 2), nch > 0 ? (nch << 3) | ((next & 3) + (e - s) - len) : 0);
-    w += (unsigned long long)(len - next);
+    const int r0 = csr_ptr[u], len = csr_ptr[u + 1] - r0, s = poff[u];
+    const int nch = (len + 3) >> 2;
+    seg[q] = make_int2(s >> 2, (nch << 2) | (4 * nch - len));
+    if (!win) continue;
+    // the window ends before the first position in (k, k + len) whose index exceeds c + size_c (position k + len holds c + n)
+    const int k = csc_pos[q] - r0;
+    int lo = k + 1, hi = k + len;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (idx1[s + mid] <= bound) lo = mid + 1; else hi = mid;
+    }
+    const int wch = ((lo + 3) >> 2) - ((k + 1) >> 2);
+    win[q] = lo > k + 1 ? make_int2((s >> 2) + ((k + 1) >> 2), (wch << 3) | (4 * wch - (lo - k - 1))) : make_int2(0, 0);
+    w += (unsigned long long)(lo - k - 1);
   }
+  if (!win) return;
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
-  if (lane == 0) { suf_work[c] = w; iota[c] = c; }
+  if (lane == 0) { win_work[c] = w; iota[c] = c; }
 }
 
 // the upper pass's work list: every column (new numbering, in the order `perm`) as (new column, original column, csc range)

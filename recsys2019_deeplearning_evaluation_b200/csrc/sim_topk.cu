@@ -107,8 +107,8 @@ struct KParams {
   int eu_mode, eu_norm, eu_signed;
   float eu_div, eu_shrink;
   float* dense_out;  // dense mode (TopK == 0 / full Gram): [n_range, n_cols] row-major, out[target - col_begin, neighbour]
-  // K1-D (sim_k1d.cuh): 4-bit counter words, key-buffer slots, norm tiles and their bounds, the n_win = 1 padded row
-  // layout with the CSC-side (row start, row chunks) list, the work items of the launch (new column, local column, csc
+  // K1-D (sim_k1d.cuh): 4-bit counter words, key-buffer slots, norm tiles and their bounds, the padded (doubled when the
+  // pair path can use it) row layout with the CSC-side (row start, row chunks) list, the work items of the launch (new column, local column, csc
   // begin, csc end), the list + counter that receive the columns to redo, and a test hook (every n-th column is handed back)
   int bm_words, cap_d, fail_every, ntile;
   const float* __restrict__ tbnd;
@@ -118,13 +118,13 @@ struct KParams {
   int* redo;
   int* fail;
   const int* n_range_dev;  // window kernel / K1-D kernel: the number of columns to process is read from here when set
-  // K1-D pair path (sim_k1d.cuh): per CSC entry the suffix of the user's padded row after the column, the work items in
-  // suffix-work order; the own lists (column i's count >= 3 cells (j << 4 | count), j > i, one contiguous run per column:
+  // K1-D pair path (sim_k1d.cuh): per CSC entry the column's window in the user's doubled row, the work items in
+  // window-work order; the own lists (column i's count >= 3 cells (j << 4 | count), j in i's window, one contiguous run per column:
   // start and length by column), their capacity and fill; the loose list of (i << 32 | j << 4 | count) cells that did not fit
   // a column's stage, its capacity and fill; the per-column mirror counts (deg) and offsets and the mirror lists built from
   // them ((i << 4 | count) in the list of j); the flag that sends the whole call down the K1-D kernel, and the columns that
   // the select kernel hands to the K1-D kernel
-  const int2* __restrict__ csc_suf;
+  const int2* __restrict__ csc_win;
   const int4* __restrict__ worklist_up;
   unsigned* own;
   int* own_off;
@@ -1247,11 +1247,11 @@ struct b200_sim_s {
   std::vector<int> h_old2new, h_csc_ptr;
   int n_sparse_last = 0, n_dense_last = 0;
   std::vector<unsigned long long> h_work;  // by ORIGINAL column index
-  // K1-D pair path (sim_k1d.cuh): row suffixes, the upper pass's work list (every column), own lists (capacity from the
+  // K1-D pair path (sim_k1d.cuh): row windows, the upper pass's work list (every column), own lists (capacity from the
   // expected pair count) with their per-column start and length, loose list, mirror lists (deg: per-column counts, zero
   // between calls), control words (own and loose fill, fallback flag, redo count), redo list, scan scratch (all allocated
   // by the first call that takes the path), the select kernel's level bounds, upper-pass geometry
-  DevBuf<int2> csc_suf;
+  DevBuf<int2> csc_win;
   DevBuf<int4> worklist_up, wl_redo;
   DevBuf<unsigned> own, mir;
   DevBuf<u64> loose;
@@ -1592,8 +1592,8 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     const long long total = (long long)n_rows * (n_win + 1);
     split_kernel<<<div_up(total, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), n_rows, n_win, win, h->split.get()); count_launch();
   }
-  DevBuf<unsigned long long> suf_work;  // K1-D upper-pass work per new column, and the new column indices
-  DevBuf<int> suf_iota;
+  DevBuf<unsigned long long> win_work;  // K1-D upper-pass work per new column, and the new column indices
+  DevBuf<int> win_iota;
   if (h->binary) {  // padded, 16-byte aligned (row, window) segments
     const long long n_seg = (long long)n_rows * n_win;
     B200_REQUIRE((long long)nnz + 3 * n_seg < (1ll << 31), "matrix too large for 32-bit positions in the padded row layout");
@@ -1614,13 +1614,12 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     const bool f_ok_c = h->formula == F_PROD || h->formula == F_NONORM || h->formula == F_JACCARD || h->formula == F_DICE ||
                         (h->formula == F_TVERSKY && h->ta >= 0.f && h->tb >= 0.f);  // decreasing in the neighbour's norm term
     if (h->want_k1c && f_ok_c && nnz > 0 && n_cols >= h->k1c_min_cols) {
-      // K1-D layout: the same rows once more as ONE window -- whole rows padded to 16-byte chunks with the index win1
-      // (>= n_cols) -- and, per CSC entry, where its user's padded row lives (start, length in 16-byte chunks)
-      const int win1 = ((n_cols + 7) / 8) * 8;
-      DevBuf<int> sp1((size_t)n_rows * 2), len1((size_t)n_rows + 1), poff1((size_t)n_rows + 1), split1((size_t)n_rows * 2);
-      split_kernel<<<div_up((long long)n_rows * 2, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), n_rows, 1, win1, sp1.get()); count_launch();
+      // K1-D layout (k1d_row_fill_kernel): every row twice, back to back, for the pair path's windows -- once when the doubled
+      // layout would not fit 32-bit positions: the K1-D kernel reads only the first copy, and the handle does not take the pair path
+      const int copies = 2 * (long long)nnz + 3ll * n_rows < (1ll << 31) ? 2 : 1;
+      DevBuf<int> len1((size_t)n_rows + 1), poff1((size_t)n_rows + 1);
       B200_CUDA(cudaMemsetAsync(len1.get() + n_rows, 0, sizeof(int), st));
-      seg_len_kernel<<<div_up(n_rows, 256), 256, 0, st>>>(sp1.get(), n_rows, 1, len1.get()); count_launch();
+      k1d_row_len_kernel<<<div_up(n_rows, 256), 256, 0, st>>>(h->csr_ptr.get(), n_rows, copies, len1.get()); count_launch();
       size_t tb1 = 0;
       B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb1, len1.get(), poff1.get(), n_rows + 1, st));
       DevBuf<unsigned char> tmp1(tb1 + 16);
@@ -1629,17 +1628,19 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       B200_CUDA(cudaMemcpyAsync(&total1, poff1.get() + n_rows, sizeof(int), cudaMemcpyDeviceToHost, st));
       B200_CUDA(cudaStreamSynchronize(st));
       h->csr_idx1.alloc((size_t)total1 + 8);
-      seg_pad_kernel<<<div_up((long long)n_rows * 8, 256), 256, 0, st>>>(sp1.get(), h->csr_idx.get(), poff1.get(), n_rows, 1, win1, total1,
-                                                                        h->csr_idx1.get(), split1.get()); count_launch();
+      k1d_row_fill_kernel<<<div_up((long long)n_rows * 8, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), poff1.get(), n_rows,
+                                                                             copies, n_cols, h->csr_idx1.get()); count_launch();
       h->csc_seg.alloc((size_t)nnz + 2);
       B200_CUDA(cudaMemsetAsync(h->csc_seg.get() + nnz, 0, 2 * sizeof(int2), st));
-      k1d_csc_seg_kernel<<<GRID1D, 256, 0, st>>>(h->csc_idx.get(), split1.get(), h->csr_ptr.get(), nnz, h->csc_seg.get()); count_launch();
-      h->csc_suf.alloc((size_t)nnz);
-      suf_work.alloc((size_t)n_cols);
-      suf_iota.alloc((size_t)n_cols);
-      k1d_csc_suffix_kernel<<<div_up((long long)n_cols * 32, 256), 256, 0, st>>>(h->csc_ptr.get(), h->csc_idx.get(), h->csr_ptr.get(),
-                                                                                 csc_pos.get(), split1.get(), n_cols, h->csc_suf.get(),
-                                                                                 suf_work.get(), suf_iota.get()); count_launch();
+      if (copies == 2) {
+        h->csc_win.alloc((size_t)nnz);
+        win_work.alloc((size_t)n_cols);
+        win_iota.alloc((size_t)n_cols);
+      }
+      k1d_csc_rows_kernel<<<div_up((long long)n_cols * 32, 256), 256, 0, st>>>(h->csc_ptr.get(), h->csc_idx.get(), h->csr_ptr.get(),
+                                                                               csc_pos.get(), poff1.get(), h->csr_idx1.get(), n_cols,
+                                                                               h->csc_seg.get(), h->csc_win.get(), win_work.get(),
+                                                                               win_iota.get()); count_launch();
       B200_CUDA(cudaStreamSynchronize(st));
     }
     h->csr_idx = std::move(idx_pad);
@@ -1703,14 +1704,14 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       // second CTA of an SM never becomes resident
       B200_CUDA(cudaFuncSetAttribute(k1d_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
 
-      // pair path: the upper pass needs the counters and the stage (two CTAs per SM when both fit, like the K1-D kernel), and
-      // it only pays when the select kernel can decide most columns itself (k1d_pair_gate); its buffers are allocated by the
-      // first call that takes it
+      // pair path: needs the doubled row layout; the upper pass needs the half-window counters and the stage (up to U_CTAS
+      // CTAs per SM as they fit), and it only pays when the select kernel can decide most columns itself (k1d_pair_gate); its
+      // buffers are allocated by the first call that takes it
       cudaFuncAttributes fu{};
       B200_CUDA(cudaFuncGetAttributes(&fu, sim_k1d_upper_kernel));
-      h->smem_up_bytes = ((size_t)h->bm_words + U_STAGE) * 4;
+      h->smem_up_bytes = ((size_t)k1d_upper_words(n_cols) + U_STAGE) * 4;
       h->ctas_up = 0;
-      for (int ctas = 2; ctas >= 1 && h->ctas_up == 0; --ctas)
+      for (int ctas = U_CTAS; ctas >= 1 && h->ctas_up == 0 && h->csc_win.n > 0; --ctas)
         if ((long long)h->smem_up_bytes <= std::min<long long>((long long)sm_total / ctas - 1024, (long long)max_smem) - (long long)fu.sharedSizeBytes)
           h->ctas_up = ctas;
       if (h->ctas_up > 0 && !k1d_pair_gate(h, cnt_new.get(), st)) h->ctas_up = 0;
@@ -1720,13 +1721,13 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
         B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_WARPS * sizeof(SelWarp))));
         B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         h->worklist_up.alloc((size_t)n_cols);
-        // the upper pass's longest-first order: every column by descending suffix work (empty columns do nothing there)
+        // the upper pass's longest-first order: every column by descending window work (empty columns do nothing there)
         DevBuf<unsigned long long> keys_out((size_t)n_cols);
         DevBuf<int> perm((size_t)n_cols);
         size_t tb = 0;
-        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, suf_work.get(), keys_out.get(), suf_iota.get(), perm.get(), n_cols, 0, 64, st));
+        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
         DevBuf<unsigned char> tmp(tb + 16);
-        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tb, suf_work.get(), keys_out.get(), suf_iota.get(), perm.get(), n_cols, 0, 64, st));
+        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
         k1d_upper_worklist_kernel<<<div_up(n_cols, 256), 256, 0, st>>>(perm.get(), h->BN.get(), h->csc_ptr.get(), n_cols, h->worklist_up.get());
         count_launch(5);
         B200_CUDA(cudaStreamSynchronize(st));
@@ -1734,7 +1735,7 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     }
   }
   if (!h->k1c) { h->csr_idx1.release(); h->csc_seg.release(); }
-  if (h->ctas_up == 0) h->csc_suf.release();
+  if (h->ctas_up == 0) h->csc_win.release();
 }
 
 }  // namespace
@@ -1920,7 +1921,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.csr_idx1 = h->csr_idx1.get(); p.csc_seg = h->csc_seg.get(); p.worklist = h->worklist.get();
   p.redo = h->order.get(); p.fail = h->fail.get();
   p.n_range_dev = nullptr;
-  p.csc_suf = h->csc_suf.get(); p.worklist_up = h->worklist_up.get();
+  p.csc_win = h->csc_win.get(); p.worklist_up = h->worklist_up.get();
   if (pair_path && h->own.n == 0) {
     // first call on the pair path: the own lists hold twice the expected pairs (a fuller list sets the fallback flag), the
     // loose list (cells past a column's stage: rare) a quarter of that, the mirror lists both; positions stay below 2^31
@@ -1954,7 +1955,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     B200_CUDA(cudaMemsetAsync(h->pair_ctl.get(), 0, 6 * sizeof(int), st));
     KParams q = p;
     q.n_range = h->n_cols;  // the upper pass's work list holds every column
-    sim_k1d_upper_kernel<<<std::min(h->n_cols, h->n_sm * h->ctas_up), D_THREADS, h->smem_up_bytes, st>>>(q);
+    sim_k1d_upper_kernel<<<std::min(h->n_cols, h->n_sm * h->ctas_up), U_THREADS, h->smem_up_bytes, st>>>(q);
     q.n_range = n_sparse;
     B200_CUDA(cudaGetLastError());
     size_t tb = h->scan_tmp_bytes;
