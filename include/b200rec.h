@@ -506,6 +506,7 @@ enum b200_eval_slot {
   B200_EVAL_PRECISION = 0, B200_EVAL_PRECISION_RECALL_MIN_DEN = 1, B200_EVAL_RECALL = 2, B200_EVAL_MAP = 3,
   B200_EVAL_MAP_MIN_DEN = 4, B200_EVAL_MRR = 5, B200_EVAL_NDCG = 6, B200_EVAL_HIT_RATE = 7, B200_EVAL_ARHR = 8,
   B200_EVAL_NOVELTY = 9, B200_EVAL_AVERAGE_POPULARITY = 10, B200_EVAL_USERS_WITH_RECS = 11, B200_EVAL_N_USERS = 12,
+  B200_EVAL_DIVERSITY_SIMILARITY = 13, B200_EVAL_SHORT_LISTS = 14,
   B200_EVAL_NACC = 16
 };
 int b200_eval_accumulate_device(const int32_t* d_users, int n_block, const int32_t* d_rec_items, const float* d_rec_scores,
@@ -513,6 +514,19 @@ int b200_eval_accumulate_device(const int32_t* d_users, int n_block, const int32
                                 const float* d_test_val, const int32_t* d_cutoffs, int n_cutoffs, const double* d_idcg,
                                 const double* d_item_novelty, const double* d_item_pop_norm, int n_items, double* d_acc,
                                 int32_t* d_rec_count, int32_t* d_hit_count, void* stream);
+
+/* Intra-list diversity, Diversity_similarity.add_recommendations (metrics.py:719-775), for one block of users.
+ * d_rec_items / d_rec_scores: the same [n_block, max_cutoff] tables and the same list rule as b200_eval_accumulate_device
+ * (the finite-score entries, in table order).  d_div: a dense row-major [n_items, n_items] matrix D of floats, or of doubles
+ * when div_fp64 != 0; every list item must be below n_items.  For every cutoff c with list r of length L = min(c, len):
+ *   value = S / (L (L - 1)),  S = sum over a <= L - 2 and b <= L - 1, b != a, of D[r_a, r_b]
+ * (the reference's row loop stops at L - 2, so row r_{L-1} never contributes while column r_{L-1} does).  S is summed in
+ * fp64 in a fixed order per user; value is added to d_acc[c, B200_EVAL_DIVERSITY_SIMILARITY].  A list with L < 2 (where
+ * the reference divides 0.0 by 0) adds 1 to d_acc[c, B200_EVAL_SHORT_LISTS] instead.  (L_max - 1)^2 reads of D per user,
+ * L_max the longest of the user's lists over the cutoffs. */
+int b200_eval_diversity_device(const int32_t* d_rec_items, const float* d_rec_scores, int n_block, int max_cutoff,
+                               const int32_t* d_cutoffs, int n_cutoffs, const void* d_div, int div_fp64, int n_items,
+                               double* d_acc, void* stream);
 
 #ifdef __cplusplus
 }

@@ -116,6 +116,8 @@ SIGNATURES = {
                                                      ctypes.c_float, ctypes.c_float, c_void]),
     "b200_eval_accumulate_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, ctypes.c_int, c_void, c_void, c_void, c_void,
                                                    ctypes.c_int, c_void, c_void, c_void, ctypes.c_int, c_void, c_void, c_void, c_void]),
+    "b200_eval_diversity_device": (ctypes.c_int, [c_void, c_void, ctypes.c_int, ctypes.c_int, c_void, ctypes.c_int, c_void, ctypes.c_int,
+                                                  ctypes.c_int, c_void, c_void]),
     "b200_ials_half_epoch_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, ctypes.c_int, ctypes.c_int,
                                                    ctypes.c_double, c_void, c_void, c_void]),
     "b200_nmf_solve_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,

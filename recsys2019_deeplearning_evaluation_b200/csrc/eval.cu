@@ -12,7 +12,8 @@
 // hit flag / gain of every recommendation is found by a binary search in the user's sorted test row, hits are
 // prefix-summed with ballots, then every cutoff (any number, any order) reduces its prefix of the list.  Sums go to fp64
 // accumulators with atomics; nothing returns to the host until the evaluation ends.  HBM-bound on the list table (4 B per
-// position) and the test rows.
+// position) and the test rows.  DIVERSITY_SIMILARITY (Diversity_similarity :719, a dense item x item matrix) has a kernel
+// of its own below, launched on the same table only when the evaluator was given a diversity object.
 #include "common.cuh"
 
 namespace b200 {
@@ -20,6 +21,22 @@ namespace eval {
 
 constexpr int WARPS = 4;
 constexpr int MAXCUT = 1024;  // list positions per user (b200_score_topn_device's limit)
+
+// The one definition of a user's recommendation list, shared by every kernel here.  A warp walks the table row
+// srow / row 32 positions per step (p0 = 0, 32, ...): the lane's entry is a recommendation iff its score is finite
+// (BaseRecommender.py:203-207 drops the rest from the first max_cutoff positions), and the recommendations are compacted
+// to list positions 0..len-1 in table order, so +inf entries before them and NaN / -inf entries among them take no
+// position.  Returns the lane's item (-1 if none) and its list position in `pos`; advances `len` for the whole warp.
+__device__ __forceinline__ int list_step(const int* row, const float* srow, int max_cutoff, int p0, int lane, int& len,
+                                         int& pos) {
+  const int p = p0 + lane;
+  int item = -1;
+  if (p < max_cutoff && isfinite(srow[p])) item = row[p];
+  const unsigned valid_mask = __ballot_sync(0xffffffffu, item >= 0);
+  pos = len + __popc(valid_mask & ((1u << lane) - 1u));
+  len += __popc(valid_mask);
+  return item;
+}
 
 __global__ void __launch_bounds__(WARPS * 32) metrics_kernel(
     const int* __restrict__ users, int n_block, const int* __restrict__ rec, const float* __restrict__ rec_score, int max_cutoff,
@@ -37,14 +54,11 @@ __global__ void __launch_bounds__(WARPS * 32) metrics_kernel(
   const int n_test = te - ts;
   const int* row = rec + (size_t)b * max_cutoff;
   const float* srow = rec_score + (size_t)b * max_cutoff;
-  // ---- phase 1: hit / gain per recommendation, running hit count, list length.  Only entries with a finite score are
-  // recommendations (BaseRecommender.py:203-207 drops the rest from the first max_cutoff positions); they are compacted
-  // to positions 0..len-1 in table order, so +inf entries before them and NaN / -inf entries among them take no position.
+  // ---- phase 1: hit / gain per recommendation, running hit count, list length (the list of list_step)
   int carry = 0, len = 0;
   for (int p0 = 0; p0 < max_cutoff; p0 += 32) {
-    const int p = p0 + lane;
-    int item = -1;
-    if (p < max_cutoff && isfinite(srow[p])) item = row[p];
+    int q;  // position among the recommendations
+    const int item = list_step(row, srow, max_cutoff, p0, lane, len, q);
     int hit = 0;
     float gain = 0.f;
     if (item >= 0) {
@@ -55,15 +69,12 @@ __global__ void __launch_bounds__(WARPS * 32) metrics_kernel(
       }
       if (lo < te && t_idx[lo] == item) { hit = 1; gain = exp2f(t_val[lo]) - 1.f; }
     }
-    const unsigned valid_mask = __ballot_sync(0xffffffffu, item >= 0);
     const unsigned hit_mask = __ballot_sync(0xffffffffu, hit);
     if (item >= 0) {
-      const int q = len + __popc(valid_mask & ((1u << lane) - 1u));  // position among the recommendations
       s_item[w][q] = item;
       s_gain[w][q] = gain;
       s_cum[w][q] = (unsigned short)(carry + __popc(hit_mask & (0xffffffffu >> (31 - lane))));
     }
-    len += __popc(valid_mask);
     carry += __popc(hit_mask);
   }
   __syncwarp();
@@ -126,6 +137,70 @@ __global__ void __launch_bounds__(WARPS * 32) metrics_kernel(
   }
 }
 
+// ---- intra-list diversity (Diversity_similarity.add_recommendations, metrics.py:733-741)
+// S(L) = sum over a <= L-2, b <= L-1, b != a of D[r_a, r_b].  A term (a, b) first appears at list length
+// max(a + 2, b + 1), so with e = max(a + 1, b) the terms fall into buckets
+//   T_e = sum_{b <= e, b != e-1} D[r_{e-1}, r_b] + sum_{a <= e-2} D[r_a, r_e]      (2e - 1 terms, e >= 1)
+// and S(L) = T_1 + ... + T_{L-1} for every L at once.  One CTA per user: warp 0 puts the list in shared memory, the warps
+// take the buckets e = 1 .. L_max - 1 in turn, so each term of D is read once ((L_max - 1)^2 reads, one 32-byte sector
+// each at worst), and then every cutoff sums its buckets.  Each sum runs in a fixed order (lane-strided, then a shuffle
+// tree), so a user's S does not depend on scheduling; across users values meet in fp64 atomics, like metrics_kernel's.
+constexpr int DIV_WARPS = 8;
+
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  return v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(DIV_WARPS * 32) diversity_kernel(
+    const int* __restrict__ rec, const float* __restrict__ rec_score, int max_cutoff, const int* __restrict__ cutoffs, int n_cut,
+    const T* __restrict__ D, int n_items, double* acc) {
+  __shared__ int s_item[MAXCUT];
+  __shared__ double s_bucket[MAXCUT];  // T_e
+  __shared__ int s_len;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (w == 0) {
+    const int* row = rec + (size_t)blockIdx.x * max_cutoff;
+    const float* srow = rec_score + (size_t)blockIdx.x * max_cutoff;
+    int len = 0;
+    for (int p0 = 0; p0 < max_cutoff; p0 += 32) {
+      int q;
+      const int item = list_step(row, srow, max_cutoff, p0, lane, len, q);
+      if (item >= 0) s_item[q] = item;
+    }
+    if (lane == 0) s_len = len;
+  }
+  __syncthreads();
+  const int len = s_len;
+  int lmax = 0;
+  for (int ci = 0; ci < n_cut; ++ci) lmax = max(lmax, min(cutoffs[ci], len));
+  for (int e = 1 + w; e < lmax; e += DIV_WARPS) {
+    const T* drow = D + (size_t)s_item[e - 1] * n_items;  // row r_{e-1}
+    const int re = s_item[e];                              // column r_e
+    double t = 0.0;
+#pragma unroll 4
+    for (int b = lane; b <= e; b += 32) t += b == e - 1 ? 0.0 : (double)drow[s_item[b]];
+#pragma unroll 4
+    for (int a = lane; a <= e - 2; a += 32) t += (double)D[(size_t)s_item[a] * n_items + re];
+    t = warp_sum(t);
+    if (lane == 0) s_bucket[e] = t;
+  }
+  __syncthreads();
+  for (int ci = w; ci < n_cut; ci += DIV_WARPS) {
+    const int L = min(cutoffs[ci], len);
+    double s = 0.0;
+    for (int e = 1 + lane; e < L; e += 32) s += s_bucket[e];
+    s = warp_sum(s);
+    if (lane == 0) {
+      double* a = acc + (size_t)ci * B200_EVAL_NACC;
+      if (L < 2) atomicAdd(a + B200_EVAL_SHORT_LISTS, 1.0);
+      else atomicAdd(a + B200_EVAL_DIVERSITY_SIMILARITY, s / ((double)L * (double)(L - 1)));
+    }
+  }
+}
+
 }  // namespace eval
 }  // namespace b200
 
@@ -148,6 +223,26 @@ int b200_eval_accumulate_device(const int32_t* d_users, int n_block, const int32
     eval::metrics_kernel<<<div_up(n_block, eval::WARPS), eval::WARPS * 32, 0, (cudaStream_t)stream>>>(
         d_users, n_block, d_rec_items, d_rec_scores, max_cutoff, d_test_ptr, d_test_idx, d_test_val, d_cutoffs, n_cutoffs, d_idcg,
         d_item_novelty, d_item_pop_norm, n_items, d_acc, d_rec_count, d_hit_count);
+    B200_CUDA(cudaGetLastError());
+    count_launch();
+  });
+}
+
+int b200_eval_diversity_device(const int32_t* d_rec_items, const float* d_rec_scores, int n_block, int max_cutoff,
+                               const int32_t* d_cutoffs, int n_cutoffs, const void* d_div, int div_fp64, int n_items,
+                               double* d_acc, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(d_rec_items && d_rec_scores && d_cutoffs && d_div && d_acc, "b200_eval_diversity: NULL argument");
+    B200_REQUIRE(max_cutoff >= 1 && max_cutoff <= eval::MAXCUT, "b200_eval_diversity: max_cutoff must be in [1, %d]", eval::MAXCUT);
+    B200_REQUIRE(n_cutoffs >= 1 && n_items > 0 && n_block >= 0, "b200_eval_diversity: bad shape");
+    if (n_block == 0) return;
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (div_fp64)
+      eval::diversity_kernel<double><<<n_block, eval::DIV_WARPS * 32, 0, s>>>(
+          d_rec_items, d_rec_scores, max_cutoff, d_cutoffs, n_cutoffs, static_cast<const double*>(d_div), n_items, d_acc);
+    else
+      eval::diversity_kernel<float><<<n_block, eval::DIV_WARPS * 32, 0, s>>>(
+          d_rec_items, d_rec_scores, max_cutoff, d_cutoffs, n_cutoffs, static_cast<const float*>(d_div), n_items, d_acc);
     B200_CUDA(cudaGetLastError());
     count_launch();
   });

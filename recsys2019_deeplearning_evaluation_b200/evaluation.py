@@ -11,7 +11,11 @@ the host only combines the final sums and the per-item recommendation counters (
 
 `EvaluatorNegativeItemSample` (Evaluator.py:466-578) walks the same blocks of users, but scores and ranks only each user's
 candidate list (test items + sampled negatives) with the csrc/score.cu candidate kernels before the same accumulate kernel.
-Not mirrored: `diversity_object` (DIVERSITY_SIMILARITY needs an item-similarity matrix, metrics.py:719-775).
+
+With a `diversity_object` (metrics.py:719-775: any object with an `item_diversity_matrix`, such as `Diversity_similarity`
+below or the reference's own class) both evaluators add DIVERSITY_SIMILARITY, the 23rd metric: the top-left
+n_items x n_items block of the matrix is uploaded once per evaluator and device, and `b200_eval_diversity_device` reduces
+each block's lists next to the accumulate kernel.
 """
 import ctypes
 
@@ -26,8 +30,24 @@ METRIC_NAMES = ["PRECISION", "PRECISION_RECALL_MIN_DEN", "RECALL", "MAP", "MAP_M
                 "COVERAGE_ITEM", "COVERAGE_ITEM_HIT", "ITEMS_IN_GT", "COVERAGE_USER", "COVERAGE_USER_HIT", "USERS_IN_GT",
                 "DIVERSITY_GINI", "SHANNON_ENTROPY"]
 _SLOT = dict(PRECISION=0, PRECISION_RECALL_MIN_DEN=1, RECALL=2, MAP=3, MAP_MIN_DEN=4, MRR=5, NDCG=6, HIT_RATE=7, ARHR_ALL_HITS=8,
-             NOVELTY=9, AVERAGE_POPULARITY=10, USERS_WITH_RECS=11, N_USERS=12)
+             NOVELTY=9, AVERAGE_POPULARITY=10, USERS_WITH_RECS=11, N_USERS=12, DIVERSITY_SIMILARITY=13, SHORT_LISTS=14)
 _NACC = 16
+# with a diversity object, the reference's EvaluatorMetrics order puts DIVERSITY_SIMILARITY after AVERAGE_POPULARITY
+_METRIC_NAMES_DIVERSITY = METRIC_NAMES[:METRIC_NAMES.index("AVERAGE_POPULARITY") + 1] + ["DIVERSITY_SIMILARITY"] + \
+    METRIC_NAMES[METRIC_NAMES.index("AVERAGE_POPULARITY") + 1:]
+
+
+class Diversity_similarity(object):
+    """metrics.py:719-731: holds the dense item-item diversity matrix D for the evaluators' `diversity_object` argument.
+    For a recommendation list r of length L >= 2 a user's value is
+    sum_{a <= L-2} sum_{b <= L-1, b != a} D[r_a, r_b] / (L (L - 1)) (the last row is skipped, its column is not); the
+    metric is the mean over the evaluated users.  A list shorter than 2 items makes the evaluation raise
+    ZeroDivisionError, as the reference's 0.0 / 0 does."""
+
+    def __init__(self, item_diversity_matrix):
+        assert np.all(item_diversity_matrix >= 0.0) and np.all(item_diversity_matrix <= 1.0), \
+            "item_diversity_matrix contains value greated than 1.0 or lower than 0.0"
+        self.item_diversity_matrix = item_diversity_matrix
 
 
 def get_result_string(results_run, n_decimals=7):
@@ -72,8 +92,6 @@ class EvaluatorHoldout(object):
     def __init__(self, URM_test_list, cutoff_list, min_ratings_per_user=1, exclude_seen=True, diversity_object=None,
                  ignore_items=None, ignore_users=None, verbose=True):
         self.verbose = verbose
-        if diversity_object is not None:
-            raise NotImplementedError("EvaluatorHoldout: diversity_object (DIVERSITY_SIMILARITY) is not on the CUDA path")
         if ignore_items is None:  # Evaluator.py:168-174
             self.ignore_items_flag = False
             self.ignore_items_ID = np.array([], dtype=np.int64)
@@ -95,6 +113,16 @@ class EvaluatorHoldout(object):
         self.URM_test.eliminate_zeros()
         self.URM_test.sort_indices()
         self.n_users, self.n_items = self.URM_test.shape
+        self._div = None  # the diversity matrix D on the host, then (_div_device) on the device
+        if diversity_object is not None:
+            D = np.asarray(diversity_object.item_diversity_matrix)
+            if D.ndim != 2 or D.shape[0] < self.n_items or D.shape[1] < self.n_items:
+                raise ValueError("{}: diversity_object.item_diversity_matrix must be a dense 2-D array of at least {} x {} "
+                                 "(n_items), got shape {}".format(self.EVALUATOR_NAME, self.n_items, self.n_items, D.shape))
+            # item ids index D, so only its top-left n_items x n_items block is read; float32 stays float32, any other
+            # dtype is read as float64
+            self._div = np.ascontiguousarray(D[:self.n_items, :self.n_items],
+                                             np.float32 if D.dtype == np.float32 else np.float64)
         pruned = _remove_item_interactions(URM_test_list, self.ignore_items_ID)  # :199
         mask = np.ediff1d(pruned.indptr) >= min_ratings_per_user  # :204-208
         if not np.all(mask):
@@ -110,10 +138,19 @@ class EvaluatorHoldout(object):
         self.users_to_evaluate = list(users)
         self._lib = _lib.load()
         self._dev = None
+        self._d_div = None
 
     def _print(self, string):
         if self.verbose:
             print("{}: {}".format(self.EVALUATOR_NAME, string))
+
+    def _div_device(self, dev):
+        """The diversity matrix on the device, uploaded once per evaluator and device (early stopping evaluates often)."""
+        import torch
+        if self._d_div is None or self._d_div.device != dev:
+            self._d_div = None  # free the copy on the old device before the new one is made
+            self._d_div = torch.from_numpy(self._div).to(dev)
+        return self._d_div
 
     # ------------------------------------------------------------------------------------------------------------
     def _device_state(self, URM_train):
@@ -135,16 +172,23 @@ class EvaluatorHoldout(object):
             acc=torch.zeros((len(self.cutoff_list), _NACC), dtype=torch.float64, device=dev),
             rec=torch.zeros((len(self.cutoff_list), self.n_items), dtype=torch.int32, device=dev),
             hit=torch.zeros((len(self.cutoff_list), self.n_items), dtype=torch.int32, device=dev))
+        if self._div is not None:
+            st["div"] = self._div_device(dev)
         return st
 
     def _accumulate(self, st, d_users, items, vals, cutoff):
         """Adds one block's [B, cutoff] top-N table to the device accumulators (csrc/eval.cu)."""
         import torch
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         _lib.check(self._lib.b200_eval_accumulate_device(
             d_users.data_ptr(), d_users.shape[0], items.data_ptr(), vals.data_ptr(), cutoff, st["ptr"].data_ptr(),
             st["idx"].data_ptr(), st["val"].data_ptr(), st["cut"].data_ptr(), len(self.cutoff_list), st["idcg"].data_ptr(),
             st["nov"].data_ptr(), st["pop"].data_ptr(), self.n_items, st["acc"].data_ptr(), st["rec"].data_ptr(),
-            st["hit"].data_ptr(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+            st["hit"].data_ptr(), stream))
+        if "div" in st:
+            _lib.check(self._lib.b200_eval_diversity_device(
+                items.data_ptr(), vals.data_ptr(), d_users.shape[0], cutoff, st["cut"].data_ptr(), len(self.cutoff_list),
+                st["div"].data_ptr(), int(st["div"].dtype == torch.float64), self.n_items, st["acc"].data_ptr(), stream))
 
     def _evaluate_blocks(self, recommender_object, users, block_size, st):
         """Hold-out evaluation scores whole blocks of users (:426-455)."""
@@ -174,10 +218,15 @@ class EvaluatorHoldout(object):
         gt_items[self.ignore_items_ID] = False
         gt_users = np.ediff1d(self.URM_test.indptr) > 0
         gt_users[self.ignore_users_ID] = False
+        names = METRIC_NAMES if self._div is None else _METRIC_NAMES_DIVERSITY
         for k, c in enumerate(self.cutoff_list):
             r = {}
             if n_eval > 0:
                 a = acc[k]
+                if self._div is not None:
+                    if a[_SLOT["SHORT_LISTS"]] > 0:  # metrics.py:741, 0.0 / (L * (L - 1)) for a list of L <= 1 items
+                        raise ZeroDivisionError("float division by zero")
+                    r["DIVERSITY_SIMILARITY"] = float(a[_SLOT["DIVERSITY_SIMILARITY"]] / n_eval)
                 for name in ("PRECISION", "PRECISION_RECALL_MIN_DEN", "RECALL", "MAP", "MAP_MIN_DEN", "MRR", "NDCG", "HIT_RATE",
                              "ARHR_ALL_HITS", "NOVELTY", "AVERAGE_POPULARITY"):
                     r[name] = float(a[_SLOT[name]] / n_eval)
@@ -200,9 +249,9 @@ class EvaluatorHoldout(object):
                 couples = n_eval ** 2 - n_eval  # :860-873 (its counter is NOT filtered by ignore_items)
                 co = np.sum(rec[k] ** 2) - n_eval * c
                 r["DIVERSITY_MEAN_INTER_LIST"] = float((couples - co / c) / couples) if couples > 0 else float("nan")
-                results_dict[c] = {name: r[name] for name in METRIC_NAMES}
+                results_dict[c] = {name: r[name] for name in names}
             else:
-                results_dict[c] = {name: 0.0 for name in METRIC_NAMES}
+                results_dict[c] = {name: 0.0 for name in names}
         if n_eval == 0:
             self._print("WARNING: No users had a sufficient number of relevant items")
         if self.ignore_items_flag:
