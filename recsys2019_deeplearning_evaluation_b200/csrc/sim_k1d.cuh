@@ -423,7 +423,7 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
 // and no count-2 / count-1 cell that can reach the floor sim(3, largest norm term) (bounded by the smallest norm term of
 // the columns with at least 2 / 1 users), the K best count >= 3 cells are the answer -- the same keys from the same counts
 // and norm terms, so the output is the same.  Every other column (fewer
-// than K candidates, count-2 / count-1 cells that matter, more than S_CAP candidates) is appended to a device
+// than K candidates, count-2 / count-1 cells that matter, more candidates than the handle's sel_cap) is appended to a device
 // redo list that the kernel above then computes in full.  A counter overflow in the upper pass (the nibble checksum over
 // the window increments) or a full list sets a flag on the device, and the select kernel then hands EVERY column to
 // the kernel above: exactness never depends on the pair path.  Whether a handle takes the path at all is decided at create
@@ -456,7 +456,7 @@ __host__ __device__ __forceinline__ int k1d_window_size(int n, int c) { return (
 // counter words of the upper pass: every window, rounded to whole 16-byte vectors
 __host__ __device__ __forceinline__ int k1d_upper_words(int n) { return (((n >> 1) + 7) / 8 + 3) / 4 * 4; }
 // own_n flag: the column's cells overflowed its stage; the cells past it went to the loose list, so its own list is
-// incomplete and the select kernel hands the column to the redo list (it has more than S_CAP candidates anyway)
+// incomplete and the select kernel hands the column to the redo list
 constexpr int OWN_SPILLED = (int)0x80000000u;
 
 struct K1DUpShared {
@@ -641,13 +641,13 @@ __global__ void k1d_pair_scatter_kernel(const KParams p) {
   }
 }
 
-constexpr int S_WARPS = 4;            // columns (warps) per CTA of the select kernel: shared memory allows 3 CTAs per SM
+constexpr int S_WARPS = 4;            // columns (warps) per CTA of the select kernel
+constexpr int S_CTAS = 6;             // CTAs per SM its registers are bounded for (shared memory allows that at C5)
 constexpr int S_CAP = 4 * D_THREADS;  // the longest candidate list the select kernel decides (the K1-D kernel's key buffer)
-constexpr int S_ILP = 16;             // candidates per lane in flight while the keys are built (C5: ~430 per column)
-struct SelWarp {
-  u64 key[S_CAP];
-  int hist[256];
-};
+constexpr int S_ILP = 12;             // candidates per lane in flight while the keys are built (C5: ~430 per column)
+// shared memory of one select warp: its radix histogram, then the keys of a list of up to sel_cap candidates (the handle's
+// bound, <= S_CAP: sized from the expected list lengths at create time, so that more warps fit on an SM)
+__host__ __device__ __forceinline__ int k1d_select_warp_bytes(int sel_cap) { return 256 * 4 + sel_cap * 8; }
 
 // One warp: the K-th largest key of buf[0..n), so that exactly the K largest keys are >= it (0 when n <= K: nothing is
 // cut).  Keys are distinct and non-zero.  d_select's MSB-first radix select with 8-bit digits on one warp and its own
@@ -703,9 +703,11 @@ __device__ u64 w_select(const u64* buf, int* hist, int n, int K) {
 // collected path, the K best, emit -- or the column goes to the redo list (all columns when the call has fallen back).
 // No block barriers: a column's three dependent loads (list bounds, list, norm terms) overlap with the other warps' work.
 template <int F>
-__global__ void __launch_bounds__(32 * S_WARPS) sim_k1d_select_kernel(const KParams p) {
+__global__ void __launch_bounds__(32 * S_WARPS, S_CTAS) sim_k1d_select_kernel(const KParams p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  SelWarp& sw = reinterpret_cast<SelWarp*>(smem_raw)[threadIdx.x >> 5];
+  unsigned char* mine = smem_raw + (size_t)(threadIdx.x >> 5) * k1d_select_warp_bytes(p.sel_cap);
+  int* hist = reinterpret_cast<int*>(mine);
+  u64* keys = reinterpret_cast<u64*>(mine + 256 * 4);
   const int lane = threadIdx.x & 31;
   const int item = blockIdx.x * S_WARPS + (threadIdx.x >> 5);
   if (item >= p.n_range) return;
@@ -718,17 +720,19 @@ __global__ void __launch_bounds__(32 * S_WARPS) sim_k1d_select_kernel(const KPar
   const int col = wi.x, lc = wi.y, K = p.K;
   const int so = p.own_off[col], no = p.own_n[col];  // no < 0: OWN_SPILLED
   const int sm = p.mir_off[col], n = no + (p.mir_off[col + 1] - sm);
-  bool ok = no >= 0 && n <= S_CAP;
+  bool ok = no >= 0 && n <= p.sel_cap;
   int n_have = 0;
   if (ok) {
     const float Ai = p.A[col];
+    const unsigned* own = p.own + so;
+    const unsigned* mir = p.mir + sm - no;  // candidate t >= no is mir[t]
     for (int t0 = 0; t0 < n; t0 += 32 * S_ILP) {
       unsigned cd[S_ILP];
       int2 bn[S_ILP];
 #pragma unroll
       for (int q = 0; q < S_ILP; ++q) {
         const int t = t0 + 32 * q + lane;
-        cd[q] = t < n ? (t < no ? p.own[so + t] : p.mir[sm + (t - no)]) : 0u;
+        cd[q] = t < n ? (t < no ? own : mir)[t] : 0u;  // one load per candidate
       }
 #pragma unroll
       for (int q = 0; q < S_ILP; ++q)
@@ -741,7 +745,7 @@ __global__ void __launch_bounds__(32 * S_WARPS) sim_k1d_select_kernel(const KPar
           if (sv > 0.f) key = (((u64)__float_as_uint(sv)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)bn[q].y);
         }
         const unsigned b = __ballot_sync(0xffffffffu, key != 0ull);
-        if (key) sw.key[n_have + __popc(b & ((1u << lane) - 1u))] = key;
+        if (key) keys[n_have + __popc(b & ((1u << lane) - 1u))] = key;
         n_have += __popc(b);
       }
     }
@@ -759,13 +763,13 @@ __global__ void __launch_bounds__(32 * S_WARPS) sim_k1d_select_kernel(const KPar
     return;
   }
   __syncwarp();
-  const u64 thr = w_select(sw.key, sw.hist, n_have, K);
+  const u64 thr = w_select(keys, hist, n_have, K);
   // emit while compacting: the kept keys of every 32 take the next output slots in lane order
   const size_t out_base = (size_t)lc * K;
   int kept = 0;
   for (int t0 = 0; t0 < n_have; t0 += 32) {
     const int t = t0 + lane;
-    const u64 k64 = t < n_have ? sw.key[t] : 0ull;
+    const u64 k64 = t < n_have ? keys[t] : 0ull;
     const bool keep = t < n_have && k64 >= thr;
     const unsigned b = __ballot_sync(0xffffffffu, keep);
     if (keep)

@@ -138,6 +138,7 @@ struct KParams {
   const int* __restrict__ mir_off;
   unsigned* mir;
   int* pair_fail;
+  int sel_cap;  // the longest list the select kernel decides (its per-warp key buffer)
   int4* wl_redo;
   int* n_redo;
   float lvl_b1, lvl_b2;  // smallest norm term of the columns with >= 1 / >= 2 users (the neighbours a count-1 / -2 cell can have)
@@ -1260,8 +1261,8 @@ struct b200_sim_s {
   float lvl_b1 = 0.f, lvl_b2 = 0.f;
   DevBuf<int> own_off, own_n, deg, mir_off, pair_ctl;
   DevBuf<unsigned char> scan_tmp;
-  size_t scan_tmp_bytes = 0, smem_up_bytes = 0;
-  int ctas_up = 0;
+  size_t scan_tmp_bytes = 0, smem_up_bytes = 0, smem_sel_bytes = 0;
+  int ctas_up = 0, sel_cap = 0;
   bool pair_path_last = false;  // the cached routing qualifies for the pair path
   DevBuf<int> counter, order;
   std::vector<int> h_order;  // cached LPT order for [order_lo, order_hi)
@@ -1328,7 +1329,10 @@ int bits_for(long long n) {
 // n_cols * P(Poisson(lambda_c) >= 3) cells with count >= 3 (lambda_c = gathered entries off the diagonal / n_cols), which
 // must reach K, and
 // no count-2 / count-1 cell may reach the floor sim(3, largest norm term).  Sets the smallest norm terms of the neighbours
-// a count-1 / count-2 cell can have, and the expected number of pairs (which sizes the pair list).
+// a count-1 / count-2 cell can have, the expected number of pairs (which sizes the pair list), and the longest list the
+// select kernel decides: the largest expected list plus six standard deviations (Poisson) and 32, in multiples of 8, at
+// most S_CAP.  A longer list is redone exactly; the bound only sizes the select kernel's shared memory, so that more of
+// its warps fit on an SM (C5: expected lists of 243 to 778, sel_cap 984, six CTAs per SM instead of three).
 template <int F>
 bool k1d_pair_gate_f(b200_sim_s* h, const KParams& p, const std::vector<int>& cnt, const std::vector<int2>& bn, const std::vector<float>& a) {
   const int n = h->n_cols;
@@ -1342,18 +1346,20 @@ bool k1d_pair_gate_f(b200_sim_s* h, const KParams& p, const std::vector<int>& cn
   h->lvl_b2 = b2;
   const float bmax = bval(n - 1);
   long long nonempty = 0, pass = 0;
-  double cells = 0.0;
+  double cells = 0.0, est_max = 0.0;
   for (int c = 0; c < n; ++c) {
     if (cnt[(size_t)c] == 0) continue;
     ++nonempty;
     const double lam = (double)(h->h_work[(size_t)bn[(size_t)c].y] - (unsigned long long)cnt[(size_t)c]) / (double)n;
     const double est = (double)n * std::max(0.0, 1.0 - std::exp(-lam) * (1.0 + lam + 0.5 * lam * lam));
     cells += est;
+    est_max = std::max(est_max, est);
     const float ai = a[(size_t)c];
     const float fl = sim_value<F>(p, 3.f, ai, bmax) * (1.f - 1e-6f);
     if (est >= (double)h->K && fl > 0.f && !(sim_value<F>(p, 2.f, ai, b2) >= fl) && !(sim_value<F>(p, 1.f, ai, b1) >= fl)) ++pass;
   }
   h->pairs_expected = 0.5 * cells;
+  h->sel_cap = (int)std::min<double>(std::ceil((est_max + 6.0 * std::sqrt(est_max) + 32.0) / 8.0) * 8.0, (double)S_CAP);
   return nonempty > 0 && (double)pass >= 0.9 * (double)nonempty;
 }
 
@@ -1718,7 +1724,9 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       if (h->ctas_up > 0) {
         B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_up_bytes));
         B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-        B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_WARPS * sizeof(SelWarp))));
+        // the launch passes this handle's size; the limit is the same for every handle that shares the kernel
+        h->smem_sel_bytes = (size_t)S_WARPS * k1d_select_warp_bytes(h->sel_cap);
+        B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributeMaxDynamicSharedMemorySize, S_WARPS * k1d_select_warp_bytes(S_CAP)));
         B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         h->worklist_up.alloc((size_t)n_cols);
         // the upper pass's longest-first order: every column by descending window work (empty columns do nothing there)
@@ -1945,6 +1953,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.pair_fail = h->pair_ctl.get() + 2; p.n_redo = h->pair_ctl.get() + 3;
   p.loose = h->loose.get(); p.n_loose = reinterpret_cast<u64*>(h->pair_ctl.get() + 4); p.loose_cap = h->loose_cap;
   p.deg = h->deg.get(); p.mir_off = h->mir_off.get(); p.mir = h->mir.get(); p.wl_redo = h->wl_redo.get();
+  p.sel_cap = h->sel_cap;
   p.lvl_b1 = h->lvl_b1; p.lvl_b2 = h->lvl_b2;
   B200_CUDA(cudaEventRecord(h->ev0, st));
   if (pair_path) {
@@ -1962,7 +1971,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     B200_CUDA(cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), tb, h->deg.get(), h->mir_off.get(), h->n_cols + 1, st));
     k1d_pair_scatter_kernel<<<div_up((long long)h->n_cols * 32, 256), 256, 0, st>>>(q);
     B200_CUDA(cudaGetLastError());
-    k1d_select_kernel_for(h->formula)<<<div_up(n_sparse, S_WARPS), 32 * S_WARPS, S_WARPS * sizeof(SelWarp), st>>>(q);
+    k1d_select_kernel_for(h->formula)<<<div_up(n_sparse, S_WARPS), 32 * S_WARPS, h->smem_sel_bytes, st>>>(q);
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
     q.worklist = h->wl_redo.get();
