@@ -28,9 +28,12 @@
 // sums, two vectors in flight) did not shorten the sweep: its shared loads queue behind the OTHER CTA's atomics.  What would: more CTAs per SM in different phases (two neighbour windows of
 // 50 KB counters each: 3-4 CTAs) or two accumulators per CTA with warp-specialised gather / select.
 //
-// Gather.  The CSC side stores, per entry, where the user's padded row lives (csc_seg: start and length in 16-byte
-// chunks), so a warp reads 32 of them with one coalesced load and then streams those rows with 128-bit loads, four rows in
-// flight per warp: 32 warps x 4 rows x ~400 B = 50 KB in flight per SM against a bandwidth-delay product of ~18 KB.
+// Gather.  Rows are packed seven entries to a 16-byte chunk (a 32-bit index and six 16-bit gaps: the layout is described
+// above K1DShared), so a gathered entry costs 2.3 bytes instead of 4.  The CSC side stores, per entry, where the user's
+// row lives (csc_seg: first chunk and chunk count), so a warp reads 32 of them with one coalesced load and then streams
+// those rows with 128-bit loads, a half warp per row (~15 chunks at C5) and four loads of two rows in flight per warp:
+// 32 warps x 8 rows x ~240 B = 60 KB in flight per SM.  With a whole warp per row more than half the lanes idle and the
+// kernel issues nearly twice the shared-atomic instructions per entry: it was 12 % slower than with four entries per chunk.
 //
 // Selection.  The neighbour axis is numbered by ascending norm term, and every formula served here increases with the
 // count and decreases with the neighbour's norm term.  One sweep finds the cells with count >= 3 (bit tricks on whole
@@ -45,8 +48,21 @@ constexpr int D_WARPS = D_THREADS / 32;
 constexpr int D_ROWS = 4;        // rows in flight per warp
 constexpr int D_TILE_LOG2 = 10;  // norm tile: 1024 neighbours = 128 counter words
 
+// The K1-D row layout.  Every user's sorted row, `copies` times back to back (copies = 2: the indices, then the same
+// indices + n_cols, so that the upper pass's cyclic window of an entry is one range of the row), as 16-byte chunks of up to
+// seven entries: int4 {base, g1 | g2 << 16, g3 | g4 << 16, g5 | g6 << 16}.  Entry 0 is `base`, an absolute index; entry e
+// is entry e - 1 plus the 16-bit gap g_e.  Rows are sorted and distinct and the second copy starts first + n_cols - last
+// >= 1 after the first ends, so a real gap is >= 1: gap 0 means "no entry", and every slot after it is empty too.  An
+// entry 65 536 or more after its predecessor starts a new chunk as its base (at C5 the mean gap is 2 000).  Every chunk's
+// base is a real entry and the bases of a row ascend, so the chunk that holds a given entry is found by value.
+constexpr int K1D_GAPS = 6;
+__device__ __forceinline__ int k1d_gap(const int4& c, int e) {  // g_(e + 1)
+  const int w = e < 2 ? c.y : (e < 4 ? c.z : c.w);
+  return (e & 1) ? (int)((unsigned)w >> 16) : (w & 0xffff);
+}
+
 struct K1DShared {
-  int item, nbuf, cnt, adds, nibsum, tstop, chunk_end, chunk_cnt;
+  int item, nbuf, cnt, nibsum, tstop, chunk_end, chunk_cnt;
   int need, digit, bincnt, ncand, expect;
   u64 kor, kand;
   int hist[256];
@@ -161,7 +177,7 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
 
   for (;;) {
     __syncthreads();
-    if (tid == 0) { ds.item = atomicAdd(p.counter, 1); ds.nbuf = 0; ds.adds = 0; ds.nibsum = 0; ds.ncand = 0; }
+    if (tid == 0) { ds.item = atomicAdd(p.counter, 1); ds.nbuf = 0; ds.nibsum = 0; ds.ncand = 0; }
     __syncthreads();
     const int item = ds.item;
     if (item >= n_items) break;
@@ -169,47 +185,49 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
     const int col = wi.x, lc = wi.y, cs = wi.z, ce = wi.w;
     const size_t out_base = (size_t)lc * K;
     const float Ai = p.A[col];
+    const int adds = __ldg(p.col_adds + col);  // increments the column's rows must produce: per row its entries - 1 (the diagonal, pyx:396)
 
     // ---------------- gather: one fire-and-forget shared atomic per gathered entry, nothing else per entry
-    int expect = 0;  // increments this warp's rows must produce: per row 4 * chunks - padding - 1 (the diagonal, pyx:396)
     for (int k0 = cs + warp * 32; k0 < ce; k0 += D_WARPS * 32) {
       const int nrows = min(32, ce - k0);
       int2 seg = make_int2(0, 0);
-      if (lane < nrows) {
-        seg = __ldg(p.csc_seg + k0 + lane);
-        expect += 4 * (seg.y >> 2) - (seg.y & 3) - 1;
-      }
-      for (int r0 = 0; r0 < nrows; r0 += D_ROWS) {
+      if (lane < nrows) seg = __ldg(p.csc_seg + k0 + lane);
+      // a half warp per row (a C5 row is ~15 chunks): D_ROWS loads of two rows each in flight, every lane's seven entries
+      // decoded by a running sum over the gaps
+      const int hl = lane & 15, hh = lane >> 4;
+      for (int r0 = 0; r0 < nrows; r0 += 2 * D_ROWS) {
         int4 v[D_ROWS];
         int rs[D_ROWS], rn[D_ROWS];
 #pragma unroll
         for (int q = 0; q < D_ROWS; ++q) {
-          const int r = r0 + q;
+          const int r = r0 + 2 * q + hh;
           rs[q] = __shfl_sync(0xffffffffu, seg.x, r & 31);
-          rn[q] = r < nrows ? (__shfl_sync(0xffffffffu, seg.y, r & 31) >> 2) : 0;
-          if (lane < rn[q]) v[q] = __ldg(reinterpret_cast<const int4*>(p.csr_idx1) + (size_t)rs[q] + lane);
+          rn[q] = __shfl_sync(0xffffffffu, seg.y, r & 31);
+          if (r >= nrows) rn[q] = 0;
+          if (hl < rn[q]) v[q] = __ldg(p.csr_idx1 + (size_t)rs[q] + hl);
         }
 #pragma unroll
         for (int q = 0; q < D_ROWS; ++q) {
           int c0 = 0;
           for (;;) {
-            if (c0 + lane < rn[q]) {
-              const int jj[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
+            if (c0 + hl < rn[q]) {
+              // the last chunk of the first copy can run on into the second one: j < n_cols masks those entries
+              int j = v[q].x;
+              if (j < p.n_cols && j != col) atomicAdd(&acc[j >> 3], 1u << ((j & 7) << 2));
 #pragma unroll
-              for (int c = 0; c < 4; ++c) {
-                const int j = jj[c];
-                if ((unsigned)j < (unsigned)p.n_cols && j != col) atomicAdd(&acc[j >> 3], 1u << ((j & 7) << 2));
+              for (int e = 0; e < K1D_GAPS; ++e) {
+                const int g = k1d_gap(v[q], e);
+                j += g;
+                if (g && j < p.n_cols && j != col) atomicAdd(&acc[j >> 3], 1u << ((j & 7) << 2));
               }
             }
-            c0 += 32;
-            if (c0 >= rn[q]) break;  // rows longer than 32 chunks (128 entries): next 512 bytes
-            if (c0 + lane < rn[q]) v[q] = __ldg(reinterpret_cast<const int4*>(p.csr_idx1) + (size_t)rs[q] + c0 + lane);
+            c0 += 16;
+            if (c0 >= rn[q]) break;  // rows longer than 16 chunks (up to 112 entries): next 256 bytes
+            if (c0 + hl < rn[q]) v[q] = __ldg(p.csr_idx1 + (size_t)rs[q] + c0 + hl);
           }
         }
       }
     }
-    expect = __reduce_add_sync(0xffffffffu, expect);
-    if (lane == 0 && expect) atomicAdd(&ds.adds, expect);
     __syncthreads();
     PROF_MARK(1);
 
@@ -254,7 +272,7 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
     }
     __syncthreads();
     const bool forced = p.fail_every > 0 && (lc % p.fail_every) == 0;  // test hook: exercises the redo path
-    if (ds.nibsum != ds.adds || forced) {
+    if (ds.nibsum != adds || forced) {
       // a counter overflowed: the window kernel redoes this column; leave clean state behind
       __syncthreads();
       if (tid == 0) p.redo[atomicAdd(p.fail, 1)] = lc;
@@ -460,7 +478,7 @@ __host__ __device__ __forceinline__ int k1d_upper_words(int n) { return (((n >> 
 constexpr int OWN_SPILLED = (int)0x80000000u;
 
 struct K1DUpShared {
-  int item, adds, nibsum, ncand, nst;
+  int item, nibsum, ncand, nst;
   unsigned long long base;
 };
 
@@ -481,33 +499,31 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
     if (tid == 0) {
       // once the call has fallen back, the remaining columns are not worth gathering
       us.item = *(volatile int*)p.pair_fail ? p.n_range : atomicAdd(p.counter, 1);
-      us.adds = 0; us.nibsum = 0; us.ncand = 0; us.nst = 0;
+      us.nibsum = 0; us.ncand = 0; us.nst = 0;
     }
     __syncthreads();
     const int item = us.item;
     if (item >= p.n_range) break;
     const int4 wi = __ldg(p.worklist_up + item);
-    const int col = wi.x, cs = wi.z, ce = wi.w;
+    const int col = wi.x, adds = wi.y, cs = wi.z, ce = wi.w;  // adds: the increments of the column's windows
     const int size_c = k1d_window_size(n, col);
 
     // ---------------- gather over the row windows: cell t = j' - col - 1 of doubled-row index j', counted iff t < size_c,
-    // which masks the entries of the first and last chunk outside the window and the padding (INT_MAX).  A window is half a
-    // row on average (C5: ~13 chunks), so one row per warp load would leave most lanes idle and issue as many
+    // which masks the entries of the first and last chunk outside the window; a gap of 0 is padding.  A window is half a
+    // row on average (C5: ~8 chunks), so one row per warp load would leave most lanes idle and issue as many
     // loads and atomic instructions as the whole row; instead the 32 windows of a batch are one stream of chunks, every
     // lane of every load busy.  Rows with chunks sit compacted in the low lanes; lane r holds row r's [beg, end) in the
     // stream, and the row of stream position f is the number of rows that end at or before f.
-    int expect = 0;
     for (int k0 = cs + warp * 32; k0 < ce; k0 += U_WARPS * 32) {
       const int nrows = min(32, ce - k0);
       int2 seg = make_int2(0, 0);
       if (lane < nrows) seg = __ldg(p.csc_win + k0 + lane);
-      expect += 4 * (seg.y >> 3) - (seg.y & 7);
-      const unsigned nz = __ballot_sync(0xffffffffu, (seg.y >> 3) > 0);
+      const unsigned nz = __ballot_sync(0xffffffffu, seg.y > 0);
       const int nr = __popc(nz);
       const int src = lane < nr ? (int)__fns(nz, 0, lane + 1) : 0;
       const int rstart = __shfl_sync(0xffffffffu, seg.x, src);
       const int sy = __shfl_sync(0xffffffffu, seg.y, src);
-      const int rn = lane < nr ? (sy >> 3) : 0;
+      const int rn = lane < nr ? sy : 0;
       int end = rn;
 #pragma unroll
       for (int off = 1; off < 32; off <<= 1) {
@@ -525,23 +541,23 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
           const unsigned ends = __reduce_or_sync(0xffffffffu, (lane < nr && end > base && end - base < 32) ? (1u << (end - base)) : 0u);
           const int row = (__popc(before) + __popc(ends & ((2u << lane) - 1u))) & 31;
           const int rb = __shfl_sync(0xffffffffu, beg, row), rs = __shfl_sync(0xffffffffu, rstart, row);
-          if (f < total) v[q] = __ldg(reinterpret_cast<const int4*>(p.csr_idx1) + (size_t)rs + (f - rb));
+          if (f < total) v[q] = __ldg(p.csr_idx1 + (size_t)rs + (f - rb));
         }
 #pragma unroll
         for (int q = 0; q < U_STEPS; ++q) {
           if (b0 + 32 * q + lane < total) {
-            const int jj[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
+            unsigned t = (unsigned)(v[q].x - col - 1);
+            if (t < (unsigned)size_c) atomicAdd(&acc[t >> 3], 1u << ((t & 7) << 2));
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const unsigned t = (unsigned)(jj[c] - col - 1);
-              if (t < (unsigned)size_c) atomicAdd(&acc[t >> 3], 1u << ((t & 7) << 2));
+            for (int e = 0; e < K1D_GAPS; ++e) {
+              const unsigned g = (unsigned)k1d_gap(v[q], e);
+              t += g;
+              if (g && t < (unsigned)size_c) atomicAdd(&acc[t >> 3], 1u << ((t & 7) << 2));
             }
           }
         }
       }
     }
-    expect = __reduce_add_sync(0xffffffffu, expect);
-    if (lane == 0 && expect) atomicAdd(&us.adds, expect);
     __syncthreads();
     PROF_MARK(8);
 
@@ -598,7 +614,7 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
     __syncthreads();
     const int nst = us.nst;
     if (tid == 0) {
-      if (us.nibsum != us.adds) atomicExch(p.pair_fail, 1);  // a counter overflowed: the call falls back
+      if (us.nibsum != adds) atomicExch(p.pair_fail, 1);  // a counter overflowed: the call falls back
       us.base = nst ? atomicAdd(p.n_own, (unsigned long long)nst) : 0ull;
       if (us.base + nst > (unsigned long long)p.pair_cap) atomicExch(p.pair_fail, 1);
       p.own_off[col] = (int)us.base;  // < pair_cap < 2^30 unless the call has fallen back
@@ -789,64 +805,113 @@ __global__ void k1d_tile_bounds_kernel(const int2* __restrict__ BN, int n_cols, 
   tb[t] = __int_as_float(BN[min(t << D_TILE_LOG2, n_cols - 1)].x);
 }
 
-// The K1-D row layout: every user's sorted row `copies` times back to back (copies = 2: the indices, then the same indices
-// + n_cols, so that the upper pass's cyclic window of an entry is one range of positions), padded to 16-byte chunks with
-// INT_MAX, which no window or neighbour test accepts.  len4[u] = the padded length; idx1 from its exclusive scan poff.
-__global__ void k1d_row_len_kernel(const int* __restrict__ csr_ptr, int n_rows, int copies, int* len4) {
+// entry m of a row written `copies` times (k1d layout above): row[m], then row[m - len] + n_cols
+__device__ __forceinline__ int k1d_row_entry(const int* __restrict__ row, int len, int n_cols, int m) {
+  return m < len ? row[m] : row[m - len] + n_cols;
+}
+
+// Walks one row in layout order and hands every chunk to emit(chunk number, chunk); returns the number of chunks.
+template <class Emit>
+__device__ __forceinline__ int k1d_row_chunks(const int* __restrict__ row, int len, int copies, int n_cols, Emit emit) {
+  const int total = copies * len;
+  int nch = 0;
+  for (int m = 0; m < total; ++nch) {
+    const int base = k1d_row_entry(row, len, n_cols, m++);
+    unsigned long long g14 = 0ull;  // gaps 1..4, then 5..6
+    unsigned g56 = 0u;
+    for (int e = 0, prev = base; e < K1D_GAPS && m < total; ++e, ++m) {
+      const int j = k1d_row_entry(row, len, n_cols, m);
+      if (j - prev >= 65536) break;
+      if (e < 4) g14 |= (unsigned long long)(j - prev) << (16 * e); else g56 |= (unsigned)(j - prev) << (16 * (e - 4));
+      prev = j;
+    }
+    emit(nch, make_int4(base, (int)(unsigned)g14, (int)(unsigned)(g14 >> 32), (int)g56));
+  }
+  return nch;
+}
+
+// nchunk[u] = chunks of row u (one thread per row); rows from its exclusive scan poff.  In the fill, eight lanes per row
+// walk it together (their loads are one broadcast) and lane l stores chunks l, l + 8, ...
+__global__ void k1d_row_len_kernel(const int* __restrict__ csr_ptr, const int* __restrict__ csr_idx, int n_rows, int copies, int n_cols,
+                                   int* nchunk) {
   const int u = blockIdx.x * blockDim.x + threadIdx.x;
-  if (u < n_rows) len4[u] = (copies * (csr_ptr[u + 1] - csr_ptr[u]) + 3) & ~3;
+  if (u >= n_rows) return;
+  nchunk[u] = k1d_row_chunks(csr_idx + csr_ptr[u], csr_ptr[u + 1] - csr_ptr[u], copies, n_cols, [](int, int4) {});
 }
 
 __global__ void k1d_row_fill_kernel(const int* __restrict__ csr_ptr, const int* __restrict__ csr_idx, const int* __restrict__ poff,
-                                    int n_rows, int copies, int n_cols, int* idx1) {
-  const int u = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 3);  // 8 lanes per row
+                                    int n_rows, int copies, int n_cols, int4* rows) {
+  const int u = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 3), l = threadIdx.x & 7;
   if (u >= n_rows) return;
-  const int r0 = csr_ptr[u], len = csr_ptr[u + 1] - r0, s = poff[u], n4 = poff[u + 1] - s;
-  for (int t = (threadIdx.x & 7); t < n4; t += 8)
-    idx1[s + t] = t < len ? csr_idx[r0 + t] : (t < copies * len ? csr_idx[r0 + t - len] + n_cols : INT_MAX);
+  int4* out = rows + poff[u];
+  k1d_row_chunks(csr_idx + csr_ptr[u], csr_ptr[u + 1] - csr_ptr[u], copies, n_cols, [=](int ch, int4 c) { if ((ch & 7) == l) out[ch] = c; });
+}
+
+// the chunk of a row (nch chunks) that holds entry m, whose value is v: the last one whose base is <= v.  The chunks before
+// it hold at most seven entries each, so it is chunk m / 7 or a later one, and m / 7 itself unless a gap before entry m
+// closed a chunk early: one look at the next base settles the usual case.
+__device__ __forceinline__ int k1d_chunk_of(const int4* __restrict__ row, int nch, int m, int v) {
+  int lo = m / (K1D_GAPS + 1), hi = nch;
+  if (lo + 1 == nch || row[lo + 1].x > v) return lo;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (row[mid].x <= v) lo = mid; else hi = mid;
+  }
+  return lo;
 }
 
 // Per CSC entry q (user u, column c; csc_pos[q] = its position in the CSR, so its place in u's row is k = csc_pos[q] - r0):
-// csc_seg[q] = u's whole row for the K1-D kernel: x = start in 16-byte chunks, y = chunks << 2 | entries of the last chunk
-// past the row (0..3; second-copy entries or padding).  With a doubled layout (win != nullptr) also win[q] = the entry's
-// window for the upper pass, positions k + 1 .. (last one <= c + size_c) of the doubled row: x = start in 16-byte chunks,
-// y = chunks << 3 | entries of those chunks that produce no increment (0..6), and win_work[c] = the increments of all of
-// column c's windows (sort key of the upper pass's longest-first order, with iota[c] = c as the value).  One warp per column.
+// csc_seg[q] = the chunks that hold the first copy of u's row, for the K1-D kernel: x = first chunk, y = chunks; and
+// col_adds[c] = the increments column c's rows produce there (entries - 1 per row).  With a doubled layout (win != nullptr)
+// also win[q] = the chunks that hold the entry's window for the upper pass, entries k + 1 .. (last one <= c + size_c) of
+// the doubled row, and win_work[c] = the increments of all of column c's windows (the upper pass's checksum target and
+// the sort key of its longest-first order, with iota[c] = c as the value).  Increments are counted in the CSR, never from
+// chunk counts.  One warp per column.
 __global__ void k1d_csc_rows_kernel(const int* __restrict__ csc_ptr, const int* __restrict__ csc_idx, const int* __restrict__ csr_ptr,
-                                    const int* __restrict__ csc_pos, const int* __restrict__ poff, const int* __restrict__ idx1,
-                                    int n_cols, int2* seg, int2* win, unsigned long long* win_work, int* iota) {
+                                    const int* __restrict__ csr_idx, const int* __restrict__ csc_pos, const int* __restrict__ poff,
+                                    const int4* __restrict__ rows, int n_cols, int2* seg, int* col_adds, int2* win,
+                                    unsigned long long* win_work, int* iota) {
   const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (c >= n_cols) return;
   const int bound = c + k1d_window_size(n_cols, c);
   unsigned long long w = 0;
+  int full = 0;
   for (int q = csc_ptr[c] + lane; q < csc_ptr[c + 1]; q += 32) {
     const int u = csc_idx[q];
-    const int r0 = csr_ptr[u], len = csr_ptr[u + 1] - r0, s = poff[u];
-    const int nch = (len + 3) >> 2;
-    seg[q] = make_int2(s >> 2, (nch << 2) | (4 * nch - len));
+    const int r0 = csr_ptr[u], len = csr_ptr[u + 1] - r0, s = poff[u], nch = poff[u + 1] - s;
+    const int* row = csr_idx + r0;
+    seg[q] = make_int2(s, k1d_chunk_of(rows + s, nch, len - 1, row[len - 1]) + 1);
+    full += len - 1;
     if (!win) continue;
-    // the window ends before the first position in (k, k + len) whose index exceeds c + size_c (position k + len holds c + n)
+    // the window ends before the first entry in (k, k + len) whose index exceeds c + size_c (entry k + len is c + n)
     const int k = csc_pos[q] - r0;
     int lo = k + 1, hi = k + len;
     while (lo < hi) {
       const int mid = (lo + hi) >> 1;
-      if (idx1[s + mid] <= bound) lo = mid + 1; else hi = mid;
+      if (k1d_row_entry(row, len, n_cols, mid) <= bound) lo = mid + 1; else hi = mid;
     }
-    const int wch = ((lo + 3) >> 2) - ((k + 1) >> 2);
-    win[q] = lo > k + 1 ? make_int2((s >> 2) + ((k + 1) >> 2), (wch << 3) | (4 * wch - (lo - k - 1))) : make_int2(0, 0);
+    int2 d = make_int2(0, 0);
+    if (lo > k + 1) {
+      const int first = k1d_chunk_of(rows + s, nch, k + 1, k1d_row_entry(row, len, n_cols, k + 1));
+      d = make_int2(s + first, k1d_chunk_of(rows + s, nch, lo - 1, k1d_row_entry(row, len, n_cols, lo - 1)) - first + 1);
+    }
+    win[q] = d;
     w += (unsigned long long)(lo - k - 1);
   }
+  full = __reduce_add_sync(0xffffffffu, full);
+  if (lane == 0) col_adds[c] = full;
   if (!win) return;
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) w += __shfl_xor_sync(0xffffffffu, w, off);
   if (lane == 0) { win_work[c] = w; iota[c] = c; }
 }
 
-// the upper pass's work list: every column (new numbering, in the order `perm`) as (new column, original column, csc range)
-__global__ void k1d_upper_worklist_kernel(const int* __restrict__ perm, const int2* __restrict__ BN, const int* __restrict__ csc_ptr,
-                                          int n_cols, int4* wl) {
+// the upper pass's work list: every column (new numbering, in the order `perm`, work[k] = its window increments) as
+// (new column, increments, csc range).  The increments are compared with a 32-bit nibble sum: their low 32 bits do.
+__global__ void k1d_upper_worklist_kernel(const int* __restrict__ perm, const unsigned long long* __restrict__ work,
+                                          const int* __restrict__ csc_ptr, int n_cols, int4* wl) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n_cols) return;
   const int c = perm[k];
-  wl[k] = make_int4(c, BN[c].y, csc_ptr[c], csc_ptr[c + 1]);
+  wl[k] = make_int4(c, (int)(unsigned)work[k], csc_ptr[c], csc_ptr[c + 1]);
 }

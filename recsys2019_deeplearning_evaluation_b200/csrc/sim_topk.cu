@@ -107,13 +107,15 @@ struct KParams {
   int eu_mode, eu_norm, eu_signed;
   float eu_div, eu_shrink;
   float* dense_out;  // dense mode (TopK == 0 / full Gram): [n_range, n_cols] row-major, out[target - col_begin, neighbour]
-  // K1-D (sim_k1d.cuh): 4-bit counter words, key-buffer slots, norm tiles and their bounds, the padded (doubled when the
-  // pair path can use it) row layout with the CSC-side (row start, row chunks) list, the work items of the launch (new column, local column, csc
-  // begin, csc end), the list + counter that receive the columns to redo, and a test hook (every n-th column is handed back)
+  // K1-D (sim_k1d.cuh): 4-bit counter words, key-buffer slots, norm tiles and their bounds, the packed (doubled when the
+  // pair path can use it) row layout with the CSC-side (first chunk, chunks) list and the increments every column's rows
+  // produce, the work items of the launch (new column, local column, csc begin, csc end), the list + counter that receive
+  // the columns to redo, and a test hook (every n-th column is handed back)
   int bm_words, cap_d, fail_every, ntile;
   const float* __restrict__ tbnd;
-  const int* __restrict__ csr_idx1;
+  const int4* __restrict__ csr_idx1;
   const int2* __restrict__ csc_seg;
+  const int* __restrict__ col_adds;
   const int4* __restrict__ worklist;
   int* redo;
   int* fail;
@@ -1237,7 +1239,8 @@ struct b200_sim_s {
   // K1-D (binary path, large sparse catalogues): second row layout with one window, CSC-side row locations, norm tile
   // bounds, ring / table geometry, routing threshold (expected hits per neighbour of a column) and last-launch statistics
   bool want_k1c = true, k1c = false;
-  DevBuf<int> csr_idx1, fail;
+  DevBuf<int4> csr_idx1;
+  DevBuf<int> col_adds, fail;
   DevBuf<int2> csc_seg;
   DevBuf<float> tbnd;
   DevBuf<int4> worklist;
@@ -1620,12 +1623,15 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     const bool f_ok_c = h->formula == F_PROD || h->formula == F_NONORM || h->formula == F_JACCARD || h->formula == F_DICE ||
                         (h->formula == F_TVERSKY && h->ta >= 0.f && h->tb >= 0.f);  // decreasing in the neighbour's norm term
     if (h->want_k1c && f_ok_c && nnz > 0 && n_cols >= h->k1c_min_cols) {
-      // K1-D layout (k1d_row_fill_kernel): every row twice, back to back, for the pair path's windows -- once when the doubled
-      // layout would not fit 32-bit positions: the K1-D kernel reads only the first copy, and the handle does not take the pair path
+      // K1-D layout (sim_k1d.cuh): every row twice, back to back, for the pair path's windows -- once when the doubled
+      // layout might not fit 32-bit chunk positions: the K1-D kernel reads only the first copy, and the handle does not take
+      // the pair path.  A row never has more chunks than entries, so the bound on the entries that the four-per-chunk layout
+      // needed still covers every matrix, whatever its gaps
       const int copies = 2 * (long long)nnz + 3ll * n_rows < (1ll << 31) ? 2 : 1;
       DevBuf<int> len1((size_t)n_rows + 1), poff1((size_t)n_rows + 1);
       B200_CUDA(cudaMemsetAsync(len1.get() + n_rows, 0, sizeof(int), st));
-      k1d_row_len_kernel<<<div_up(n_rows, 256), 256, 0, st>>>(h->csr_ptr.get(), n_rows, copies, len1.get()); count_launch();
+      k1d_row_len_kernel<<<div_up(n_rows, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), n_rows, copies, n_cols, len1.get());
+      count_launch();
       size_t tb1 = 0;
       B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb1, len1.get(), poff1.get(), n_rows + 1, st));
       DevBuf<unsigned char> tmp1(tb1 + 16);
@@ -1633,9 +1639,10 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       int total1 = 0;
       B200_CUDA(cudaMemcpyAsync(&total1, poff1.get() + n_rows, sizeof(int), cudaMemcpyDeviceToHost, st));
       B200_CUDA(cudaStreamSynchronize(st));
-      h->csr_idx1.alloc((size_t)total1 + 8);
+      h->csr_idx1.alloc((size_t)total1 + 2);
       k1d_row_fill_kernel<<<div_up((long long)n_rows * 8, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), poff1.get(), n_rows,
                                                                              copies, n_cols, h->csr_idx1.get()); count_launch();
+      h->col_adds.alloc((size_t)n_cols);
       h->csc_seg.alloc((size_t)nnz + 2);
       B200_CUDA(cudaMemsetAsync(h->csc_seg.get() + nnz, 0, 2 * sizeof(int2), st));
       if (copies == 2) {
@@ -1644,8 +1651,9 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
         win_iota.alloc((size_t)n_cols);
       }
       k1d_csc_rows_kernel<<<div_up((long long)n_cols * 32, 256), 256, 0, st>>>(h->csc_ptr.get(), h->csc_idx.get(), h->csr_ptr.get(),
-                                                                               csc_pos.get(), poff1.get(), h->csr_idx1.get(), n_cols,
-                                                                               h->csc_seg.get(), h->csc_win.get(), win_work.get(),
+                                                                               h->csr_idx.get(), csc_pos.get(), poff1.get(),
+                                                                               h->csr_idx1.get(), n_cols, h->csc_seg.get(),
+                                                                               h->col_adds.get(), h->csc_win.get(), win_work.get(),
                                                                                win_iota.get()); count_launch();
       B200_CUDA(cudaStreamSynchronize(st));
     }
@@ -1736,13 +1744,13 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
         B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
         DevBuf<unsigned char> tmp(tb + 16);
         B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
-        k1d_upper_worklist_kernel<<<div_up(n_cols, 256), 256, 0, st>>>(perm.get(), h->BN.get(), h->csc_ptr.get(), n_cols, h->worklist_up.get());
+        k1d_upper_worklist_kernel<<<div_up(n_cols, 256), 256, 0, st>>>(perm.get(), keys_out.get(), h->csc_ptr.get(), n_cols, h->worklist_up.get());
         count_launch(5);
         B200_CUDA(cudaStreamSynchronize(st));
       }
     }
   }
-  if (!h->k1c) { h->csr_idx1.release(); h->csc_seg.release(); }
+  if (!h->k1c) { h->csr_idx1.release(); h->csc_seg.release(); h->col_adds.release(); }
   if (h->ctas_up == 0) h->csc_win.release();
 }
 
@@ -1926,7 +1934,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.dense_out = d_dense;
   p.prof = h->prof_on ? h->prof.get() : nullptr;
   p.bm_words = h->bm_words; p.cap_d = h->cap_d; p.fail_every = h->fail_every; p.ntile = h->ntile; p.tbnd = h->tbnd.get();
-  p.csr_idx1 = h->csr_idx1.get(); p.csc_seg = h->csc_seg.get(); p.worklist = h->worklist.get();
+  p.csr_idx1 = h->csr_idx1.get(); p.csc_seg = h->csc_seg.get(); p.col_adds = h->col_adds.get(); p.worklist = h->worklist.get();
   p.redo = h->order.get(); p.fail = h->fail.get();
   p.n_range_dev = nullptr;
   p.csc_win = h->csc_win.get(); p.worklist_up = h->worklist_up.get();

@@ -14,7 +14,10 @@ if sys.argv[1] == "--child":
     from recsys2019_deeplearning_evaluation_b200 import _lib
     z = np.load(sys.argv[2])
     X = sps.csr_matrix((z["data"], z["indices"], z["indptr"]), shape=tuple(z["shape"]))
+    t0 = time.time()
     sim = Compute_Similarity_Cython(X, topK=200, shrink=100, similarity="cosine")
+    torch.cuda.synchronize()
+    create_s = time.time() - t0  # uploads, relabelling, row layouts: the first create of a process also loads the library
     n = X.shape[1]
     ms = []
     for r in range(4):
@@ -22,6 +25,17 @@ if sys.argv[1] == "--child":
         torch.cuda.synchronize()
         ms.append(sim.last_kernel_ms())
     chk = int(tab.cnt.sum().item()), float(tab.val.double().sum().item())
+    # the range as two half-range calls: the K1-D kernel alone on every column (a sub-range never takes the pair path)
+    halves = []
+    for r in range(3):
+        t = 0.0
+        for lo, hi in ((0, n // 2), (n // 2, n)):
+            sim.compute_topk_device(lo, hi)
+            torch.cuda.synchronize()
+            t += sim.last_kernel_ms()
+        halves.append(t)
+    print("%-10s create %.3f s  two half-range calls, kernel ms %s" % (sys.argv[3], create_s, " ".join("%.2f" % m for m in halves)),
+          flush=True)
     L = _lib.load()
     _lib.check(L.b200_sim_debug_phase_cycles(sim._h, 1, None))
     sim.compute_topk_device(0, n); torch.cuda.synchronize()
