@@ -393,13 +393,13 @@ int b200_lu_inverse_device(double* d_A, int n_pad, double* d_work, void* stream)
  * M, N multiples of 128, K a multiple of 16. */
 int b200_debug_dgemm_device(int kind, int M, int N, int K, double alpha, const double* d_A, int lda, const double* d_B, int ldb,
                             double beta, double* d_C, int ldc, void* stream);
-/* TEST HOOK: one GEMM of the blocked inverse through tensor-core GEMM version 1 (the default, gemm_tc.cuh) or 2
- * (gemm_tc2.cuh: pre-packed hi/lo TF32 operands fed by cp.async.bulk, opt-in via B200REC_GEMM=2).
+/* TEST HOOK: one GEMM of the blocked inverse through the 3xTF32 tensor-core GEMM (gemm_tc2.cuh: pre-packed hi/lo TF32
+ * operands fed by cp.async.bulk).
  * kind 0: C = alpha A B^T + beta C (A [M,K], B [N,K]); kind 1: C = alpha A B + beta C (B [K,N]);
  * kind 2: C = alpha A^T B + beta C with k >= max(row block, column block) only (A [K,M], B [K,N]; the L^T L product).
  * Row-major device pointers; M, N multiples of 128, K a multiple of 32. */
-int b200_debug_gemm_device(int version, int kind, int M, int N, int K, float alpha, const float* d_A, int lda,
-                           const float* d_B, int ldb, float beta, float* d_C, int ldc, void* stream);
+int b200_debug_gemm_device(int kind, int M, int N, int K, float alpha, const float* d_A, int lda, const float* d_B, int ldb,
+                           float beta, float* d_C, int ldc, void* stream);
 /* d_G: dense [n_items, n_items] Gram block X^T X (b200_sim_compute_dense_device with normalize=0, shrink=0); the
  * diagonal is replaced by item popularity (stored-entry count per column of the URM, :62-63) + l2_norm, the matrix is
  * inverted, and B[i, j] = P[i, j] / (-P[j, j]), B[j, j] = 0 is written to h_B (host) and/or d_B (device).

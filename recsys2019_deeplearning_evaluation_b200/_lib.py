@@ -106,7 +106,7 @@ SIGNATURES = {
     "b200_cand_topn_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, c_void, c_void, ctypes.c_int, c_void,
                                              c_void, c_void]),
     "b200_spd_inverse_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void]),
-    "b200_debug_gemm_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_void,
+    "b200_debug_gemm_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_void,
                                               ctypes.c_int, c_void, ctypes.c_int, ctypes.c_float, c_void, ctypes.c_int, c_void]),
     "b200_lu_inverse_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void]),
     "b200_debug_dgemm_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, c_void,

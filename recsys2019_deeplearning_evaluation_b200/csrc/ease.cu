@@ -10,16 +10,14 @@
 //      panel L21 = A21 inv(L11)^T and trailing update A22 -= L21 L21^T as GEMMs;
 //   2. inverse of the factor block column by block column, one batched GEMM pair per block diagonal;
 //   3. P = Linv^T Linv with the K range of every tile clipped to the non-zero (lower-triangular) part.
-// All three are O(n^3) GEMM work and run on the tensor cores: gemm_tc2.cuh / gemm_tc.cuh (wgmma .tf32 with a 3xTF32 operand
-// split for fp32-level accuracy, accumulators in registers).  Only the 128 x 128 diagonal-block factorisations stay on the
+// All three are O(n^3) GEMM work and run on the tensor cores: gemm_tc2.cuh (wgmma .tf32 with a 3xTF32 operand split for
+// fp32-level accuracy, accumulators in registers).  Only the 128 x 128 diagonal-block factorisations stay on the
 // CUDA cores (one CTA each, O(n * NB^2) work in total).
 // The popularity diagonal is a count, below sum r^2 on explicit ratings, so there G can be indefinite.  When the Cholesky
 // meets a non-positive pivot, G is inverted again in fp64 by the pivoted LU of lu_inverse.cu (what np.linalg.inv does);
 // an fp32 LU of these systems (cond up to ~1e7) would be far from the reference.
 #include <algorithm>
 #include <vector>
-
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "gemm_tc.cuh"
@@ -116,22 +114,15 @@ __global__ void copy_block_kernel(const float* __restrict__ src, int lds, float*
   dst[(long long)r * ldd + c] = src[(long long)r * lds + c];
 }
 
-// 2 = gemm_tc2.cuh (default: packed operands + cp.async.bulk producer), 1 = gemm_tc.cuh (the first kernel, kept selectable
-// with B200REC_GEMM=1 for A/B timing)
-int g_gemm_version = -1;
-int gemm_version() {
-  if (g_gemm_version < 0) {
-    const char* e = getenv("B200REC_GEMM");
-    g_gemm_version = (e && atoi(e) == 1) ? 1 : 2;
-  }
-  return g_gemm_version;
-}
+DevBuf<float> g_pack_a, g_pack_b;  // packed-operand workspaces of gemm, grown on demand
 
-DevBuf<float> g_pack_a, g_pack_b;  // packed-operand workspaces of the v2 path, grown on demand
-
+// C = alpha op(A) op(B) + beta C through gemm_tc2.cuh: pack op(A) and op(B) into the workspaces, then the GEMM kernel.
+// TA: op(A)(m, k) = A[k * lda + m]; TB: op(B)(k, n) = B[n * ldb + k].  TRI: op(A) = L^T, op(B) = L with L lower
+// triangular, so only k >= max(m0, n0) contributes.  M, N multiples of 128, K a multiple of 32.
 template <bool TA, bool TB, bool TRI>
-void gemm_v2(cudaStream_t st, int M, int N, int K, float alpha, const float* A, int lda, long long sA, const float* B, int ldb,
-             long long sB, float beta, float* C, int ldc, long long sC, int batch) {
+void gemm(cudaStream_t st, int M, int N, int K, float alpha, const float* A, int lda, long long sA, const float* B, int ldb,
+          long long sB, float beta, float* C, int ldc, long long sC, int batch) {
+  if (M <= 0 || N <= 0 || batch <= 0) return;
   const int KC = K / tc::BK, RA = M / tc::BM, RB = N / tc::BN;
   const long long strideAp = (long long)RA * KC * tc2::PAIR_FLOATS, strideBp = (long long)RB * KC * tc2::PAIR_FLOATS;
   // op(A) and op(B) are the same memory pattern of the same matrix (L21 L21^T, Linv^T Linv): pack once
@@ -155,24 +146,6 @@ void gemm_v2(cudaStream_t st, int M, int N, int K, float alpha, const float* A, 
   }
   tc2::tc2_gemm_kernel<<<dim3(RB, RA, batch), tc2::GEMM_THREADS, tc2::SMEM_BYTES, st>>>(
       K, TRI ? 1 : 0, alpha, g_pack_a.get(), strideAp, share ? g_pack_a.get() : g_pack_b.get(), share ? strideAp : strideBp, beta, C, ldc, sC);
-  count_launch();
-}
-
-template <bool TA, bool TB, bool TRI>
-void gemm(cudaStream_t st, int M, int N, int K, float alpha, const float* A, int lda, long long sA, const float* B, int ldb,
-          long long sB, float beta, float* C, int ldc, long long sC, int batch) {
-  if (M <= 0 || N <= 0 || batch <= 0) return;
-  if (gemm_version() == 2) {
-    gemm_v2<TA, TB, TRI>(st, M, N, K, alpha, A, lda, sA, B, ldb, sB, beta, C, ldc, sC, batch);
-    return;
-  }
-  static bool configured = false;
-  if (!configured) {
-    B200_CUDA(cudaFuncSetAttribute(tc::tc_gemm_kernel<TA, TB, TRI>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
-    configured = true;
-  }
-  tc::tc_gemm_kernel<TA, TB, TRI><<<dim3(N / tc::BN, M / tc::BM, batch), tc::THREADS, tc::SMEM_BYTES, st>>>(
-      M, N, K, alpha, A, lda, sA, B, ldb, sB, beta, C, ldc, sC);
   count_launch();
 }
 
@@ -251,32 +224,23 @@ int b200_spd_inverse_device(float* d_A, int n_pad, float* d_work, void* stream) 
   });
 }
 
-// TEST HOOK: one GEMM of the blocked inverse through version 1 (gemm_tc.cuh) or 2 (gemm_tc2.cuh):
+// TEST HOOK: one GEMM of the blocked inverse (gemm_tc2.cuh):
 //   kind 0: C = alpha A B^T + beta C   (A [M,K] row-major, B [N,K] row-major)        -- panel / trailing updates
 //   kind 1: C = alpha A B + beta C     (A [M,K] row-major, B [K,N] row-major)        -- factor-inverse blocks
 //   kind 2: C = alpha A^T B + beta C restricted to k >= max(row block, column block) (A [K,M], B [K,N]) -- Linv^T Linv
 // M, N multiples of 128, K a multiple of 32; all pointers on the device.
-int b200_debug_gemm_device(int version, int kind, int M, int N, int K, float alpha, const float* d_A, int lda, const float* d_B,
-                           int ldb, float beta, float* d_C, int ldc, void* stream) {
+int b200_debug_gemm_device(int kind, int M, int N, int K, float alpha, const float* d_A, int lda, const float* d_B, int ldb,
+                           float beta, float* d_C, int ldc, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(version == 1 || version == 2, "b200_debug_gemm: version must be 1 or 2");
     B200_REQUIRE(kind >= 0 && kind <= 2, "b200_debug_gemm: kind must be 0, 1 or 2");
     B200_REQUIRE(d_A && d_B && d_C && M > 0 && N > 0 && K > 0 && M % 128 == 0 && N % 128 == 0 && K % 32 == 0,
                  "b200_debug_gemm: M, N must be multiples of 128 and K of 32");
     cudaStream_t st = (cudaStream_t)stream;
-    const int saved = gemm_version();
-    g_gemm_version = version;
-    try {
-      if (kind == 0) gemm<false, true, false>(st, M, N, K, alpha, d_A, lda, 0, d_B, ldb, 0, beta, d_C, ldc, 0, 1);
-      else if (kind == 1) gemm<false, false, false>(st, M, N, K, alpha, d_A, lda, 0, d_B, ldb, 0, beta, d_C, ldc, 0, 1);
-      else gemm<true, false, true>(st, M, N, K, alpha, d_A, lda, 0, d_B, ldb, 0, beta, d_C, ldc, 0, 1);
-      B200_CUDA(cudaGetLastError());
-      B200_CUDA(cudaStreamSynchronize(st));
-    } catch (...) {
-      g_gemm_version = saved;
-      throw;
-    }
-    g_gemm_version = saved;
+    if (kind == 0) gemm<false, true, false>(st, M, N, K, alpha, d_A, lda, 0, d_B, ldb, 0, beta, d_C, ldc, 0, 1);
+    else if (kind == 1) gemm<false, false, false>(st, M, N, K, alpha, d_A, lda, 0, d_B, ldb, 0, beta, d_C, ldc, 0, 1);
+    else gemm<true, false, true>(st, M, N, K, alpha, d_A, lda, 0, d_B, ldb, 0, beta, d_C, ldc, 0, 1);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaStreamSynchronize(st));
   });
 }
 

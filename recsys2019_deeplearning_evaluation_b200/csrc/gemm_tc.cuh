@@ -1,16 +1,16 @@
-// fp32-accurate GEMM on the Hopper tensor cores (wgmma, sm_90a): C = alpha * op(A) * op(B) + beta * C.
+// Building blocks of the fp32-accurate GEMMs on the Hopper tensor cores (wgmma .tf32, sm_90a), shared by the EASE_R GEMM
+// (gemm_tc2.cuh) and the tensor-core IALS Gram (ials_v2.cuh).
 //
 // Each operand element x is split into two TF32 numbers, x = hi + lo (hi = rna_tf32(x), lo = rna_tf32(x - hi)), and every
-// 64 x 128 x 8 step of a warpgroup issues three wgmma.mma_async .tf32 instructions, hi*hi + hi*lo + lo*hi, into one fp32
+// K = 8 step of a warpgroup issues three wgmma.mma_async .tf32 instructions, hi*hi + hi*lo + lo*hi, into one fp32
 // accumulator tile held in registers ("3xTF32": the dropped lo*lo term is ~2^-22 relative, so the result is fp32-accurate,
 // which the 1e-4 parity bar of the EASE_R inverse needs; a single TF32 pass is not).
 //
-// One CTA (256 threads = two warpgroups) per 128 x 128 output tile; warpgroup g owns rows 64 g .. 64 g + 63.  K is consumed
-// in chunks of 32: all threads load the two operand chunks from global memory, split them and store hi / lo tiles in shared
-// memory in the canonical no-swizzle K-major layout (8-row x 16-byte core matrices; LBO = 128 B between K-adjacent cores,
-// SBO = 1024 B between 8-row groups), two stages deep.  The loads of chunk k+1 overlap the wgmmas of chunk k: a warpgroup
-// waits for its own wgmmas of chunk k before the block-wide barrier that publishes chunk k+1, so once that barrier is passed
-// nobody reads the stage chunk k+2 will overwrite.  Descriptor bit layout as cute/arch/mma_sm90_desc.hpp (GmmaDescriptor).
+// Operand tiles hold BK = 32 tf32 per row in shared memory in the canonical no-swizzle K-major layout (8-row x 16-byte core
+// matrices; LBO = 128 B between K-adjacent cores, SBO = 1024 B between 8-row groups), hi and lo in separate tiles.
+// tile_offset addresses that layout, make_smem_desc builds the wgmma descriptor of it (bit layout as
+// cute/arch/mma_sm90_desc.hpp, GmmaDescriptor), and load_tile_* fill a 128 x 32 hi / lo tile pair from global memory with
+// THREADS threads.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -20,8 +20,6 @@ namespace tc {
 
 constexpr int BM = 128, BN = 128, BK = 32;   // BK in fp32/tf32 elements (128 bytes per row)
 constexpr int TILE_BYTES = BM * BK * 4;      // 16 KB
-constexpr int STAGES = 2;
-constexpr int SMEM_BYTES = STAGES * 4 * TILE_BYTES;  // {A_hi, A_lo, B_hi, B_lo} per stage
 constexpr int THREADS = 256;
 constexpr uint32_t WG_ROWS_BYTES = 64 / 8 * (BK / 4) * 128;  // 64 tile rows = 8 row groups of 1024 B
 
@@ -148,66 +146,6 @@ __device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t a_d
 // row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
 __device__ __forceinline__ int frag_row(int i, int t) { return 16 * ((t >> 5) & 3) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
 __device__ __forceinline__ int frag_col(int i, int t) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
-
-// TA: op(A)(m, k) = A[k * lda + m]; TB: op(B)(k, n) = B[n * ldb + k].  TRI: op(A) = L^T, op(B) = L with L lower
-// triangular, so only k >= max(m0, n0) contributes.  M, N multiples of 128, K a multiple of 32.  blockIdx.z = batch.
-template <bool TA, bool TB, bool TRI>
-__global__ void __launch_bounds__(THREADS, 1) tc_gemm_kernel(int M, int N, int K, float alpha, const float* __restrict__ A, int lda,
-                                                             long long strideA, const float* __restrict__ B, int ldb, long long strideB,
-                                                             float beta, float* C, int ldc, long long strideC) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  A += (long long)blockIdx.z * strideA;
-  B += (long long)blockIdx.z * strideB;
-  C += (long long)blockIdx.z * strideC;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int tid = threadIdx.x, wg = tid >> 7;
-  unsigned char* tiles = smem;
-
-  float acc[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-
-  const int k_begin = TRI ? (max(m0, n0) / BK) * BK : 0;
-  const int nk = (K - k_begin) / BK;
-  for (int kb = 0; kb < nk; ++kb) {
-    const int s = kb & 1;
-    const int k0 = k_begin + kb * BK;
-    unsigned char* a_hi = tiles + (s * 4 + 0) * TILE_BYTES;
-    unsigned char* a_lo = tiles + (s * 4 + 1) * TILE_BYTES;
-    unsigned char* b_hi = tiles + (s * 4 + 2) * TILE_BYTES;
-    unsigned char* b_lo = tiles + (s * 4 + 3) * TILE_BYTES;
-    if (TA) load_tile_rowcontig(A, lda, m0, k0, a_hi, a_lo, tid); else load_tile_kcontig(A, lda, m0, k0, a_hi, a_lo, tid);
-    if (TB) load_tile_kcontig(B, ldb, n0, k0, b_hi, b_lo, tid); else load_tile_rowcontig(B, ldb, n0, k0, b_hi, b_lo, tid);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
-    wgmma_wait<0>();  // this warpgroup's wgmmas of chunk kb-1 (the other stage) are done
-    __syncthreads();
-    wgmma_fence();
-    const uint32_t ah = smem_u32(a_hi) + wg * WG_ROWS_BYTES, al = smem_u32(a_lo) + wg * WG_ROWS_BYTES;
-    const uint32_t bh = smem_u32(b_hi), bl = smem_u32(b_lo);
-#pragma unroll
-    for (int ks = 0; ks < BK / 8; ++ks) {  // one wgmma consumes K = 8 tf32 = two core matrices = 256 bytes
-      const uint32_t o = ks * 256u;
-      wgmma_m64n128k8_tf32(acc, make_smem_desc(ah + o), make_smem_desc(bh + o));
-      wgmma_m64n128k8_tf32(acc, make_smem_desc(ah + o), make_smem_desc(bl + o));
-      wgmma_m64n128k8_tf32(acc, make_smem_desc(al + o), make_smem_desc(bh + o));
-    }
-    wgmma_commit();
-  }
-  wgmma_wait<0>();
-
-  // epilogue: every thread writes its accumulator fragment, two adjacent columns per store
-  const int t = tid & 127;
-#pragma unroll
-  for (int i = 0; i < 64; i += 2) {
-    float2* dst = reinterpret_cast<float2*>(C + (long long)(m0 + wg * 64 + frag_row(i, t)) * ldc + n0 + frag_col(i, t));
-    float2 o = make_float2(alpha * acc[i], alpha * acc[i + 1]);
-    if (beta != 0.f) {
-      const float2 old = *dst;
-      o.x += beta * old.x; o.y += beta * old.y;
-    }
-    *dst = o;
-  }
-}
 
 }  // namespace tc
 }  // namespace b200

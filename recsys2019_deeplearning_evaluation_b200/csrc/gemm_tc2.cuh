@@ -1,16 +1,14 @@
-// Second-generation 3xTF32 wgmma GEMM (sm_90a): pre-packed operands fed by the TMA engine's bulk copies.
+// 3xTF32 wgmma GEMM of the EASE_R inverse (sm_90a): pre-packed operands fed by the TMA engine's bulk copies.
 //
-// gemm_tc.cuh spends most of its time converting operands (cvt.rna.tf32) and storing them transposed with 4-byte stores,
-// and the loads of chunk k+1 only start after the whole block has synchronised on chunk k.  Here
 //   * a pack pass splits every operand ONCE into hi / lo TF32 parts and writes them in the exact shared-memory image of a
-//     128 x 32 wgmma tile (canonical no-swizzle K-major layout, same tile_offset as gemm_tc.cuh), hi and lo adjacent:
+//     128 x 32 wgmma tile (canonical no-swizzle K-major layout, tc::tile_offset of gemm_tc.cuh), hi and lo adjacent:
 //     packed[(row_block * KC + k_chunk) * 8192 floats] = {hi tile 16 KB, lo tile 16 KB};
 //   * the GEMM kernel is warp-specialised: one producer lane (warpgroup 0) issues two 32 KB `cp.async.bulk` copies per
 //     128x128x32 step (A hi+lo, B hi+lo) that complete on the stage's "full" mbarrier; each of the two consumer warpgroups
 //     waits for it, issues the 12 wgmmas of its 64 x 128 half of the step (hi*hi + hi*lo + lo*hi) and, once the wgmmas of
 //     the step before have completed, releases that step's stage on its "empty" mbarrier; three stages deep (192 KB), no
 //     block-wide barrier at all;
-//   * each consumer warpgroup writes its accumulators from registers (the epilogue of gemm_tc.cuh).
+//   * each consumer warpgroup writes its accumulators from registers.
 // O(M K + N K) pack work against O(M N K) MMA work; the packed copies live in a workspace the caller provides.
 #pragma once
 #include "gemm_tc.cuh"

@@ -96,13 +96,7 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-__device__ __forceinline__ void red_add4(float* addr, float4 v) {
-#if __CUDA_ARCH__ >= 900
-  atomicAdd(reinterpret_cast<float4*>(addr), v);
-#else
-  atomicAdd(addr, v.x); atomicAdd(addr + 1, v.y); atomicAdd(addr + 2, v.z); atomicAdd(addr + 3, v.w);
-#endif
-}
+__device__ __forceinline__ void red_add4(float* addr, float4 v) { atomicAdd(reinterpret_cast<float4*>(addr), v); }
 
 __device__ __forceinline__ void touch(int* flag, int* list, int* counter, int row) {
   if (atomicExch(flag + row, 1) == 0) list[atomicAdd(counter, 1)] = row;

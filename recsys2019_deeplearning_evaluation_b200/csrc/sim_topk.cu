@@ -55,19 +55,6 @@ constexpr int SELT = B200_SELT;  // threads that run the select
 #define B200_UB 2
 #endif
 constexpr int UB = B200_UB;      // 128-bit loads in flight per lane
-#ifndef B200_PREFETCH
-#define B200_PREFETCH 0
-#endif
-#ifndef B200_GUESS
-#define B200_GUESS 0
-#endif
-// B200_GUESS: every CTA carries a guess of the K-th best similarity over to its next column (0.9 x the K-th best of
-// the column it just finished; consecutive columns of the longest-first order are alike).  One sweep of the first window
-// counts the cells that are GUARANTEED to reach the guess (one half-word compare + popcount per vector); if there are at
-// least K the guess is a valid floor and the three-level bootstrap histogram is skipped, otherwise it runs as before.
-// B200_PREFETCH: while the select group (SELT threads) prunes the finished column, the other threads walk the NEXT
-// column's CSC entries -> row-segment bounds and issue L2 prefetches for those row segments, so that the next column's
-// stage and accumulate phases find their three dependent levels of data in L2 instead of DRAM.
 constexpr int MAXTILES = 16;
 #define B200_MAX_PEERS 8  // output tables one launch can write: the local one + up to 7 peers of an 8-GPU box
 
@@ -205,30 +192,6 @@ __device__ __forceinline__ float dot_threshold(const KParams& p, float t, float 
   return r > 0.f ? r * (1.f - 1e-5f) : 0.f;
 }
 
-// Smallest dot product that reaches similarity `t` (> 0) for EVERY neighbour norm term in [b_lo, b_hi] (the inverse is
-// monotone in b for every formula, so the larger end decides), widened upwards by 1e-4 so that a cell counted with it
-// survives the exact evaluation; 3.4e38 when no such dot product exists.
-template <int F>
-__device__ __forceinline__ float dot_threshold_sure(const KParams& p, float t, float a, float b_lo, float b_hi) {
-  float r = 0.f;
-#pragma unroll
-  for (int e = 0; e < 2; ++e) {
-    const float b = e ? b_hi : b_lo;
-    float v;
-    if (F == F_PROD) v = t * (a * b + p.se);
-    else if (F == F_NONORM) v = t * p.shrink_div;
-    else if (F == F_JACCARD) v = t * (a + b + p.se) / (1.f + t);
-    else if (F == F_DICE) v = t * (a + b + p.se);
-    else if (F == F_SCALE) v = (a * b > 0.f) ? t / (a * b) : 3.4e38f;
-    else {
-      const float den = 1.f - t * (1.f - p.ta - p.tb);
-      v = (den > 1e-6f && p.ta >= 0.f && p.tb >= 0.f) ? t * (a * p.ta + b * p.tb + p.se) / den : 3.4e38f;
-    }
-    r = fmaxf(r, v);
-  }
-  return r < 1e37f ? r * (1.f + 1e-4f) + 1e-30f : 3.4e38f;
-}
-
 // s such that sim_value(d, a, b) >= d * s for every positive d the data can produce and every b in
 // [b_lo, b_hi] (a cheap per-tile lower bound for the bootstrap histogram); 0 when no useful bound exists.
 template <int F>
@@ -272,8 +235,6 @@ __device__ __forceinline__ unsigned key32_of(float v) {
 
 struct Shared {
   int col;
-  float guess;  // B200_GUESS: 0 = none
-  int next;  // B200_PREFETCH: the counter value (position in the processing order) this CTA handles after `col`
   int nbuf;
   int overflow;
   int npos, nneg;
@@ -465,34 +426,6 @@ __device__ __forceinline__ void store_cells(void* acc, int iv, const float* k) {
     reinterpret_cast<int4*>(acc)[iv] = make_int4((int)k[0], (int)k[1], (int)k[2], (int)k[3]);
   } else {
     reinterpret_cast<float4*>(acc)[iv] = make_float4(k[0], k[1], k[2], k[3]);
-  }
-}
-
-__device__ __forceinline__ void prefetch_l2_range(const void* base, long long byte_lo, long long byte_hi) {
-  const char* b = reinterpret_cast<const char*>(base);
-  for (long long o = byte_lo & ~127ll; o < byte_hi; o += 128)
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(b + o));
-}
-
-// Threads q = 0 .. nthr-1 (the ones that idle during the last select of a column): L2 prefetch of everything the column
-// at position `c_next` of the processing order will gather.
-template <bool BINARY>
-__device__ __forceinline__ void prefetch_column(const KParams& p, int c_next, int q, int nthr) {
-  if (c_next >= p.n_range) return;
-  const int lc = p.order ? p.order[c_next] : c_next;
-  const int col = p.old2new[p.col_begin + lc];
-  const int cs = p.csc_ptr[col], ce = p.csc_ptr[col + 1];
-  for (int t = cs + q; t < ce; t += nthr) {
-    const int u = BINARY ? p.csc_idx[t] : p.csc_ent[t].x;
-    if (p.n_win == 1 && !BINARY) {
-      const int s0 = p.csr_ptr[u], e0 = p.csr_ptr[u + 1];
-      prefetch_l2_range(p.csr_ent, 8ll * s0, 8ll * e0);
-    } else {
-      const int* sp = p.split + (size_t)u * (p.n_win + 1);
-      const int s0 = sp[0], e0 = sp[p.n_win];  // the windows of a row are contiguous in memory
-      if (BINARY) prefetch_l2_range(p.csr_idx, 4ll * s0, 4ll * e0);
-      else prefetch_l2_range(p.csr_ent, 8ll * s0, 8ll * e0);
-    }
   }
 }
 
@@ -713,35 +646,6 @@ __device__ void process_column(const KParams& p, int col, int target, int out_ba
     }
 
     nbuf = sh->nbuf;
-#if B200_GUESS
-    if (F != F_EUCLID && !NEG && thr == 0 && nbuf == 0 && win_n > 2 * target && sh->guess > 0.f) {
-      const float g = sh->guess;
-      if (tid == 0) sh->cnt = 0;
-      if (tid < ntiles) {
-        const float dt = dot_threshold_sure<F>(p, g, Ai, tB[tid], tB[tid + 1]);
-        sh->dthr[tid] = dt;
-        if (PACK) sh->k2[tid] = half_k2(dt);
-      }
-      __syncthreads();
-      int sure = 0;
-      for (int iv = tid; iv < winv; iv += THREADS) {
-        if (PACK) {
-          sure += __popc(half_ge_mask(reinterpret_cast<const uint4*>(acci)[iv], sh->k2[iv / THREADS]));
-        } else {
-          float d[CPV];
-          if (!load_cells<BINARY, PACK>(acci, iv, d)) continue;
-          const float dthr = sh->dthr[iv / THREADS];
-#pragma unroll
-          for (int c = 0; c < CPV; ++c) sure += (d[c] > 0.f && d[c] >= dthr) ? 1 : 0;
-        }
-      }
-      sure = __reduce_add_sync(0xffffffffu, sure);
-      if (lane == 0 && sure) atomicAdd(&sh->cnt, sure);
-      __syncthreads();
-      if (sh->cnt >= target) thr = ((u64)__float_as_uint(g)) << 32;
-      __syncthreads();  // sh->cnt, dthr and k2 are rewritten below
-    }
-#endif
     // ---------------- bootstrap: floor of the target-th best similarity from per-cell lower bounds
     if (!NEG && thr == 0 && nbuf == 0 && win_n > 2 * target) {
       for (int i = tid; i < HBINS; i += THREADS) hist[i] = 0;
@@ -903,16 +807,6 @@ __device__ void process_column(const KParams& p, int col, int target, int out_ba
     nbuf = sh->nbuf;
     if (nbuf > p.cap / 2 || w == p.n_win - 1) {
       int kept;  // the window is all zero here and select leaves its scratch zeroed
-#if B200_PREFETCH
-      if (w == p.n_win - 1) {
-        __syncthreads();
-        if (tid < SELT) select_group(buf, nbuf, target, sh, acci);
-        else prefetch_column<BINARY>(p, sh->next, tid - SELT, THREADS - SELT);
-        __syncthreads();
-        kept = sh->cnt;
-        thr = max(thr, sh->sel_thr);
-      } else
-#endif
       thr = max(thr, block_select(buf, nbuf, target, sh, acci, &kept));
       if (tid == 0) sh->nbuf = kept;
       nbuf = kept;
@@ -922,23 +816,13 @@ __device__ void process_column(const KParams& p, int col, int target, int out_ba
   }
 
   // ---------------- emit (keys carry the ORIGINAL neighbour index; the last select left no dead slots)
-#if B200_GUESS
-  if (!NEG && tid == 0) sh->kmin = 0xFFFFFFFFu;
-  __syncthreads();
-#endif
   for (int t = tid; t < nbuf; t += THREADS) {
     const u64 k = buf[t];
     const unsigned hi = (unsigned)(k >> 32);
-#if B200_GUESS
-    if (!NEG) atomicMin(&sh->kmin, hi);
-#endif
     emit_entry(p, (size_t)out_base + t, (int)(0xFFFFFFFFu - (unsigned)k), __uint_as_float(NEG ? ~hi : hi));
   }
   *n_emitted = nbuf;
   __syncthreads();
-#if B200_GUESS
-  if (!NEG && tid == 0) sh->guess = (F != F_EUCLID && nbuf >= target) ? 0.9f * __uint_as_float(sh->kmin) : 0.f;
-#endif
   PROF_MARK(6);
 }
 
@@ -954,26 +838,14 @@ __global__ void __launch_bounds__(THREADS, 1) sim_topk_kernel(const KParams p) {
     const int4 z = make_int4(0, 0, 0, 0);
     for (int i4 = tid; i4 < (p.acc_cells >> 2); i4 += THREADS) reinterpret_cast<int4*>(smem_raw)[i4] = z;
     for (int i = tid; i < p.n_win * (MAXTILES + 1); i += THREADS) s_tileB[i] = p.tileB[i];
-    if (tid == 0) sh.guess = 0.f;
   }
   __syncthreads();
   const int n_range = p.n_range_dev ? *p.n_range_dev : p.n_range;
-#if B200_PREFETCH
-  if (tid == 0) sh.next = atomicAdd(p.counter, 1);
-#endif
   while (true) {
-#if B200_PREFETCH
-    __syncthreads();
-    const int c = sh.next;
-    __syncthreads();
-    if (c >= n_range) break;
-    if (tid == 0) sh.next = atomicAdd(p.counter, 1);  // read by the prefetching threads many barriers later
-#else
     if (tid == 0) sh.col = atomicAdd(p.counter, 1);
     __syncthreads();
     const int c = sh.col;
     if (c >= n_range) break;
-#endif
     const int lc = p.order ? p.order[c] : c;
     const int col = p.old2new[p.col_begin + lc];  // new numbering
     const int out_base_row = lc;

@@ -68,7 +68,7 @@ def test_dense_similarity_outputs():
     assert (np.diff(Wk.tocsc().indptr) <= 2100).all() and Wk.nnz > 0
 
 
-def _gemm_case(version, kind, M, N, K, beta):
+def _gemm_case(kind, M, N, K, beta):
     import ctypes
     import torch
     from recsys2019_deeplearning_evaluation_b200 import _lib
@@ -81,26 +81,21 @@ def _gemm_case(version, kind, M, N, K, beta):
         A, B = torch.tril(A), torch.tril(B)
     C0 = torch.randn((M, N), generator=g, dtype=torch.float32).cuda()
     C = C0.clone()
-    _lib.check(_lib.load().b200_debug_gemm_device(version, kind, M, N, K, 0.75, A.data_ptr(), A.shape[1], B.data_ptr(), B.shape[1],
-                                                  beta, C.data_ptr(), N, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    _lib.check(_lib.load().b200_debug_gemm_device(kind, M, N, K, 0.75, A.data_ptr(), A.shape[1], B.data_ptr(), B.shape[1], beta,
+                                                  C.data_ptr(), N, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
     Ad, Bd = A.double(), B.double()
     ref = 0.75 * (Ad @ Bd.t() if kind == 0 else (Ad @ Bd if kind == 1 else Ad.t() @ Bd)) + beta * C0.double()
     err = (C.double() - ref).abs().max().item() / ref.abs().max().item()
     # 3xTF32: fp32-level accuracy (a single TF32 pass gives ~3e-4).  The tensor core accumulates with truncation, so the
     # error grows linearly with the number of K = 8 steps.
-    assert err < 1e-5 * max(1.0, K / 512.0), (version, kind, M, N, K, beta, err)
+    assert err < 1e-5 * max(1.0, K / 512.0), (kind, M, N, K, beta, err)
 
 
 GEMM_SHAPES = [(0, 384, 128, 128, 0.0), (0, 256, 256, 128, 1.0), (1, 128, 128, 640, 0.0), (2, 512, 512, 512, 0.0)]
 
 
-@pytest.mark.parametrize("kind,M,N,K,beta", GEMM_SHAPES)
-def test_tensor_core_gemm_v1(kind, M, N, K, beta):
-    """The three GEMM shapes of the blocked inverse through the first wgmma kernel (B200REC_GEMM=1), against fp64."""
-    _gemm_case(1, kind, M, N, K, beta)
-
-
 @pytest.mark.parametrize("kind,M,N,K,beta", GEMM_SHAPES + [(0, 1024, 1024, 128, 1.0), (2, 2048, 2048, 2048, 0.0)])
-def test_tensor_core_gemm_v2(kind, M, N, K, beta):
-    """The default kernel (pre-packed hi/lo TF32 operands, cp.async.bulk producer, mbarrier ring)."""
-    _gemm_case(2, kind, M, N, K, beta)
+def test_tensor_core_gemm(kind, M, N, K, beta):
+    """The three GEMM shapes of the blocked inverse (pre-packed hi/lo TF32 operands, cp.async.bulk producer, mbarrier
+    ring), against fp64."""
+    _gemm_case(kind, M, N, K, beta)

@@ -1,5 +1,5 @@
 """Development A/B timing of libb200rec variants on one GPU (one URM generation, one subprocess per library):
-    python tools/ab_sim_bench.py C5 binary default prefetch ...
+    python tools/ab_sim_bench.py C5 binary default ub4 ...
 `default` = the in-tree libb200rec.so, any other name = recsys2019_deeplearning_evaluation_b200/_variants/libb200rec_<name>.so"""
 import os, subprocess, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
