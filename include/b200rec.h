@@ -288,7 +288,12 @@ int b200_slim_shard_device(b200_slim_t h, float** d_S, int* col_lo, int* col_hi)
  * replaces  Base/Recommender_utils.py:55-122 similarityMatrixTopK            (along_columns=1, mode 0)
  *           SLIM_BPR_Cython_Epoch.pyx:1335-1415 / :371,386 row top-K of get_S (along_columns=0, mode 1 / 0)
  * mode 0: the K largest of the non-zero values; mode 1: the K largest over all cells, zeros then dropped.
- * Output table [n, K] like b200_sim_compute_device (line = row or column, idx = position along it).
+ * Ties go to the ascending index; -0.0 is a zero.  NaN is a non-zero cell: it ranks above +inf in mode 0 (the
+ * reference's argsort, last K) and below -inf in modes 1 and 2 (argpartition of the negated line).
+ * Output table [n, K] like b200_sim_compute_device (line = row or column, idx = position along it): d_cnt[l] <= K
+ * entries in slots 0..d_cnt[l]-1 (in no particular order), slots d_cnt[l]..K-1 hold idx -1 / value 0.0.  A line
+ * never writes outside its K slots, whatever the input (a duplicated (index, value) entry of a compressed line is
+ * taken at most as often as the selection needs).
  * ------------------------------------------------------------------------------------------------ */
 enum b200_topk_mode { B200_TOPK_NONZERO = 0, B200_TOPK_ZEROS_OUTRANK = 1,
                       /* SLIMElasticNetRecommender.py:99-107: the min(nnz - 1, K) largest non-zero values of a line */

@@ -9,6 +9,10 @@
 //     coefficients: a line with <= k non-zeros loses its smallest one                  -> mode 2
 // One CTA per line; the line is streamed from HBM/L2 once per radix pass (11-bit digits over the 64-bit key
 // value-bits << 32 | ~index, so ties resolve to the ascending index); survivors are written as a [lines, K] table.
+// NaN is a non-zero cell and ranks where the reference's numpy call puts it: above +inf in mode 0 (argsort ascending,
+// last k), below -inf in modes 1 and 2 (argpartition of the negated line). A line never emits more than K entries:
+// cells whose key equals the threshold (a duplicated (index, value) entry of a compressed line) are taken only as many
+// times as the selection still needs.
 #include <algorithm>
 
 #include "common.cuh"
@@ -27,6 +31,11 @@ __device__ __forceinline__ unsigned orderable(float v) {
 __device__ __forceinline__ float from_orderable(unsigned o) {
   return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
 }
+// orderable() maps +NaN above +inf and -NaN below -inf; every NaN is moved to one end instead, by mode
+__device__ __forceinline__ u64 line_key(float v, int qi, bool nan_high) {
+  const unsigned o = v != v ? (nan_high ? 0xFFFFFFFFu : 0u) : orderable(v);
+  return (((u64)o) << 32) | (u64)(0xFFFFFFFFu - (unsigned)qi);
+}
 
 // SPARSE: line l is the segment [ptr[l], ptr[l+1]) of (sidx, M); its cells are the stored entries and the implicit
 // zeros of a length-n_inner line.
@@ -36,33 +45,39 @@ __global__ void __launch_bounds__(THREADS) topk_lines_kernel(const float* __rest
                                                              long long stride_line, long long stride_inner, int K, int mode,
                                                              int* out_idx, float* out_val, int* out_cnt, int idx_off = 0) {
   __shared__ int hist[BINS];
-  __shared__ int s_digit, s_need, s_cnt, s_npos, s_nneg;
+  __shared__ int s_digit, s_need, s_cnt, s_tie, s_npos, s_nneg, s_nnan;
   const int tid = threadIdx.x, lane = tid & 31;
+  const bool nan_high = mode == 0;
   for (int line = blockIdx.x; line < n_lines; line += gridDim.x) {
     const float* L = SPARSE ? M + ptr[line] : M + (long long)line * stride_line;
     const int* LI = SPARSE ? sidx + ptr[line] : nullptr;
     const int n_inner = SPARSE ? ptr[line + 1] - ptr[line] : n_inner_dense;
     if (SPARSE) stride_inner = 1;
-    if (tid == 0) { s_npos = 0; s_nneg = 0; s_cnt = 0; }
+    if (tid == 0) { s_npos = 0; s_nneg = 0; s_nnan = 0; s_cnt = 0; s_tie = 0; }
     __syncthreads();
-    int npos = 0, nneg = 0;
+    int npos = 0, nneg = 0, nnan = 0;
     for (int q = tid; q < n_inner; q += THREADS) {
       const float v = L[(long long)q * stride_inner];
       npos += v > 0.f;
       nneg += v < 0.f;
+      nnan += v != v;
     }
     npos = __reduce_add_sync(0xffffffffu, npos);
     nneg = __reduce_add_sync(0xffffffffu, nneg);
-    if (lane == 0) { atomicAdd(&s_npos, npos); atomicAdd(&s_nneg, nneg); }
+    nnan = __reduce_add_sync(0xffffffffu, nnan);
+    if (lane == 0) { atomicAdd(&s_npos, npos); atomicAdd(&s_nneg, nneg); atomicAdd(&s_nnan, nnan); }
     __syncthreads();
-    npos = s_npos; nneg = s_nneg;
-    const int nzero = n_inner_dense - npos - nneg;
+    npos = s_npos; nneg = s_nneg; nnan = s_nnan;
+    const int nnz = npos + nneg + nnan;  // the cells with v != 0
+    const int nzero = n_inner_dense - nnz;
     int keep;  // how many non-zero cells survive
-    if (mode == 0) keep = min(K, npos + nneg);                                   // similarityMatrixTopK
-    else if (mode == 2) keep = max(0, min(K, npos + nneg - 1));                  // SLIMElasticNetRecommender.py:103
-    else keep = min(K, npos) + min(nneg, max(0, K - npos - nzero));               // zeros outrank negatives
+    if (mode == 0) keep = min(K, nnz);                                           // similarityMatrixTopK
+    else if (mode == 2) keep = max(0, min(K, nnz - 1));                          // SLIMElasticNetRecommender.py:103
+    else keep = min(K, npos) + min(nneg + nnan, max(0, K - npos - nzero));        // zeros outrank negatives, NaN last
+    keep = min(keep, K);  // nzero < 0 when a compressed line holds more entries than n
     u64 thr = 0;
-    if (keep > 0 && keep < npos + nneg) {
+    int ties = keep;  // how many cells with key == thr are taken
+    if (keep > 0 && keep < nnz) {
       u64 prefix = 0, mask = 0;
       int need = keep;
       for (int shift = 53; ; shift -= 11) {
@@ -73,7 +88,7 @@ __global__ void __launch_bounds__(THREADS) topk_lines_kernel(const float* __rest
         for (int q = tid; q < n_inner; q += THREADS) {
           const float v = L[(long long)q * stride_inner];
           if (v != 0.f) {
-            const u64 key = (((u64)orderable(v)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)(SPARSE ? LI[q] : q + idx_off));
+            const u64 key = line_key(v, SPARSE ? LI[q] : q + idx_off, nan_high);
             if ((key & mask) == prefix) atomicAdd(&hist[(int)((key >> sh) & ((1u << nb) - 1))], 1);
           }
         }
@@ -102,16 +117,17 @@ __global__ void __launch_bounds__(THREADS) topk_lines_kernel(const float* __rest
         __syncthreads();
         if (shift <= 0) break;
       }
-      thr = prefix;  // the keep-th largest key itself (keys are distinct)
+      thr = prefix;  // the keep-th largest key itself
+      ties = need;   // 1 unless entries repeat (index, value): keys are distinct within a line otherwise
     }
-    // emit
+    // emit: keep - ties keys above thr, then `ties` of the keys equal to it
     if (keep > 0) {
       for (int q = tid; q < n_inner; q += THREADS) {
         const float v = L[(long long)q * stride_inner];
         if (v != 0.f) {
           const int qi = SPARSE ? LI[q] : q + idx_off;
-          const u64 key = (((u64)orderable(v)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)qi);
-          if (key >= thr) {
+          const u64 key = line_key(v, qi, nan_high);
+          if (key > thr || (key == thr && atomicAdd(&s_tie, 1) < ties)) {
             const int pos = atomicAdd(&s_cnt, 1);
             out_idx[(size_t)line * K + pos] = qi;
             out_val[(size_t)line * K + pos] = v;

@@ -28,10 +28,14 @@ def _row_l1_normalize(M):
 
 
 def sparse_column_topk(W, k):
-    """similarityMatrixTopK (Base/Recommender_utils.py:55-122) for a scipy sparse matrix, on the device."""
+    """similarityMatrixTopK (Base/Recommender_utils.py:55-122) for a scipy sparse matrix, on the device.  A duplicated
+    entry stands for the sum of its values, as everywhere in scipy."""
     import torch
     lib = _lib.load()
     Wc = sps.csc_matrix(W, dtype=np.float32)
+    if not Wc.has_canonical_format:  # the kernel reads every stored entry as a cell of its own; W stays untouched
+        Wc = Wc.copy()
+        Wc.sum_duplicates()
     n = Wc.shape[1]
     k = int(min(k, n))
     dev = torch.device("cuda", torch.cuda.current_device())

@@ -40,50 +40,53 @@ def test_sequential_parity_on_the_glibc_stream(symmetric, mode):
 
 def test_get_S_topk_semantics():
     """Row top-K: symmetric = K largest over all cells with zeros dropped (pyx:1335-1415); dense = K largest non-zero
-    (similarityMatrixTopK(S.T).T, pyx:371,386)."""
-    X = synth_urm(400, 150, 0.06, seed=5)
-    for symmetric in (True, False):
-        kw = dict(learning_rate=0.05, li_reg=1e-3, lj_reg=1e-3, topK=10, symmetric=symmetric, random_seed=1, sgd_mode="adagrad")
-        g = _cls()(X, **kw)
-        for _ in range(4):
-            g.epochIteration_Cython()
-        D = g.get_S_dense().astype(np.float64)
-        W = g.get_S()
-        assert sps.issparse(W) and W.shape == (150, 150)
-        W = W.toarray()
-        for r in range(150):
-            row = D[r]
-            if symmetric:
-                order = np.lexsort((np.arange(150), -row))[:10]
-                keep = order[row[order] != 0]
-            else:
-                nz = np.flatnonzero(row)
-                keep = nz[np.lexsort((nz, -row[nz]))][:10]
-            ref = np.zeros(150)
-            ref[keep] = row[keep]
-            assert np.allclose(W[r], ref, rtol=1e-6, atol=0), r
+    (similarityMatrixTopK(S.T).T, pyx:371,386).  1 200 items: more rows than the selection kernel's grid of 8 CTAs per SM."""
+    for X in (synth_urm(400, 150, 0.06, seed=5), synth_urm(2500, 1200, 0.02, seed=5)):
+        n = X.shape[1]
+        for symmetric in (True, False):
+            kw = dict(learning_rate=0.05, li_reg=1e-3, lj_reg=1e-3, topK=10, symmetric=symmetric, random_seed=1, sgd_mode="adagrad")
+            g = _cls()(X, **kw)
+            for _ in range(4):
+                g.epochIteration_Cython()
+            D = g.get_S_dense().astype(np.float64)
+            W = g.get_S()
+            assert sps.issparse(W) and W.shape == (n, n)
+            W = W.toarray()
+            for r in range(n):
+                row = D[r]
+                if symmetric:
+                    order = np.lexsort((np.arange(n), -row))[:10]
+                    keep = order[row[order] != 0]
+                else:
+                    nz = np.flatnonzero(row)
+                    keep = nz[np.lexsort((nz, -row[nz]))][:10]
+                ref = np.zeros(n)
+                ref[keep] = row[keep]
+                assert np.allclose(W[r], ref, rtol=1e-6, atol=0), (n, r)
 
 
 def test_similarityMatrixTopK_gpu_matches_recipe():
-    """Base/Recommender_utils_Test.py:18-50: nnz per column and dense == sparse; plus the negatives-survive rule."""
+    """Base/Recommender_utils_Test.py:18-50: nnz per column and dense == sparse; plus the negatives-survive rule.
+    1 200 columns: more lines than the selection kernel's grid of 8 CTAs per SM."""
     from recsys2019_deeplearning_evaluation_b200.slim_bpr_epoch import similarityMatrixTopK
     rng = np.random.default_rng(0)
-    n, k = 200, 20
-    D = rng.standard_normal((n, n)).astype(np.float32)
-    D[rng.random((n, n)) < 0.7] = 0
-    D[:, 3] = 0
-    D[:5, 7] = [-1, -2, -3, 0.5, 0]; D[5:, 7] = 0   # 1 positive, 3 negatives: all four survive for k >= 4
-    W = similarityMatrixTopK(D, k=k)
-    assert sps.isspmatrix_csc(W) and W.dtype == np.float32
-    Wd = W.toarray()
-    for c in range(n):
-        col = D[:, c]
-        nz = np.flatnonzero(col)
-        keep = nz[np.lexsort((nz, -col[nz]))][:k]
-        ref = np.zeros(n, np.float32)
-        ref[keep] = col[keep]
-        assert np.array_equal(Wd[:, c], ref), c
-    assert (np.diff(W.indptr) <= k).all() and W[:, 3].nnz == 0 and W[:, 7].nnz == 4
+    for n in (200, 1200):
+        k = 20
+        D = rng.standard_normal((n, n)).astype(np.float32)
+        D[rng.random((n, n)) < 0.7] = 0
+        D[:, 3] = 0
+        D[:5, 7] = [-1, -2, -3, 0.5, 0]; D[5:, 7] = 0   # 1 positive, 3 negatives: all four survive for k >= 4
+        W = similarityMatrixTopK(D, k=k)
+        assert sps.isspmatrix_csc(W) and W.dtype == np.float32
+        Wd = W.toarray()
+        for c in range(n):
+            col = D[:, c]
+            nz = np.flatnonzero(col)
+            keep = nz[np.lexsort((nz, -col[nz]))][:k]
+            ref = np.zeros(n, np.float32)
+            ref[keep] = col[keep]
+            assert np.array_equal(Wd[:, c], ref), (n, c)
+        assert (np.diff(W.indptr) <= k).all() and W[:, 3].nnz == 0 and W[:, 7].nnz == 4
 
 
 def test_philox_stream_and_hogwild():
