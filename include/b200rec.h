@@ -334,6 +334,14 @@ int b200_score_mask_device(const int32_t* d_users, int n_users_block, const int3
  * -inf, then NaN; ties (-0 == +0) by ascending item index.  [n_rows, cutoff] tables; past the end of a row -1 / -inf */
 int b200_score_topn_device(const float* d_scores, int n_rows, int n_items, int cutoff, int32_t* d_items,
                            float* d_item_scores, void* stream);
+/* The two calls above on a dense row-major [n_rows, n_items] fp64 block: the score blocks of recommenders that score on
+ * the host in float64, ranked without rounding them to fp32.  The top-N order is that of b200_score_topn_device on the fp64
+ * values (96-bit keys: the orderable double, then ~item).  d_item_scores receives each selected score rounded to fp32 with
+ * finite values saturated to +-FLT_MAX, so that an entry is finite exactly when its fp64 score is. */
+int b200_score_mask_f64_device(const int32_t* d_users, int n_users_block, const int32_t* d_urm_ptr, const int32_t* d_urm_idx,
+                               const unsigned char* d_items_keep, int n_items, double* d_scores, void* stream);
+int b200_score_topn_f64_device(const double* d_scores, int n_rows, int n_items, int cutoff, int32_t* d_items,
+                               float* d_item_scores, void* stream);
 /* Candidate lists (EvaluatorNegativeItemSample, Evaluator.py:466-578): row b of a block of n_block users is d_users[b]'s
  * list d_cand_idx[d_cand_ptr[b] .. d_cand_ptr[b+1]) of strictly ascending item ids (d_cand_ptr may point into a larger
  * CSR: offsets stay absolute).  Per-candidate arrays are ragged fp32 [d_cand_ptr[n_block] - d_cand_ptr[0]], entry k at

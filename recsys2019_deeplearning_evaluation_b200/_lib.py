@@ -96,6 +96,8 @@ SIGNATURES = {
     "b200_score_mf_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void, c_void, c_void]),
     "b200_score_mask_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, ctypes.c_int, c_void, c_void]),
     "b200_score_topn_device": (ctypes.c_int, [c_void, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void]),
+    "b200_score_mask_f64_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, ctypes.c_int, c_void, c_void]),
+    "b200_score_topn_f64_device": (ctypes.c_int, [c_void, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void]),
     "b200_cand_score_sparse_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, c_void, c_void, c_void, c_void,
                                                      c_void, c_void]),
     "b200_cand_score_dense_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, c_void, c_void, ctypes.c_int, c_void, c_void,

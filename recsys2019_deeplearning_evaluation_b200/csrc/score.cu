@@ -10,7 +10,10 @@
 // mask / top-N passes) and, for the sparse product, 8 bytes per gathered (j, w) pair of W.
 // The cand_* kernels score and rank per-user candidate lists instead (Evaluator.py:466-578, test items plus sampled
 // negatives, ~100 per user): the work is proportional to the candidates, not to B * n_items.
+// The mask and top-N kernels also take fp64 blocks: the evaluators rank the host score blocks of recommenders that are
+// not this package's mirrors, and those often score in float64.
 #include <algorithm>
+#include <cfloat>
 
 #include "common.cuh"
 
@@ -94,8 +97,9 @@ __global__ void transpose_kernel(const float* __restrict__ in, int rows, int col
 }
 
 // scores[b, seen items of users[b]] = -inf (BaseRecommender.py:164-169); one warp per user
+template <typename T>
 __global__ void mask_seen_kernel(const int* __restrict__ users, int n_users_block, const int* __restrict__ ptr,
-                                 const int* __restrict__ idx, int n_items, float* scores) {
+                                 const int* __restrict__ idx, int n_items, T* scores) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= n_users_block) return;
   const int u = users[warp];
@@ -103,7 +107,8 @@ __global__ void mask_seen_kernel(const int* __restrict__ users, int n_users_bloc
 }
 
 // items_to_compute (BaseSimilarityMatrixRecommender.py:80-86): every other item -> -inf.  keep[j] != 0 marks kept items.
-__global__ void mask_items_kernel(const unsigned char* __restrict__ keep, int n_users_block, int n_items, float* scores) {
+template <typename T>
+__global__ void mask_items_kernel(const unsigned char* __restrict__ keep, int n_users_block, int n_items, T* scores) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= (long long)n_users_block * n_items) return;
   if (!keep[g % n_items]) scores[g] = -INFINITY;
@@ -116,33 +121,104 @@ __device__ __forceinline__ unsigned orderable(float v) {
   const unsigned b = __float_as_uint(v == 0.f ? 0.f : v);
   return v != v ? 0u : (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
+// the same order on doubles: NaN -> 0, below -inf's 0x000FFFFFFFFFFFFF
+__device__ __forceinline__ u64 orderable(double v) {
+  const u64 b = (u64)__double_as_longlong(v == 0.0 ? 0.0 : v);
+  return v != v ? 0ull : (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
+}
+
+// The top-N key of the score at position q: the orderable score, then ~q, so that larger keys rank first and equal
+// scores go to the lower position.  fp32: one 64-bit word, 6 radix passes of 11 bits.  fp64: 96 bits (the 64-bit
+// orderable double, then ~q), 9 passes; the radix digit at bit `sh` may straddle the two words.  `image` is what the
+// table reports for a score: fp32 as it is; fp64 rounded to fp32 with finite values saturated to +-FLT_MAX, so that an
+// entry is finite exactly when its score is (the evaluation kernels read nothing else).
+template <typename T> struct TopnKey;
+template <> struct TopnKey<float> {
+  typedef u64 Key;
+  static constexpr int TOP_SHIFT = 53;  // digits at bits 53, 42, ..., 9 and the last 9 bits
+  static __device__ __forceinline__ Key make(float v, int q) {
+    return (((u64)orderable(v)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
+  }
+  static __device__ __forceinline__ int digit(Key k, int sh, int nb) { return (int)((k >> sh) & ((1u << nb) - 1)); }
+  static __device__ __forceinline__ bool matches(Key k, Key prefix, Key mask) { return (k & mask) == prefix; }
+  static __device__ __forceinline__ void fix_digit(Key& prefix, Key& mask, int d, int sh, int nb) {
+    prefix |= ((u64)d) << sh;
+    mask |= ((u64)((1u << nb) - 1)) << sh;
+  }
+  static __device__ __forceinline__ bool greater(Key a, Key b) { return a > b; }
+  static __device__ __forceinline__ bool at_least(Key a, Key b) { return a >= b; }
+  static __device__ __forceinline__ int position(Key k) { return (int)(0xFFFFFFFFu - (unsigned)k); }
+  static __device__ __forceinline__ float image(float v) { return v; }
+};
+struct Key96 {
+  u64 hi;       // orderable(score)
+  unsigned lo;  // ~position
+};
+template <> struct TopnKey<double> {
+  typedef Key96 Key;
+  static constexpr int TOP_SHIFT = 85;  // digits at bits 85, 74, ..., 8 and the last 8 bits
+  static __device__ __forceinline__ Key make(double v, int q) { return Key96{orderable(v), 0xFFFFFFFFu - (unsigned)q}; }
+  static __device__ __forceinline__ int digit(const Key& k, int sh, int nb) {
+    const u64 w = sh >= 32 ? k.hi >> (sh - 32) : (k.hi << (32 - sh)) | (u64)(k.lo >> sh);
+    return (int)(w & ((1u << nb) - 1));
+  }
+  static __device__ __forceinline__ bool matches(const Key& k, const Key& prefix, const Key& mask) {
+    return (k.hi & mask.hi) == prefix.hi && (k.lo & mask.lo) == prefix.lo;
+  }
+  static __device__ __forceinline__ void fix_digit(Key& prefix, Key& mask, int d, int sh, int nb) {
+    const u64 m = (1u << nb) - 1;
+    if (sh >= 32) {
+      prefix.hi |= (u64)d << (sh - 32);
+      mask.hi |= m << (sh - 32);
+    } else {
+      prefix.hi |= (u64)d >> (32 - sh);
+      mask.hi |= m >> (32 - sh);
+      prefix.lo |= (unsigned)((u64)d << sh);
+      mask.lo |= (unsigned)(m << sh);
+    }
+  }
+  static __device__ __forceinline__ bool greater(const Key& a, const Key& b) {
+    return a.hi > b.hi || (a.hi == b.hi && a.lo > b.lo);
+  }
+  static __device__ __forceinline__ bool at_least(const Key& a, const Key& b) {
+    return a.hi > b.hi || (a.hi == b.hi && a.lo >= b.lo);
+  }
+  static __device__ __forceinline__ int position(const Key& k) { return (int)(0xFFFFFFFFu - k.lo); }
+  static __device__ __forceinline__ float image(double v) {
+    const float f = (float)v;
+    return isfinite(v) ? fminf(fmaxf(f, -FLT_MAX), FLT_MAX) : f;
+  }
+};
 
 // The `cutoff` best of the n scores L[0..n) of one row, best first (BaseRecommender.py:189-196); ties -> ascending
 // position.  Position q is item q, or items[q] when a (strictly ascending) item map is given, so that ties go to the
 // ascending item either way.  Called by all TOPN_THREADS threads of a CTA: MSB radix select of the cutoff-th key over
-// 64-bit keys (score bits, ~position), then the survivors are ranked by counting (cutoff is small: <= 1024).
+// the TopnKey keys (score bits, ~position), then the survivors are ranked by counting (cutoff is small: <= 1024).
 // out_items / out_scores: this row's `cutoff` slots; past the end of the row -1 / -inf.
 constexpr int TOPN_THREADS = 256;
 constexpr int TOPN_MAX = 1024;
+template <typename T>
 struct TopnSmem {
   int hist[2048];
   int digit, need, cnt;
-  u64 cand[TOPN_MAX];
+  typename TopnKey<T>::Key cand[TOPN_MAX];
 };
-__device__ __forceinline__ void topn_row(const float* L, int n, int cutoff, const int* items, int* out_items, float* out_scores,
-                                         TopnSmem& sm) {
+template <typename T>
+__device__ __forceinline__ void topn_row(const T* L, int n, int cutoff, const int* items, int* out_items, float* out_scores,
+                                         TopnSmem<T>& sm) {
+  typedef TopnKey<T> K;
   const int tid = threadIdx.x;
   const int keep = min(cutoff, n);
-  u64 prefix = 0, mask = 0;
+  typename K::Key prefix{}, mask{};
   int need = keep;
   if (keep < n) {
-    for (int shift = 53;; shift -= 11) {
+    for (int shift = K::TOP_SHIFT;; shift -= 11) {
       const int sh = max(shift, 0), nb = shift >= 0 ? 11 : 11 + shift;
       for (int i = tid; i < 2048; i += TOPN_THREADS) sm.hist[i] = 0;
       __syncthreads();
       for (int q = tid; q < n; q += TOPN_THREADS) {
-        const u64 key = (((u64)orderable(L[q])) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
-        if ((key & mask) == prefix) atomicAdd(&sm.hist[(int)((key >> sh) & ((1u << nb) - 1))], 1);
+        const typename K::Key key = K::make(L[q], q);
+        if (K::matches(key, prefix, mask)) atomicAdd(&sm.hist[K::digit(key, sh, nb)], 1);
       }
       __syncthreads();
       if (tid < 32) {
@@ -162,8 +238,7 @@ __device__ __forceinline__ void topn_row(const float* L, int n, int cutoff, cons
         }
       }
       __syncthreads();
-      prefix |= ((u64)sm.digit) << sh;
-      mask |= ((u64)((1u << nb) - 1)) << sh;
+      K::fix_digit(prefix, mask, sm.digit, sh, nb);
       need = sm.need;
       __syncthreads();
       if (shift <= 0) break;
@@ -172,27 +247,28 @@ __device__ __forceinline__ void topn_row(const float* L, int n, int cutoff, cons
   if (tid == 0) sm.cnt = 0;
   __syncthreads();
   for (int q = tid; q < n; q += TOPN_THREADS) {
-    const u64 key = (((u64)orderable(L[q])) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
-    if (key >= prefix) sm.cand[atomicAdd(&sm.cnt, 1)] = key;
+    const typename K::Key key = K::make(L[q], q);
+    if (K::at_least(key, prefix)) sm.cand[atomicAdd(&sm.cnt, 1)] = key;
   }
   __syncthreads();
   const int m = sm.cnt;  // == keep
   for (int t = tid; t < m; t += TOPN_THREADS) {
-    const u64 k = sm.cand[t];
+    const typename K::Key k = sm.cand[t];
     int rank = 0;
-    for (int q = 0; q < m; ++q) rank += sm.cand[q] > k;
-    const int q = (int)(0xFFFFFFFFu - (unsigned)k);
+    for (int q = 0; q < m; ++q) rank += K::greater(sm.cand[q], k);
+    const int q = K::position(k);
     out_items[rank] = items ? items[q] : q;
-    out_scores[rank] = L[q];
+    out_scores[rank] = K::image(L[q]);
   }
   for (int t = m + tid; t < cutoff; t += TOPN_THREADS) { out_items[t] = -1; out_scores[t] = -INFINITY; }
   __syncthreads();
 }
 
 // per row of a dense [n_rows, n_items] block the `cutoff` best items; one CTA per row
-__global__ void __launch_bounds__(TOPN_THREADS) topn_rows_kernel(const float* __restrict__ scores, int n_rows, int n_items,
+template <typename T>
+__global__ void __launch_bounds__(TOPN_THREADS) topn_rows_kernel(const T* __restrict__ scores, int n_rows, int n_items,
                                                                 int cutoff, int* out_items, float* out_scores) {
-  __shared__ TopnSmem sm;
+  __shared__ TopnSmem<T> sm;
   for (int row = blockIdx.x; row < n_rows; row += gridDim.x)
     topn_row(scores + (size_t)row * n_items, n_items, cutoff, nullptr, out_items + (size_t)row * cutoff,
              out_scores + (size_t)row * cutoff, sm);
@@ -378,7 +454,7 @@ __global__ void __launch_bounds__(TOPN_THREADS) cand_topn_cta_kernel(
     const int* __restrict__ users, int n_block, const int* __restrict__ cand_ptr, const int* __restrict__ cand_idx,
     float* scores, const int* __restrict__ seen_ptr, const int* __restrict__ seen_idx, const unsigned char* __restrict__ ignore,
     int cutoff, int* out_items, float* out_scores) {
-  __shared__ TopnSmem sm;
+  __shared__ TopnSmem<float> sm;
   for (int b = blockIdx.x; b < n_block; b += gridDim.x) {
     const int cs = cand_ptr[b], n = cand_ptr[b + 1] - cs;
     if (n <= CAND_WARP_LIST) continue;
@@ -395,6 +471,36 @@ __global__ void __launch_bounds__(TOPN_THREADS) cand_topn_cta_kernel(
     __syncthreads();
     topn_row(L, n, cutoff, items, out_items + (size_t)b * cutoff, out_scores + (size_t)b * cutoff, sm);
   }
+}
+
+// the bodies of b200_score_mask_device / b200_score_topn_device and their fp64 twins; `fn` names the entry point in errors
+template <typename T>
+void score_mask(const char* fn, const int32_t* d_users, int n_users_block, const int32_t* d_urm_ptr, const int32_t* d_urm_idx,
+                const unsigned char* d_items_keep, int n_items, T* d_scores, void* stream) {
+  B200_REQUIRE(d_scores && n_items > 0 && n_users_block >= 0, "%s: bad argument", fn);
+  if (n_users_block == 0) return;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d_items_keep) {
+    mask_items_kernel<<<div_up((long long)n_users_block * n_items, 256), 256, 0, st>>>(d_items_keep, n_users_block, n_items, d_scores);
+    count_launch();
+  }
+  if (d_users && d_urm_ptr && d_urm_idx) {
+    mask_seen_kernel<<<div_up((long long)n_users_block * 32, 256), 256, 0, st>>>(d_users, n_users_block, d_urm_ptr, d_urm_idx, n_items, d_scores);
+    count_launch();
+  }
+  B200_CUDA(cudaGetLastError());
+}
+
+template <typename T>
+void score_topn(const char* fn, const T* d_scores, int n_rows, int n_items, int cutoff, int32_t* d_items, float* d_item_scores,
+                void* stream) {
+  B200_REQUIRE(d_scores && d_items && d_item_scores, "%s: NULL argument", fn);
+  B200_REQUIRE(cutoff >= 1 && cutoff <= TOPN_MAX, "%s: cutoff must be in [1, %d]", fn, TOPN_MAX);
+  if (n_rows == 0) return;
+  topn_rows_kernel<<<std::min(n_rows, sm_count() * 8), TOPN_THREADS, 0, (cudaStream_t)stream>>>(d_scores, n_rows, n_items, cutoff,
+                                                                                                d_items, d_item_scores);
+  B200_CUDA(cudaGetLastError());
+  count_launch();
 }
 
 }  // namespace score
@@ -455,33 +561,24 @@ int b200_score_mf_device(const int32_t* d_users, int n_users_block, const float*
 
 int b200_score_mask_device(const int32_t* d_users, int n_users_block, const int32_t* d_urm_ptr, const int32_t* d_urm_idx,
                            const unsigned char* d_items_keep, int n_items, float* d_scores, void* stream) {
+  return guarded([&] { score_mask("b200_score_mask", d_users, n_users_block, d_urm_ptr, d_urm_idx, d_items_keep, n_items, d_scores, stream); });
+}
+
+int b200_score_mask_f64_device(const int32_t* d_users, int n_users_block, const int32_t* d_urm_ptr, const int32_t* d_urm_idx,
+                               const unsigned char* d_items_keep, int n_items, double* d_scores, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(d_scores && n_items > 0 && n_users_block >= 0, "b200_score_mask: bad argument");
-    if (n_users_block == 0) return;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (d_items_keep) {
-      mask_items_kernel<<<div_up((long long)n_users_block * n_items, 256), 256, 0, st>>>(d_items_keep, n_users_block, n_items, d_scores);
-      count_launch();
-    }
-    if (d_users && d_urm_ptr && d_urm_idx) {
-      mask_seen_kernel<<<div_up((long long)n_users_block * 32, 256), 256, 0, st>>>(d_users, n_users_block, d_urm_ptr, d_urm_idx, n_items, d_scores);
-      count_launch();
-    }
-    B200_CUDA(cudaGetLastError());
+    score_mask("b200_score_mask_f64", d_users, n_users_block, d_urm_ptr, d_urm_idx, d_items_keep, n_items, d_scores, stream);
   });
 }
 
 int b200_score_topn_device(const float* d_scores, int n_rows, int n_items, int cutoff, int32_t* d_items, float* d_item_scores,
                            void* stream) {
-  return guarded([&] {
-    B200_REQUIRE(d_scores && d_items && d_item_scores, "b200_score_topn: NULL argument");
-    B200_REQUIRE(cutoff >= 1 && cutoff <= TOPN_MAX, "b200_score_topn: cutoff must be in [1, %d]", TOPN_MAX);
-    if (n_rows == 0) return;
-    topn_rows_kernel<<<std::min(n_rows, sm_count() * 8), TOPN_THREADS, 0, (cudaStream_t)stream>>>(d_scores, n_rows, n_items, cutoff,
-                                                                                                  d_items, d_item_scores);
-    B200_CUDA(cudaGetLastError());
-    count_launch();
-  });
+  return guarded([&] { score_topn("b200_score_topn", d_scores, n_rows, n_items, cutoff, d_items, d_item_scores, stream); });
+}
+
+int b200_score_topn_f64_device(const double* d_scores, int n_rows, int n_items, int cutoff, int32_t* d_items,
+                               float* d_item_scores, void* stream) {
+  return guarded([&] { score_topn("b200_score_topn_f64", d_scores, n_rows, n_items, cutoff, d_items, d_item_scores, stream); });
 }
 
 int b200_cand_score_sparse_device(const int32_t* d_users, int n_block, const int32_t* d_a_ptr, const int32_t* d_a_idx,

@@ -16,6 +16,13 @@ With a `diversity_object` (metrics.py:719-775: any object with an `item_diversit
 below or the reference's own class) both evaluators add DIVERSITY_SIMILARITY, the 23rd metric: the top-left
 n_items x n_items block of the matrix is uploaded once per evaluator and device, and `b200_eval_diversity_device` reduces
 each block's lists next to the accumulate kernel.
+
+Any other recommender object -- the reference's own `BaseRecommender` subclasses, such as the neural wrappers or
+`GlobalEffects` -- is a *foreign* recommender.  It needs only the reference methods the reference evaluator calls:
+`_compute_item_score(user_id_array, items_to_compute=None)`, `get_URM_train()`, `set_items_to_ignore` and
+`reset_items_to_ignore`.  Its host score blocks are uploaded and ranked on the device (fp32 blocks on the fp32 top-N keys,
+fp64 blocks on 96-bit fp64 keys, csrc/score.cu) and go to the same accumulate kernel (see
+`EvaluatorHoldout.evaluateRecommender`).
 """
 import ctypes
 
@@ -23,6 +30,7 @@ import numpy as np
 import scipy.sparse as sps
 
 from . import _lib
+from .recommenders import BaseRecommender
 
 # order of Base/Evaluation/Evaluator.py:20-45
 METRIC_NAMES = ["PRECISION", "PRECISION_RECALL_MIN_DEN", "RECALL", "MAP", "MAP_MIN_DEN", "MRR", "NDCG", "F1", "HIT_RATE",
@@ -84,6 +92,22 @@ def _ideal_dcg(URM_test, cutoffs):
     for k, c in enumerate(cutoffs):
         out[:, k] = np.bincount(rows, weights=np.where(pos < c, terms, 0.0), minlength=n_users)
     return out
+
+
+def _foreign_scores(recommender_object, user_id_array, n_items, items_to_compute=None):
+    """One `_compute_item_score` call of a foreign recommender, as the reference's `recommend` makes it: the block as a
+    C-contiguous float32 or float64 array of shape (len(user_id_array), n_items).  Other real dtypes become float64."""
+    block = np.asarray(recommender_object._compute_item_score(user_id_array, items_to_compute=items_to_compute))
+    want = (len(user_id_array), n_items)
+    if block.shape != want:
+        raise ValueError("{}._compute_item_score returned a score block of shape {}, expected {} (users, n_items)".format(
+            type(recommender_object).__name__, block.shape, want))
+    if block.dtype.kind not in "biuf":
+        raise ValueError("{}._compute_item_score returned scores of dtype {}, expected real numbers".format(
+            type(recommender_object).__name__, block.dtype))
+    if block.dtype != np.float32 and block.dtype != np.float64:
+        block = np.asarray(block, np.float64)
+    return np.ascontiguousarray(block)
 
 
 class EvaluatorHoldout(object):
@@ -200,15 +224,78 @@ class EvaluatorHoldout(object):
             items, vals = recommender_object._topn_device(scores, cutoff)
             self._accumulate(st, d_users, items, vals, cutoff)
 
+    def _foreign_blocks(self, recommender_object, users, block_size):
+        """(users, host score block) of a foreign recommender: one call per block of users, items_to_compute=None (:426-437)."""
+        for b0 in range(0, len(users), block_size):
+            b_users = users[b0:b0 + block_size]
+            yield b_users, _foreign_scores(recommender_object, b_users, self.n_items)
+
+    def _evaluate_foreign(self, recommender_object, users, block_size, st, URM_train):
+        """Ranks every host score block of a foreign recommender on the device: upload, seen (the structure of its
+        URM_train) and ignored items to -inf, [B, max_cutoff] top-N table, accumulate.  Nothing here waits for the device,
+        so the GPU ranks block b while the model scores block b + 1 on the host."""
+        import torch
+        URM_train = sps.csr_matrix(URM_train)
+        if URM_train.shape[0] < self.n_users or URM_train.shape[1] != self.n_items:
+            raise ValueError("{}: get_URM_train() has shape {}, the test matrix {}".format(
+                self.EVALUATOR_NAME, URM_train.shape, self.URM_test.shape))
+        dev = st["ptr"].device
+        seen_ptr = seen_idx = keep = None
+        if self.exclude_seen:
+            seen_ptr, seen_idx = (torch.from_numpy(np.ascontiguousarray(a, np.int32)).to(dev)
+                                  for a in (URM_train.indptr, URM_train.indices))
+        if self.ignore_items_flag and len(self.ignore_items_ID):
+            k = np.ones(self.n_items, np.uint8)
+            k[self.ignore_items_ID] = 0
+            keep = torch.from_numpy(k).to(dev)
+        cutoff = int(min(self.max_cutoff, self.n_items))
+        rows = min(block_size, max(len(users), 1))
+        items = torch.empty((rows, cutoff), dtype=torch.int32, device=dev)
+        vals = torch.empty((rows, cutoff), dtype=torch.float32, device=dev)
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        for b_users, block in self._foreign_blocks(recommender_object, users, block_size):
+            nb = len(b_users)
+            # non_blocking: torch's blocking host-to-device copy synchronises the stream after the copy; a copy from pageable
+            # memory has still consumed the host array when the call returns
+            d_users = torch.from_numpy(np.ascontiguousarray(b_users, np.int32)).to(dev, non_blocking=True)
+            d_scores = torch.from_numpy(block).to(dev, non_blocking=True)
+            f64 = block.dtype == np.float64
+            if seen_ptr is not None or keep is not None:
+                mask = self._lib.b200_score_mask_f64_device if f64 else self._lib.b200_score_mask_device
+                _lib.check(mask(d_users.data_ptr() if seen_ptr is not None else None, nb,
+                                seen_ptr.data_ptr() if seen_ptr is not None else None,
+                                seen_idx.data_ptr() if seen_idx is not None else None,
+                                keep.data_ptr() if keep is not None else None, self.n_items, d_scores.data_ptr(), stream))
+            topn = self._lib.b200_score_topn_f64_device if f64 else self._lib.b200_score_topn_device
+            _lib.check(topn(d_scores.data_ptr(), nb, self.n_items, cutoff, items.data_ptr(), vals.data_ptr(), stream))
+            self._accumulate(st, d_users, items[:nb], vals[:nb], cutoff)
+
     def evaluateRecommender(self, recommender_object, block_size=None):
-        """Evaluator.py:240-288 + :413-461."""
+        """Evaluator.py:240-288 + :413-461.
+
+        `recommender_object` is one of this package's `BaseRecommender` mirrors, whose score blocks never leave the
+        device, or any foreign object with the reference's `_compute_item_score(user_id_array, items_to_compute=None)`,
+        `get_URM_train()`, `set_items_to_ignore` and `reset_items_to_ignore`.  A foreign object is called as the reference
+        evaluator calls it: `_compute_item_score` once per block of users here (consecutive int64 slices of
+        `users_to_evaluate`, items_to_compute=None), once per user in EvaluatorNegativeItemSample; `get_URM_train()` once.
+        Its block must be `np.asarray`-able to shape (len(user_id_array), n_items), else ValueError.  float32 blocks are
+        ranked in fp32 and float64 blocks in fp64; any other real dtype (ints, bool, float16) is converted with
+        `np.asarray(block, np.float64)`, which is exact except for int64 magnitudes above 2^53.  The seen items (the
+        structure of `sps.csr_matrix(get_URM_train())`, with exclude_seen) and the ignored items score -inf, and the
+        ranking is the package's own: np.lexsort((arange, -s)), ties to the ascending item, +inf first and NaN last, and
+        only the finite entries of the first max_cutoff positions are recommendations (DESIGN.md §6c).  The object's own
+        `recommend()` is not called (the reference's argpartition leaves its tie order unspecified)."""
         if self.ignore_items_flag:
             recommender_object.set_items_to_ignore(self.ignore_items_ID)
         users = np.asarray(self.users_to_evaluate, dtype=np.int64)
         if block_size is None:  # :422
             block_size = min([1000, int(4 * 1e9 * 8 / 64 / self.n_items), max(len(users), 1)])
-        st = self._device_state(recommender_object.get_URM_train())
-        self._evaluate_blocks(recommender_object, users, block_size, st)
+        URM_train = recommender_object.get_URM_train()
+        st = self._device_state(URM_train)
+        if isinstance(recommender_object, BaseRecommender):
+            self._evaluate_blocks(recommender_object, users, block_size, st)
+        else:
+            self._evaluate_foreign(recommender_object, users, block_size, st, URM_train)
         acc, rec, hit = st["acc"].cpu().numpy(), st["rec"].cpu().numpy().astype(np.float64), st["hit"].cpu().numpy().astype(np.float64)
         n_eval = len(users)
         results_dict = {}
@@ -288,6 +375,16 @@ class EvaluatorNegativeItemSample(EvaluatorHoldout):
     def _get_user_specific_items_to_compute(self, user_id):
         r = self.URM_items_to_rank
         return r.indices[r.indptr[user_id]:r.indptr[user_id + 1]]
+
+    def _foreign_blocks(self, recommender_object, users, block_size):
+        """A foreign recommender is called once per user with the user's sorted candidate row as items_to_compute (:553-571);
+        the rows are stacked into blocks of block_size users and each full row is ranked, so a non-candidate counts as
+        whatever score the model gave it, as in the reference's `recommend`."""
+        for b0 in range(0, len(users), block_size):
+            b_users = users[b0:b0 + block_size]
+            rows = [_foreign_scores(recommender_object, np.atleast_1d(u), self.n_items, self._get_user_specific_items_to_compute(u))
+                    for u in b_users]
+            yield b_users, rows[0] if len(rows) == 1 else np.concatenate(rows)
 
     def _cand_device(self, dev):
         """(users, candidate pointer, candidate items) on the device, uploaded once per evaluator."""
