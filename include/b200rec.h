@@ -167,6 +167,8 @@ enum b200_sampler { B200_SAMPLER_GLIBC = 0, /* host replay of srand(seed)/rand()
 /* URM: CSR, sorted indices (pyx:118-119).  h_user_factors / h_item_factors: the initial factors, row-major
  * [n_users x f] / [n_items x f] doubles -- the caller draws them exactly as pyx:177-178 does (numpy legacy RNG)
  * so that parity runs start from the reference's own initial point.  has_seed == 0 mirrors random_seed=None.
+ * The Philox sampler redraws a user until 0 < profile length < n_items (the reference's rule): B200_E_INVALID when no user
+ * qualifies, since no sample could ever be drawn (the glibc replay keeps the reference's endless loop).
  * hogwild != 0: no mini-batch barrier, every sample updates at once (batch_size is then only used for the
  * per-epoch sample count, pyx:586 / :292). */
 int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* h_indptr,
@@ -180,7 +182,8 @@ int b200_mf_destroy(b200_mf_t h);
 int b200_mf_epoch(b200_mf_t h, void* stream);
 /* multi-GPU data parallelism: this rank's device sampler draws users from [user_lo, user_hi) only (so user rows are
  * never shared between ranks) and an epoch consumes samples_per_epoch samples (0 = the reference's epoch length); stream_id (the rank)
- * selects a distinct Philox stream */
+ * selects a distinct Philox stream, derived from the handle's random_seed: calling this again with the same stream_id draws
+ * the same stream.  B200_E_INVALID when no user of the range has 0 < profile length < n_items. */
 int b200_mf_set_user_shard(b200_mf_t h, int user_lo, int user_hi, int64_t samples_per_epoch, uint32_t stream_id);
 int b200_mf_samples_last_epoch(b200_mf_t h, int64_t* n);
 /* the (user, item, neg item | rating) stream the last epoch consumed (for replaying it through the oracle) */
@@ -236,7 +239,8 @@ typedef struct b200_slim_s* b200_slim_t;
 
 /* URM_mask: CSR, sorted indices (pyx:100-119).  S starts at zero; the dense n_items^2 fp32 S is allocated by the first call
  * that needs it, so a handle that becomes a tree handle never holds one.  hogwild == 0: the batch-1 recursion in stream
- * order on one CTA (the reference's semantics); hogwild != 0: all SMs, atomics, no ordering between samples. */
+ * order on one CTA (the reference's semantics); hogwild != 0: all SMs, atomics, no ordering between samples.
+ * The Philox sampler (and b200_slim_create_sharded) return B200_E_INVALID when no user has 0 < profile length < n_items. */
 int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* h_indptr,
                      const int32_t* h_indices, float learning_rate, float li_reg, float lj_reg, int symmetric,
                      int sgd_mode, float gamma, float beta_1, float beta_2, int has_seed, uint32_t random_seed,

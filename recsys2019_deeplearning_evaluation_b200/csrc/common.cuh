@@ -119,4 +119,14 @@ struct GlibcRandHost {
 
 inline unsigned div_up(long long a, long long b) { return static_cast<unsigned>((a + b - 1) / b); }
 
+// Whether a user in [lo, hi) has 0 < profile length < n_items: the device samplers redraw the user until one does
+// (sampleBPR_Cython's acceptance rule), so a range without such a user would never finish a sample.
+inline bool has_sampleable_user(const int32_t* h_indptr, int64_t lo, int64_t hi, int64_t n_items) {
+  for (int64_t u = lo; u < hi; ++u) {
+    const int64_t n = (int64_t)h_indptr[u + 1] - h_indptr[u];
+    if (n > 0 && n < n_items) return true;
+  }
+  return false;
+}
+
 }  // namespace b200

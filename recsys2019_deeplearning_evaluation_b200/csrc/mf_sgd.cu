@@ -755,7 +755,8 @@ using namespace b200::mf;
 struct b200_mf_s {
   Params p{};
   int sampler = 0;  // 0 glibc replay on the host, 1 Philox on the device
-  unsigned seed = 1;
+  unsigned seed = 1;       // the Philox key of the draws
+  unsigned base_seed = 1;  // random_seed as created: b200_mf_set_user_shard derives `seed` from it
   unsigned epoch = 0;
   long long nnz = 0;
   float quota = 0.5f;
@@ -933,6 +934,8 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
     B200_REQUIRE(n_factors >= 1 && batch_size >= 1, "b200_mf_create: n_factors and batch_size must be >= 1");
     B200_REQUIRE(algorithm == MF_BPR || algorithm == FUNK_SVD, "b200_mf_create: unknown algorithm %d", algorithm);
     B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_mf_create: unknown sgd_mode %d", sgd_mode);
+    B200_REQUIRE(sampler == 0 || has_sampleable_user(h_indptr, 0, n_users, n_items),
+                 "b200_mf_create: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
     h = new b200_mf_s();
     Params& p = h->p;
     p.n_users = (int)n_users; p.n_items = (int)n_items; p.f = n_factors; p.batch_size = batch_size;
@@ -944,7 +947,7 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
     h->nnz = nnz;
     h->quota = negative_interactions_quota;
     h->sampler = sampler;
-    h->seed = has_seed ? random_seed : 1u;
+    h->seed = h->base_seed = has_seed ? random_seed : 1u;
     h->rng.seed(h->seed);
     if (const char* e = getenv("B200REC_GLIBC_HOST")) h->glibc_device = atoi(e) == 0;  // 1: the sequential host replay (A/B, tests)
     h->h_indptr.assign(h_indptr, h_indptr + n_users + 1);
@@ -1140,10 +1143,12 @@ int b200_mf_set_user_shard(b200_mf_t h, int user_lo, int user_hi, int64_t sample
     B200_REQUIRE(h->sampler != 0, "b200_mf_set_user_shard: only the device (Philox) sampler can be sharded");
     B200_REQUIRE(0 <= user_lo && user_lo < user_hi && user_hi <= h->p.n_users, "b200_mf_set_user_shard: bad range [%d,%d)", user_lo, user_hi);
     B200_REQUIRE(samples_per_epoch >= 0 && samples_per_epoch <= h->cap_samples, "b200_mf_set_user_shard: samples_per_epoch out of range");
+    B200_REQUIRE(has_sampleable_user(h->h_indptr.data(), user_lo, user_hi, h->p.n_items),
+                 "b200_mf_set_user_shard: no user of [%d,%d) has 0 < profile length < n_items", user_lo, user_hi);
     h->shard_lo = user_lo;
     h->shard_hi = user_hi;
     h->epoch_samples_override = samples_per_epoch;
-    h->seed += 0x9E3779B9u * stream_id;  // decorrelates the ranks' Philox streams
+    h->seed = h->base_seed + 0x9E3779B9u * stream_id;  // decorrelates the ranks' Philox streams; a repeated call does not compound
     h->hog_blocks = 6;  // 1536 of an SM's 2048 threads: the all-reduce kernels of the overlapped exchange fit beside it
   });
 }

@@ -804,6 +804,8 @@ int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t
     B200_REQUIRE(out && h_indptr && (nnz == 0 || h_indices), "b200_slim_create: NULL argument");
     B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_slim_create: bad shape");
     B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_slim_create: unknown sgd_mode %d", sgd_mode);
+    B200_REQUIRE(sampler == 0 || has_sampleable_user(h_indptr, 0, n_users, n_items),
+                 "b200_slim_create: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
     h = new b200_slim_s();
     Params& p = h->p;
     p.n_users = (int)n_users; p.n_items = (int)n_items; p.symmetric = symmetric != 0; p.sgd_mode = sgd_mode;
@@ -851,6 +853,8 @@ int b200_slim_create_sharded(b200_slim_t* out, int64_t n_users, int64_t n_items,
     B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_slim_create_sharded: bad shape");
     B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_slim_create_sharded: unknown sgd_mode %d", sgd_mode);
     B200_REQUIRE(0 <= col_lo && col_lo < col_hi && col_hi <= n_items, "b200_slim_create_sharded: bad column range [%d,%d)", col_lo, col_hi);
+    B200_REQUIRE(has_sampleable_user(h_indptr, 0, n_users, n_items),
+                 "b200_slim_create_sharded: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
     h = new b200_slim_s();
     Params& p = h->p;
     p.n_users = (int)n_users; p.n_items = (int)n_items; p.symmetric = 0; p.sgd_mode = sgd_mode;

@@ -689,9 +689,13 @@ class EASE_R_Recommender(BaseItemSimilarityMatrixRecommender):
 
     def _gram_device(self, rows=None):
         """X^T X (EASE_R_Recommender.py:55-56) as a dense [n_items, n_items] fp32 CUDA tensor, from all users or from the
-        user rows [rows[0], rows[1]) only (the partial Gram of one rank, dist.make_sharded_ease)."""
+        user rows [rows[0], rows[1]) only (the partial Gram of one rank, dist.make_sharded_ease).  An empty row range (which
+        balanced_ranges gives a rank when a few users carry most of the interactions) contributes a zero matrix."""
+        import torch
         from .similarity import Compute_Similarity_Cython
         n = self.n_items
+        if rows is not None and rows[1] <= rows[0]:
+            return torch.zeros((n, n), dtype=torch.float32, device=torch.device("cuda", torch.cuda.current_device()))
         X = self.URM_train if rows is None else self.URM_train[rows[0]:rows[1]]
         sim = Compute_Similarity_Cython(X, shrink=0, topK=n if n > 2048 else 0, normalize=False, similarity="cosine")
         G = sim.compute_dense_device(0, n)  # symmetric: orientation is irrelevant
