@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "sampler.cuh"
 
 namespace b200 {
 namespace asy {
@@ -252,8 +253,9 @@ struct b200_asysvd_s {
   Params p{};
   double quota = 0.0;
   GlibcRandHost rng;
-  std::vector<int> h_indptr, h_indices, hs_u, hs_i;
-  std::vector<float> h_data, hs_r;
+  std::vector<int> h_indptr, h_indices;
+  std::vector<float> h_data;
+  HostSamples hs;
   DevBuf<int> d_indptr, d_indices, su, si;
   DevBuf<float> sr, Y, X, bu, bi, mu, cY, cX, cbu, cbi, cmu, m2Y, m2X, m2bu, m2bi, m2mu;
   DevBuf<double> pow_out;
@@ -365,36 +367,10 @@ int b200_asysvd_epoch(b200_asysvd_t h, void* stream) {
     const long long n = (long long)h->h_indices.size() + 1;
     p.n_samples = n;
     p.prof = getenv("B200REC_ASY_PROF") != nullptr;
-    h->hs_u.resize((size_t)n); h->hs_i.resize((size_t)n); h->hs_r.resize((size_t)n);
-    const int* indptr = h->h_indptr.data();
-    const int* indices = h->h_indices.data();
-    for (long long g = 0; g < n; ++g) {  // sampleMSE_Cython pyx:881-938, draw for draw
-      long u = 0, start = 0, len = 0;
-      while (len == 0 || len == p.n_items) {
-        u = h->rng.next() % p.n_users;
-        start = indptr[u];
-        len = indptr[u + 1] - start;
-      }
-      bool positive = true;
-      if (h->quota != 0.0) positive = (double)h->rng.next() <= h->quota * 2147483647.0;  // pyx:901
-      long item;
-      float rating = 0.f;
-      if (positive) {
-        const long idx = h->rng.next() % len;
-        item = indices[start + idx];
-        rating = h->h_data[(size_t)(start + idx)];
-      } else {
-        for (;;) {
-          item = h->rng.next() % p.n_items;
-          const int* lo = std::lower_bound(indices + start, indices + start + len, (int)item);
-          if (lo == indices + start + len || *lo != item) break;
-        }
-      }
-      h->hs_u[(size_t)g] = (int)u; h->hs_i[(size_t)g] = (int)item; h->hs_r[(size_t)g] = rating;
-    }
-    B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs_u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs_i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs_r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
+    h->hs.draw(h->rng, h->h_indptr.data(), h->h_indices.data(), h->h_data.data(), p.n_users, p.n_items, false, h->quota, n);
+    B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs.u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs.r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaEventRecord(h->ev0, st));
     const size_t smem = (size_t)(WARPS + 2) * (size_t)p.fp * sizeof(float);
     // per launch: the attribute belongs to the function, and handles with other factor counts share it
@@ -415,9 +391,9 @@ int b200_asysvd_epoch(b200_asysvd_t h, void* stream) {
 int b200_asysvd_get_samples(b200_asysvd_t h, int32_t* u, int32_t* i, float* r) {
   return guarded([&] {
     B200_REQUIRE(h && u && i && r && h->n_last > 0, "b200_asysvd_get_samples: NULL argument or no epoch run yet");
-    std::copy(h->hs_u.begin(), h->hs_u.end(), u);
-    std::copy(h->hs_i.begin(), h->hs_i.end(), i);
-    std::copy(h->hs_r.begin(), h->hs_r.end(), r);
+    std::copy(h->hs.u.begin(), h->hs.u.end(), u);
+    std::copy(h->hs.i.begin(), h->hs.i.end(), i);
+    std::copy(h->hs.r.begin(), h->hs.r.end(), r);
   });
 }
 

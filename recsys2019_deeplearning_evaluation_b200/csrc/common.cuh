@@ -89,44 +89,6 @@ inline int sm_count() {
   return n;
 }
 
-// Host-side replay of glibc's srand(seed) / rand() (TYPE_3 additive-feedback generator; the reference's samplers call libc's
-// rand(), SLIM_BPR_Cython_Epoch.pyx:436-480, MatrixFactorization_Cython_Epoch.pyx:881-987): next() is rand().
-struct GlibcRandHost {
-  int32_t r[31];
-  int f = 3, b = 0;
-  void seed(unsigned s) {
-    int32_t word = s == 0 ? 1 : (int32_t)s;
-    r[0] = word;
-    for (int i = 1; i < 31; ++i) {
-      const long hi = word / 127773, lo = word % 127773;
-      long w = 16807 * lo - 2836 * hi;
-      if (w < 0) w += 2147483647;
-      word = (int32_t)w;
-      r[i] = word;
-    }
-    f = 3; b = 0;
-    for (int i = 0; i < 310; ++i) raw();
-  }
-  uint32_t raw() {
-    const uint32_t v = (uint32_t)r[f] + (uint32_t)r[b];
-    r[f] = (int32_t)v;
-    f = (f + 1) % 31;
-    b = (b + 1) % 31;
-    return v;
-  }
-  int next() { return (int)(raw() >> 1); }
-};
-
 inline unsigned div_up(long long a, long long b) { return static_cast<unsigned>((a + b - 1) / b); }
-
-// Whether a user in [lo, hi) has 0 < profile length < n_items: the device samplers redraw the user until one does
-// (sampleBPR_Cython's acceptance rule), so a range without such a user would never finish a sample.
-inline bool has_sampleable_user(const int32_t* h_indptr, int64_t lo, int64_t hi, int64_t n_items) {
-  for (int64_t u = lo; u < hi; ++u) {
-    const int64_t n = (int64_t)h_indptr[u + 1] - h_indptr[u];
-    if (n > 0 && n < n_items) return true;
-  }
-  return false;
-}
 
 }  // namespace b200

@@ -32,6 +32,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "sampler.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -569,67 +570,18 @@ __global__ void mf_deps_kernel(const unsigned long long* __restrict__ keys, cons
   }
 }
 
-// ---- device sampler: Philox4x32-10, counter = (sample index, draw block), key = (seed, epoch)
-__device__ __forceinline__ void philox_round(unsigned& c0, unsigned& c1, unsigned& c2, unsigned& c3, unsigned k0, unsigned k1) {
-  const unsigned hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-  const unsigned hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-  c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
-}
-__device__ __forceinline__ uint4 philox(unsigned long long idx, unsigned blk, unsigned seed, unsigned epoch) {
-  unsigned c0 = (unsigned)idx, c1 = (unsigned)(idx >> 32), c2 = blk, c3 = 0x9E3779B9u;
-  unsigned k0 = seed, k1 = epoch;
-#pragma unroll
-  for (int r = 0; r < 10; ++r) { philox_round(c0, c1, c2, c3, k0, k1); k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
-  return make_uint4(c0, c1, c2, c3);
-}
-
-struct Draws {
-  unsigned long long idx; unsigned seed, epoch, blk; uint4 cur; int pos;
-  __device__ Draws(unsigned long long i, unsigned s, unsigned e) : idx(i), seed(s), epoch(e), blk(0), pos(4) {}
-  __device__ unsigned next() {
-    if (pos == 4) { cur = philox(idx, blk++, seed, epoch); pos = 0; }
-    const unsigned v = pos == 0 ? cur.x : (pos == 1 ? cur.y : (pos == 2 ? cur.z : cur.w));
-    ++pos;
-    return v;
-  }
-};
-
-// same acceptance rules as sampleBPR_Cython / sampleMSE_Cython (users with 0 < profile < n_items; negative item
-// not in the sorted profile, binary search instead of the linear scan), different random stream
+// Philox stream of the user shard [user_lo, user_lo + n_users) (sampler.cuh)
 __global__ void mf_sample_kernel(const int* __restrict__ indptr, const int* __restrict__ indices, const float* __restrict__ data,
                                  int user_lo, int n_users, int n_items, int algorithm, float quota, long long n_samples, unsigned seed,
                                  unsigned epoch, int* su, int* si, int* sj, float* sr) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= n_samples) return;
-  Draws d((unsigned long long)g, seed, epoch);
-  int u, s, n;
-  do {
-    u = user_lo + (int)(d.next() % (unsigned)n_users);  // n_users = size of this rank's user shard
-    s = indptr[u];
-    n = indptr[u + 1] - s;
-  } while (n == 0 || n == n_items);
-  bool positive = true;
-  if (algorithm == FUNK_SVD && quota != 0.f) positive = (float)(d.next() >> 8) * (1.f / 16777216.f) <= quota;
-  int item;
-  float r = 0.f;
-  if (algorithm == MF_BPR || positive) {
-    const int k = (int)(d.next() % (unsigned)n);
-    item = indices[s + k];
-    if (algorithm == FUNK_SVD) r = data[s + k];
-  }
-  if (algorithm == MF_BPR || !positive) {
-    int neg;
-    while (true) {
-      neg = (int)(d.next() % (unsigned)n_items);
-      int lo = 0, hi = n;
-      while (lo < hi) { const int mid = (lo + hi) >> 1; if (indices[s + mid] < neg) lo = mid + 1; else hi = mid; }
-      if (lo == n || indices[s + lo] != neg) break;
-    }
-    if (algorithm == MF_BPR) sj[g] = neg; else { item = neg; r = 0.f; }
-  }
-  su[g] = u;
-  si[g] = item;
-  if (algorithm == FUNK_SVD) sr[g] = r;
+  PhiloxDraws d{(unsigned long long)g, seed, epoch, 0x9E3779B9u};
+  Sample s;
+  draw_sample(d, indptr, indices, data, user_lo, n_users, n_items, algorithm == MF_BPR, quota, s);
+  su[g] = s.u;
+  si[g] = s.i;
+  if (algorithm == MF_BPR) sj[g] = s.j; else sr[g] = s.r;
 }
 
 
@@ -651,50 +603,18 @@ struct GlibcView {
 };
 
 // the sample starting at raw position p: returns the position after its last draw (> R when the buffer ran out)
-__device__ __forceinline__ int glibc_sample_at(const GlibcView& v, int p, int* u_out, int* i_out, int* j_out, float* r_out) {
-  int q = p;
-  int u = 0, s = 0, n = 0;
-  for (;;) {  // pyx:952-960 / :890-898: users with an empty or a full profile are redrawn
-    if (q >= v.R) return v.R + 1;
-    u = v.raw[q++] % v.n_users;
-    s = v.indptr[u];
-    n = v.indptr[u + 1] - s;
-    if (n != 0 && n != v.n_items) break;
-  }
-  bool positive = true;
-  if (v.algorithm == FUNK_SVD && v.quota != 0.f) {  // pyx:901
-    if (q >= v.R) return v.R + 1;
-    positive = (double)v.raw[q++] <= (double)v.quota * 2147483647.0;
-  }
-  int item = -1;
-  float r = 0.f;
-  if (v.algorithm == MF_BPR || positive) {
-    if (q >= v.R) return v.R + 1;
-    const int k = v.raw[q++] % n;
-    item = v.indices[s + k];
-    if (v.algorithm == FUNK_SVD) r = v.data[s + k];
-  }
-  if (v.algorithm == MF_BPR || !positive) {
-    int neg;
-    for (;;) {
-      if (q >= v.R) return v.R + 1;
-      neg = v.raw[q++] % v.n_items;
-      int lo = 0, hi = n;
-      while (lo < hi) { const int mid = (lo + hi) >> 1; if (v.indices[s + mid] < neg) lo = mid + 1; else hi = mid; }
-      if (lo == n || v.indices[s + lo] != neg) break;
-    }
-    if (v.algorithm == MF_BPR) { if (j_out) *j_out = neg; } else { item = neg; r = 0.f; }
-  }
-  if (u_out) *u_out = u;
-  if (i_out) *i_out = item;
-  if (r_out) *r_out = r;
-  return q;
+__device__ __forceinline__ int glibc_sample_at(const GlibcView& v, int p, Sample* out) {
+  GlibcReplay d{v.raw, p, v.R};
+  Sample s{};
+  if (!draw_sample(d, v.indptr, v.indices, v.data, 0, v.n_users, v.n_items, v.algorithm == MF_BPR, v.quota, s)) return v.R + 1;
+  if (out) *out = s;
+  return d.q;
 }
 
 __global__ void glibc_len_kernel(const GlibcView v, int* __restrict__ nxt) {  // nxt[p] = start of the following sample; nxt[R] = R
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p > v.R) return;
-  nxt[p] = p == v.R ? v.R : min(glibc_sample_at(v, p, nullptr, nullptr, nullptr, nullptr), v.R);
+  nxt[p] = p == v.R ? v.R : min(glibc_sample_at(v, p, nullptr), v.R);
 }
 
 __global__ void glibc_double_kernel(const int* __restrict__ jk, int R, int* __restrict__ jk1) {
@@ -710,41 +630,13 @@ __global__ void glibc_emit_kernel(const GlibcView v, const int* __restrict__ tab
   int p = 0;
   for (int k = 0; k < levels; ++k)
     if ((g >> k) & 1) p = tables[(size_t)k * (v.R + 1) + p];
-  int u = 0, i = 0, j = 0;
-  float r = 0.f;
-  const int q = p < v.R ? glibc_sample_at(v, p, &u, &i, &j, &r) : v.R + 1;
-  su[g] = u; si[g] = i;
-  if (v.algorithm == MF_BPR) sj[g] = j; else sr[g] = r;
+  Sample s{};
+  const int q = p < v.R ? glibc_sample_at(v, p, &s) : v.R + 1;
+  su[g] = s.u; si[g] = s.i;
+  if (v.algorithm == MF_BPR) sj[g] = s.j; else sr[g] = s.r;
   if (q > v.R) atomicMax(consumed, 0x7FFFFFFF);  // the buffer ran out somewhere: the host extends it and repeats
   else if (g == n_samples - 1) atomicMax(consumed, q);
 }
-
-// host replay of glibc srand()/rand() (TYPE_3 additive feedback, r[i] = r[i-31] + r[i-3], 310 discarded, >> 1)
-struct GlibcRand {
-  int32_t r[31];
-  int f = 3, b = 0;
-  void seed(unsigned s) {
-    int32_t word = s == 0 ? 1 : (int32_t)s;
-    r[0] = word;
-    for (int i = 1; i < 31; ++i) {
-      const long hi = word / 127773, lo = word % 127773;
-      long w = 16807 * lo - 2836 * hi;
-      if (w < 0) w += 2147483647;
-      word = (int32_t)w;
-      r[i] = word;
-    }
-    f = 3; b = 0;
-    for (int i = 0; i < 310; ++i) next_raw();
-  }
-  uint32_t next_raw() {
-    const uint32_t v = (uint32_t)r[f] + (uint32_t)r[b];
-    r[f] = (int32_t)v;
-    if (++f == 31) f = 0;
-    if (++b == 31) b = 0;
-    return v;
-  }
-  int next() { return (int)(next_raw() >> 1); }
-};
 
 }  // namespace mf
 }  // namespace b200
@@ -760,7 +652,7 @@ struct b200_mf_s {
   unsigned epoch = 0;
   long long nnz = 0;
   float quota = 0.5f;
-  GlibcRand rng;
+  GlibcRandHost rng;
   std::vector<int> h_indptr, h_indices;
   std::vector<float> h_data;
   DevBuf<int> d_indptr, d_indices;
@@ -776,8 +668,7 @@ struct b200_mf_s {
   DevBuf<int> flagI, flagU, listI, listU, cnt, su, si, sj;
   DevBuf<float> sr;
   DevBuf<double> pow_out;
-  std::vector<int> hs_u, hs_i, hs_j;
-  std::vector<float> hs_r;
+  HostSamples hs;  // the host replay's samples (B200REC_GLIBC_HOST=1, or a stream too long for the device replay)
   long long samples_last = 0, cap_samples = 0, epoch_samples_override = 0;
   int shard_lo = 0, shard_hi = 0;  // device sampler draws users from [shard_lo, shard_hi) when set (multi-GPU user sharding)
   int grid = 0;
@@ -826,45 +717,6 @@ long long epoch_batches(const b200_mf_s* h) {
   // pyx:586 (BPR: n_users / batch_size + 1) and pyx:292 (FunkSVD: nnz / batch_size + 1)
   return (h->p.algorithm == MF_BPR ? (long long)h->p.n_users : h->nnz) / h->p.batch_size + 1;
 }
-
-void host_samples(b200_mf_s* h, long long n) {
-  // sampleBPR_Cython pyx:943-987 / sampleMSE_Cython pyx:881-938, draw for draw
-  h->hs_u.resize((size_t)n); h->hs_i.resize((size_t)n);
-  if (h->p.algorithm == MF_BPR) h->hs_j.resize((size_t)n); else h->hs_r.resize((size_t)n);
-  const int* indptr = h->h_indptr.data();
-  const int* indices = h->h_indices.data();
-  const int nU = h->p.n_users, nI = h->p.n_items;
-  for (long long g = 0; g < n; ++g) {
-    long u = 0, start = 0, len = 0;
-    while (len == 0 || len == nI) {
-      u = h->rng.next() % nU;
-      start = indptr[u];
-      len = indptr[u + 1] - start;
-    }
-    bool positive = true;
-    if (h->p.algorithm == FUNK_SVD && h->quota != 0.0f) positive = h->rng.next() <= (double)h->quota * 2147483647.0;
-    long item = -1;
-    float r = 0.f;
-    if (h->p.algorithm == MF_BPR || positive) {
-      const long k = h->rng.next() % len;
-      item = indices[start + k];
-      if (h->p.algorithm == FUNK_SVD) r = h->h_data[(size_t)(start + k)];
-    }
-    if (h->p.algorithm == MF_BPR || !positive) {
-      long neg;
-      for (;;) {
-        neg = h->rng.next() % nI;
-        const int* lo = std::lower_bound(indices + start, indices + start + len, (int)neg);
-        if (lo == indices + start + len || *lo != neg) break;
-      }
-      if (h->p.algorithm == MF_BPR) h->hs_j[(size_t)g] = (int)neg; else { item = neg; r = 0.f; }
-    }
-    h->hs_u[(size_t)g] = (int)u;
-    h->hs_i[(size_t)g] = (int)item;
-    if (h->p.algorithm == FUNK_SVD) h->hs_r[(size_t)g] = r;
-  }
-}
-
 
 // The epoch's n samples from the glibc stream, resolved on the device (see glibc_len_kernel).  Synchronises the stream once
 // (the host must know how many draws were consumed before it can continue the stream).
@@ -1060,11 +912,11 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
     if (h->sampler == 0 && h->glibc_device && n * 4 + 65536 < (1ll << 30)) {
       glibc_device_samples(h, n, st);
     } else if (h->sampler == 0) {
-      host_samples(h, n);
-      B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs_u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs_i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      if (p.algorithm == MF_BPR) B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs_j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      else B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs_r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
+      h->hs.draw(h->rng, h->h_indptr.data(), h->h_indices.data(), h->h_data.data(), p.n_users, p.n_items, p.algorithm == MF_BPR, h->quota, n);
+      B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs.u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+      B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+      if (p.algorithm == MF_BPR) B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs.j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+      else B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs.r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
     }
     B200_CUDA(cudaEventRecord(h->ev0, st));
     if (h->sampler != 0) {

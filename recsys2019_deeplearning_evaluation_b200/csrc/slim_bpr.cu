@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "sampler.cuh"
 
 namespace b200 {
 namespace slim {
@@ -585,51 +586,16 @@ __global__ void slim_full_kernel(const float* __restrict__ S, int n, int symmetr
   out[g] = v;
 }
 
-// device Philox sampler (same acceptance rules as sampleBPR_Cython, pyx:436-480)
-__device__ __forceinline__ void philox_round(unsigned& c0, unsigned& c1, unsigned& c2, unsigned& c3, unsigned k0, unsigned k1) {
-  const unsigned hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-  const unsigned hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-  c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
-}
-__device__ __forceinline__ uint4 philox(unsigned long long idx, unsigned blk, unsigned seed, unsigned epoch) {
-  unsigned c0 = (unsigned)idx, c1 = (unsigned)(idx >> 32), c2 = blk, c3 = 0x243F6A88u;
-  unsigned k0 = seed, k1 = epoch;
-#pragma unroll
-  for (int r = 0; r < 10; ++r) { philox_round(c0, c1, c2, c3, k0, k1); k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
-  return make_uint4(c0, c1, c2, c3);
-}
-
+// Philox stream of the epoch (sampler.cuh)
 __global__ void slim_sample_kernel(const int* __restrict__ indptr, const int* __restrict__ indices, int n_users, int n_items,
                                    long long n_samples, unsigned seed, unsigned epoch, int* su, int* si, int* sj) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= n_samples) return;
-  unsigned blk = 0;
-  uint4 cur = philox((unsigned long long)g, blk++, seed, epoch);
-  int pos = 0;
-  auto next = [&]() {
-    if (pos == 4) { cur = philox((unsigned long long)g, blk++, seed, epoch); pos = 0; }
-    const unsigned v = pos == 0 ? cur.x : (pos == 1 ? cur.y : (pos == 2 ? cur.z : cur.w));
-    ++pos;
-    return v;
-  };
-  int u, s, n;
-  do {
-    u = (int)(next() % (unsigned)n_users);
-    s = indptr[u];
-    n = indptr[u + 1] - s;
-  } while (n == 0 || n == n_items);
-  const int item = indices[s + (int)(next() % (unsigned)n)];
-  int neg;
-  while (true) {
-    neg = (int)(next() % (unsigned)n_items);
-    int lo = 0, hi = n;
-    while (lo < hi) { const int mid = (lo + hi) >> 1; if (indices[s + mid] < neg) lo = mid + 1; else hi = mid; }
-    if (lo == n || indices[s + lo] != neg) break;
-  }
-  su[g] = u; si[g] = item; sj[g] = neg;
+  PhiloxDraws d{(unsigned long long)g, seed, epoch, 0x243F6A88u};
+  Sample s;
+  draw_sample(d, indptr, indices, nullptr, 0, n_users, n_items, true, 0.0, s);
+  su[g] = s.u; si[g] = s.i; sj[g] = s.j;
 }
-
-using GlibcRand = GlibcRandHost;  // common.cuh
 
 // grows a scratch buffer to at least `count` elements (contents are not kept)
 template <typename T>
@@ -717,8 +683,9 @@ struct b200_slim_s {
   Params p{};
   int sampler = 0, hogwild = 0;
   unsigned seed = 1, epoch = 0;
-  GlibcRand rng;
-  std::vector<int> h_indptr, h_indices, hs_u, hs_i, hs_j;
+  GlibcRandHost rng;
+  std::vector<int> h_indptr, h_indices;
+  HostSamples hs;
   DevBuf<int> d_indptr, d_indices, su, si, sj;
   DevBuf<float> S, c, m1, m2;
   DevBuf<double> pow_out;
@@ -962,28 +929,10 @@ int b200_slim_epoch(b200_slim_t h, void* stream) {
     p.n_samples = n;
     p.prof = getenv("B200REC_SLIM_PROF") != nullptr;
     if (h->sampler == 0) {
-      h->hs_u.resize((size_t)n); h->hs_i.resize((size_t)n); h->hs_j.resize((size_t)n);
-      const int* indptr = h->h_indptr.data();
-      const int* indices = h->h_indices.data();
-      for (long long g = 0; g < n; ++g) {  // sampleBPR_Cython pyx:436-480, draw for draw
-        long u = 0, start = 0, len = 0;
-        while (len == 0 || len == p.n_items) {
-          u = h->rng.next() % p.n_users;
-          start = indptr[u];
-          len = indptr[u + 1] - start;
-        }
-        const long item = indices[start + h->rng.next() % len];
-        long neg;
-        for (;;) {
-          neg = h->rng.next() % p.n_items;
-          const int* lo = std::lower_bound(indices + start, indices + start + len, (int)neg);
-          if (lo == indices + start + len || *lo != neg) break;
-        }
-        h->hs_u[(size_t)g] = (int)u; h->hs_i[(size_t)g] = (int)item; h->hs_j[(size_t)g] = (int)neg;
-      }
-      B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs_u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs_i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs_j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+      h->hs.draw(h->rng, h->h_indptr.data(), h->h_indices.data(), nullptr, p.n_users, p.n_items, true, 0.0, n);
+      B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs.u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+      B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+      B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs.j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
     }
     B200_CUDA(cudaEventRecord(h->ev0, st));
     if (h->sampler != 0) {

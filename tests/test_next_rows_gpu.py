@@ -115,6 +115,7 @@ def test_asysvd_matches_the_oracle_on_the_glibc_stream(n):
     X = asy_urm()
     g = _mf()(X, **common, **kw)
     o = MFOracle(X, record=2 * (X.nnz + 1), **common, **kw)
+    dense = sps.csr_matrix(X, dtype=np.float32).toarray()
     for e in range(2):
         g.epochIteration_Cython()
         o.epochIteration_Cython()
@@ -122,6 +123,7 @@ def test_asysvd_matches_the_oracle_on_the_glibc_stream(n):
         ou, oi, _ = o.recorded()
         assert len(u) == X.nnz + 1                                     # pyx:402
         assert np.array_equal(u, ou[e * len(u):(e + 1) * len(u)]) and np.array_equal(i, oi[e * len(u):(e + 1) * len(u)])
+        assert np.array_equal(r, dense[u, i])  # the oracle records u and i: r is the rating of a positive, 0 for a negative
     assert g.get_USER_factors().shape == (X.shape[1], 8)               # Y: one row per ITEM (pyx:163-166)
     names = ("get_USER_factors", "get_ITEM_factors") + (("get_USER_bias", "get_ITEM_bias", "get_GLOBAL_bias") if kw["use_bias"] else ())
     for name in names:
