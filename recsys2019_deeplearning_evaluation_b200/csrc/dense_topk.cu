@@ -7,7 +7,7 @@
 //     largest over ALL cells, zeros then dropped (zeros outrank negatives)            -> mode B200_TOPK_ZEROS_OUTRANK
 //   * SLIM_ElasticNet/SLIMElasticNetRecommender.py:99-107 -- per item, the min(nnz - 1, k) largest of the non-zero
 //     coefficients: a line with <= k non-zeros loses its smallest one                  -> mode 2
-// One CTA per line; the line is streamed from HBM/L2 once per radix pass (11-bit digits over the 64-bit key
+// One CTA per line; the line is streamed from HBM/L2 once per radix pass (select.cuh, 11-bit digits over the 64-bit key
 // value-bits << 32 | ~index, so ties resolve to the ascending index); survivors are written as a [lines, K] table.
 // NaN is a non-zero cell and ranks where the reference's numpy call puts it: above +inf in mode 0 (argsort ascending,
 // last k), below -inf in modes 1 and 2 (argpartition of the negated line). A line never emits more than K entries:
@@ -16,6 +16,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "select.cuh"
 
 namespace b200 {
 namespace dtk {
@@ -24,13 +25,6 @@ typedef unsigned long long u64;
 constexpr int THREADS = 256;
 constexpr int BINS = 2048;
 
-__device__ __forceinline__ unsigned orderable(float v) {
-  const unsigned b = __float_as_uint(v);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float from_orderable(unsigned o) {
-  return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
-}
 // orderable() maps +NaN above +inf and -NaN below -inf; every NaN is moved to one end instead, by mode
 __device__ __forceinline__ u64 line_key(float v, int qi, bool nan_high) {
   const unsigned o = v != v ? (nan_high ? 0xFFFFFFFFu : 0u) : orderable(v);
@@ -38,14 +32,15 @@ __device__ __forceinline__ u64 line_key(float v, int qi, bool nan_high) {
 }
 
 // SPARSE: line l is the segment [ptr[l], ptr[l+1]) of (sidx, M); its cells are the stored entries and the implicit
-// zeros of a length-n_inner line.
+// zeros of a length-n_inner line.  Residency: 8 CTAs per SM for compressed lines (32 registers: the grid of sm_count * 8
+// is resident at once), 6 for dense ones (40 registers).
 template <bool SPARSE>
-__global__ void __launch_bounds__(THREADS) topk_lines_kernel(const float* __restrict__ M, const int* __restrict__ ptr,
-                                                             const int* __restrict__ sidx, int n_lines, int n_inner_dense,
-                                                             long long stride_line, long long stride_inner, int K, int mode,
-                                                             int* out_idx, float* out_val, int* out_cnt, int idx_off = 0) {
-  __shared__ int hist[BINS];
-  __shared__ int s_digit, s_need, s_cnt, s_tie, s_npos, s_nneg, s_nnan;
+__global__ void __launch_bounds__(THREADS, SPARSE ? 8 : 6)
+    topk_lines_kernel(const float* __restrict__ M, const int* __restrict__ ptr, const int* __restrict__ sidx, int n_lines,
+                      int n_inner_dense, long long stride_line, long long stride_inner, int K, int mode, int* out_idx,
+                      float* out_val, int* out_cnt, int idx_off = 0) {
+  __shared__ CtaSelectSmem<BINS> sel;
+  __shared__ int s_cnt, s_tie, s_npos, s_nneg, s_nnan;
   const int tid = threadIdx.x, lane = tid & 31;
   const bool nan_high = mode == 0;
   for (int line = blockIdx.x; line < n_lines; line += gridDim.x) {
@@ -78,49 +73,16 @@ __global__ void __launch_bounds__(THREADS) topk_lines_kernel(const float* __rest
     u64 thr = 0;
     int ties = keep;  // how many cells with key == thr are taken
     if (keep > 0 && keep < nnz) {
-      u64 prefix = 0, mask = 0;
-      int need = keep;
-      for (int shift = 53; ; shift -= 11) {
-        const int sh = max(shift, 0);
-        const int nb = shift >= 0 ? 11 : 11 + shift;  // last digit is 9 bits wide
-        for (int i = tid; i < BINS; i += THREADS) hist[i] = 0;
-        __syncthreads();
-        for (int q = tid; q < n_inner; q += THREADS) {
-          const float v = L[(long long)q * stride_inner];
-          if (v != 0.f) {
-            const u64 key = line_key(v, SPARSE ? LI[q] : q + idx_off, nan_high);
-            if ((key & mask) == prefix) atomicAdd(&hist[(int)((key >> sh) & ((1u << nb) - 1))], 1);
-          }
-        }
-        __syncthreads();
-        if (tid < 32) {
-          constexpr int PER = BINS / 32;
-          int local = 0;
-          for (int b = 0; b < PER; ++b) local += hist[tid * PER + b];
-          int incl = local;
-#pragma unroll
-          for (int off = 1; off < 32; off <<= 1) {
-            const int t = __shfl_down_sync(0xffffffffu, incl, off);
-            if (tid + off < 32) incl += t;
-          }
-          int cum = incl - local;
-          for (int b = PER - 1; b >= 0; --b) {
-            const int c = hist[tid * PER + b];
-            if (cum < need && cum + c >= need) { s_digit = tid * PER + b; s_need = need - cum; }
-            cum += c;
-          }
-        }
-        __syncthreads();
-        prefix |= ((u64)s_digit) << sh;
-        mask |= ((u64)((1u << nb) - 1)) << sh;
-        need = s_need;
-        __syncthreads();
-        if (shift <= 0) break;
-      }
-      thr = prefix;  // the keep-th largest key itself
-      ties = need;   // 1 unless entries repeat (index, value): keys are distinct within a line otherwise
+      const auto sel_key = [&](int q, u64& key) {
+        const float v = L[(long long)q * stride_inner];
+        if (v != 0.f) key = line_key(v, SPARSE ? LI[q] : q + idx_off, nan_high);
+        return v != 0.f;
+      };
+      const Threshold<u64> t = radix_select<u64, 11, false>(CtaSelect<THREADS, BINS>(sel), n_inner, keep, sel_key);
+      thr = t.thr;
+      ties = t.need;  // 1 unless entries repeat (index, value): keys are distinct within a line otherwise
     }
-    // emit: keep - ties keys above thr, then `ties` of the keys equal to it
+    // emit: the keys above thr, then at most `ties` of the keys equal to it
     if (keep > 0) {
       for (int q = tid; q < n_inner; q += THREADS) {
         const float v = L[(long long)q * stride_inner];

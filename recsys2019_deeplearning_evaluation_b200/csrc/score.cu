@@ -16,6 +16,7 @@
 #include <cfloat>
 
 #include "common.cuh"
+#include "select.cuh"
 
 namespace b200 {
 namespace score {
@@ -117,73 +118,23 @@ __global__ void mask_items_kernel(const unsigned char* __restrict__ keep, int n_
 // Unsigned key in the order of np.lexsort((arange, -s)), the host ranking (BaseRecommender.py:189-196): +inf, finite
 // values descending, -inf, then NaN of either sign (key 0, below -inf's 0x007FFFFF).  -0 and +0 are one value, so they
 // tie and fall back to the item index.
-__device__ __forceinline__ unsigned orderable(float v) {
-  const unsigned b = __float_as_uint(v == 0.f ? 0.f : v);
-  return v != v ? 0u : (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
+__device__ __forceinline__ unsigned lexsort_order(float v) { return v != v ? 0u : orderable(v == 0.f ? 0.f : v); }
 // the same order on doubles: NaN -> 0, below -inf's 0x000FFFFFFFFFFFFF
-__device__ __forceinline__ u64 orderable(double v) {
-  const u64 b = (u64)__double_as_longlong(v == 0.0 ? 0.0 : v);
-  return v != v ? 0ull : (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
-}
+__device__ __forceinline__ u64 lexsort_order(double v) { return v != v ? 0ull : orderable(v == 0.0 ? 0.0 : v); }
 
-// The top-N key of the score at position q: the orderable score, then ~q, so that larger keys rank first and equal
-// scores go to the lower position.  fp32: one 64-bit word, 6 radix passes of 11 bits.  fp64: 96 bits (the 64-bit
-// orderable double, then ~q), 9 passes; the radix digit at bit `sh` may straddle the two words.  `image` is what the
-// table reports for a score: fp32 as it is; fp64 rounded to fp32 with finite values saturated to +-FLT_MAX, so that an
-// entry is finite exactly when its score is (the evaluation kernels read nothing else).
+// The top-N key of the score at position q: the lexsort order of the score, then ~q, so that larger keys rank first and
+// equal scores go to the lower position.  fp32: one 64-bit word, 6 radix passes of 11 bits.  fp64: 96 bits, 9 passes.
+// `image` is what the table reports for a score: fp32 as it is; fp64 rounded to fp32 with finite values saturated to
+// +-FLT_MAX, so that an entry is finite exactly when its score is (the evaluation kernels read nothing else).
 template <typename T> struct TopnKey;
 template <> struct TopnKey<float> {
   typedef u64 Key;
-  static constexpr int TOP_SHIFT = 53;  // digits at bits 53, 42, ..., 9 and the last 9 bits
-  static __device__ __forceinline__ Key make(float v, int q) {
-    return (((u64)orderable(v)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
-  }
-  static __device__ __forceinline__ int digit(Key k, int sh, int nb) { return (int)((k >> sh) & ((1u << nb) - 1)); }
-  static __device__ __forceinline__ bool matches(Key k, Key prefix, Key mask) { return (k & mask) == prefix; }
-  static __device__ __forceinline__ void fix_digit(Key& prefix, Key& mask, int d, int sh, int nb) {
-    prefix |= ((u64)d) << sh;
-    mask |= ((u64)((1u << nb) - 1)) << sh;
-  }
-  static __device__ __forceinline__ bool greater(Key a, Key b) { return a > b; }
-  static __device__ __forceinline__ bool at_least(Key a, Key b) { return a >= b; }
-  static __device__ __forceinline__ int position(Key k) { return (int)(0xFFFFFFFFu - (unsigned)k); }
+  static __device__ __forceinline__ Key make(float v, int q) { return KeyBits<Key>::make(lexsort_order(v), 0xFFFFFFFFu - (unsigned)q); }
   static __device__ __forceinline__ float image(float v) { return v; }
-};
-struct Key96 {
-  u64 hi;       // orderable(score)
-  unsigned lo;  // ~position
 };
 template <> struct TopnKey<double> {
   typedef Key96 Key;
-  static constexpr int TOP_SHIFT = 85;  // digits at bits 85, 74, ..., 8 and the last 8 bits
-  static __device__ __forceinline__ Key make(double v, int q) { return Key96{orderable(v), 0xFFFFFFFFu - (unsigned)q}; }
-  static __device__ __forceinline__ int digit(const Key& k, int sh, int nb) {
-    const u64 w = sh >= 32 ? k.hi >> (sh - 32) : (k.hi << (32 - sh)) | (u64)(k.lo >> sh);
-    return (int)(w & ((1u << nb) - 1));
-  }
-  static __device__ __forceinline__ bool matches(const Key& k, const Key& prefix, const Key& mask) {
-    return (k.hi & mask.hi) == prefix.hi && (k.lo & mask.lo) == prefix.lo;
-  }
-  static __device__ __forceinline__ void fix_digit(Key& prefix, Key& mask, int d, int sh, int nb) {
-    const u64 m = (1u << nb) - 1;
-    if (sh >= 32) {
-      prefix.hi |= (u64)d << (sh - 32);
-      mask.hi |= m << (sh - 32);
-    } else {
-      prefix.hi |= (u64)d >> (32 - sh);
-      mask.hi |= m >> (32 - sh);
-      prefix.lo |= (unsigned)((u64)d << sh);
-      mask.lo |= (unsigned)(m << sh);
-    }
-  }
-  static __device__ __forceinline__ bool greater(const Key& a, const Key& b) {
-    return a.hi > b.hi || (a.hi == b.hi && a.lo > b.lo);
-  }
-  static __device__ __forceinline__ bool at_least(const Key& a, const Key& b) {
-    return a.hi > b.hi || (a.hi == b.hi && a.lo >= b.lo);
-  }
-  static __device__ __forceinline__ int position(const Key& k) { return (int)(0xFFFFFFFFu - k.lo); }
+  static __device__ __forceinline__ Key make(double v, int q) { return KeyBits<Key>::make(lexsort_order(v), 0xFFFFFFFFu - (unsigned)q); }
   static __device__ __forceinline__ float image(double v) {
     const float f = (float)v;
     return isfinite(v) ? fminf(fmaxf(f, -FLT_MAX), FLT_MAX) : f;
@@ -192,71 +143,46 @@ template <> struct TopnKey<double> {
 
 // The `cutoff` best of the n scores L[0..n) of one row, best first (BaseRecommender.py:189-196); ties -> ascending
 // position.  Position q is item q, or items[q] when a (strictly ascending) item map is given, so that ties go to the
-// ascending item either way.  Called by all TOPN_THREADS threads of a CTA: MSB radix select of the cutoff-th key over
-// the TopnKey keys (score bits, ~position), then the survivors are ranked by counting (cutoff is small: <= 1024).
+// ascending item either way.  Called by all TOPN_THREADS threads of a CTA: radix select of the cutoff-th TopnKey key
+// (select.cuh, 11-bit digits), then the survivors are ranked by counting (cutoff is small: <= 1024).
 // out_items / out_scores: this row's `cutoff` slots; past the end of the row -1 / -inf.
 constexpr int TOPN_THREADS = 256;
 constexpr int TOPN_MAX = 1024;
 template <typename T>
 struct TopnSmem {
-  int hist[2048];
-  int digit, need, cnt;
+  CtaSelectSmem<2048> sel;
+  int cnt;
   typename TopnKey<T>::Key cand[TOPN_MAX];
 };
 template <typename T>
 __device__ __forceinline__ void topn_row(const T* L, int n, int cutoff, const int* items, int* out_items, float* out_scores,
                                          TopnSmem<T>& sm) {
   typedef TopnKey<T> K;
+  typedef typename K::Key Key;
+  typedef KeyBits<Key> KB;
   const int tid = threadIdx.x;
   const int keep = min(cutoff, n);
-  typename K::Key prefix{}, mask{};
-  int need = keep;
+  Key thr{};
   if (keep < n) {
-    for (int shift = K::TOP_SHIFT;; shift -= 11) {
-      const int sh = max(shift, 0), nb = shift >= 0 ? 11 : 11 + shift;
-      for (int i = tid; i < 2048; i += TOPN_THREADS) sm.hist[i] = 0;
-      __syncthreads();
-      for (int q = tid; q < n; q += TOPN_THREADS) {
-        const typename K::Key key = K::make(L[q], q);
-        if (K::matches(key, prefix, mask)) atomicAdd(&sm.hist[K::digit(key, sh, nb)], 1);
-      }
-      __syncthreads();
-      if (tid < 32) {
-        int local = 0;
-        for (int b = 0; b < 64; ++b) local += sm.hist[tid * 64 + b];
-        int incl = local;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-          const int t = __shfl_down_sync(0xffffffffu, incl, off);
-          if (tid + off < 32) incl += t;
-        }
-        int cum = incl - local;
-        for (int b = 63; b >= 0; --b) {
-          const int c = sm.hist[tid * 64 + b];
-          if (cum < need && cum + c >= need) { sm.digit = tid * 64 + b; sm.need = need - cum; }
-          cum += c;
-        }
-      }
-      __syncthreads();
-      K::fix_digit(prefix, mask, sm.digit, sh, nb);
-      need = sm.need;
-      __syncthreads();
-      if (shift <= 0) break;
-    }
+    const auto sel_key = [&](int q, Key& key) {
+      key = K::make(L[q], q);
+      return true;
+    };
+    thr = radix_select<Key, 11, false>(CtaSelect<TOPN_THREADS, 2048>(sm.sel), n, keep, sel_key).thr;
   }
   if (tid == 0) sm.cnt = 0;
   __syncthreads();
   for (int q = tid; q < n; q += TOPN_THREADS) {
-    const typename K::Key key = K::make(L[q], q);
-    if (K::at_least(key, prefix)) sm.cand[atomicAdd(&sm.cnt, 1)] = key;
+    const Key key = K::make(L[q], q);
+    if (KB::at_least(key, thr)) sm.cand[atomicAdd(&sm.cnt, 1)] = key;
   }
   __syncthreads();
   const int m = sm.cnt;  // == keep
   for (int t = tid; t < m; t += TOPN_THREADS) {
-    const typename K::Key k = sm.cand[t];
+    const Key k = sm.cand[t];
     int rank = 0;
-    for (int q = 0; q < m; ++q) rank += K::greater(sm.cand[q], k);
-    const int q = K::position(k);
+    for (int q = 0; q < m; ++q) rank += KB::greater(sm.cand[q], k);
+    const int q = (int)(0xFFFFFFFFu - KB::low(k));
     out_items[rank] = items ? items[q] : q;
     out_scores[rank] = K::image(L[q]);
   }
@@ -435,7 +361,7 @@ __global__ void __launch_bounds__(CAND_TOPN_WARPS * 32) cand_topn_warp_kernel(
   for (int q = lane; q < n; q += 32) {
     const float v = cand_masked(L[q], items[q], seen, n_seen, ignore);
     s_val[w][q] = v;
-    s_key[w][q] = (((u64)orderable(v)) << 32) | (u64)(0xFFFFFFFFu - (unsigned)q);
+    s_key[w][q] = TopnKey<float>::make(v, q);
   }
   __syncwarp();
   int* oi = out_items + (size_t)b * cutoff;

@@ -40,8 +40,9 @@
 // words), they are evaluated exactly into 64-bit keys (similarity bits << 32 | ~original index: ties -> ascending index).
 // If there are at least K of them, the similarity of (count 3, largest norm) is a floor of the K-th best, and count-2 /
 // count-1 cells can only matter in the leading norm tiles whose best possible similarity reaches the floor (none at C5).
-// One radix select (8-bit digits, 512 threads) at the end keeps the K best.  Pushes are chunked by norm tile with known
-// cell counts, so the key buffer cannot overflow; a full buffer is pruned to the K best first (raising the floor).
+// One radix select (select.cuh: 8-bit digits, 512 threads) at the end keeps the K best.  Pushes are chunked by norm tile
+// with known cell counts, so the key buffer cannot overflow; a full buffer is pruned to the K best first (raising the
+// floor).
 
 constexpr int D_THREADS = 512;
 constexpr int D_WARPS = D_THREADS / 32;
@@ -63,9 +64,8 @@ __device__ __forceinline__ int k1d_gap(const int4& c, int e) {  // g_(e + 1)
 
 struct K1DShared {
   int item, nbuf, cnt, nibsum, tstop, chunk_end, chunk_cnt;
-  int need, digit, bincnt, ncand, expect;
-  u64 kor, kand;
-  int hist[256];
+  int ncand, expect;
+  CtaSelectSmem<256> sel;
 };
 
 // bit 0 of every nibble of the result is set iff that nibble of w is >= 3 / == 2 / == 1
@@ -81,62 +81,16 @@ __device__ __forceinline__ int nib_sum(unsigned w) {
 }
 
 // Block-wide (all D_THREADS threads): keeps the K largest keys of buf[0..n) compacted at the front (any order), returns
-// the K-th largest key (0 when n <= K: nothing is cut).  Keys are distinct and non-zero.  MSB-first radix select with
-// 8-bit digits; stops as soon as a whole bin is taken.
+// the K-th largest key (0 when n <= K: nothing is cut).  Keys are distinct and non-zero.
 __device__ u64 d_select(u64* buf, int n, int K, K1DShared* ds, int* n_out) {
   const int tid = threadIdx.x;
   __syncthreads();
   if (n <= K) { *n_out = n; return 0ull; }
-  // digits above the highest bit in which two keys differ are the same for every key: start below them
-  {
-    if (tid == 0) { ds->kor = 0ull; ds->kand = ~0ull; }
-    __syncthreads();
-    u64 o = 0ull, a = ~0ull;
-    for (int q = tid; q < n; q += D_THREADS) { const u64 k = buf[q]; o |= k; a &= k; }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) { o |= __shfl_xor_sync(0xffffffffu, o, off); a &= __shfl_xor_sync(0xffffffffu, a, off); }
-    if ((tid & 31) == 0) { atomicOr(&ds->kor, o); atomicAnd(&ds->kand, a); }
-    __syncthreads();
-  }
-  const u64 diff = ds->kor ^ ds->kand;
-  int pass = diff ? (63 - __clzll((long long)diff)) >> 3 : 0;
-  u64 prefix = pass < 7 ? (ds->kor >> ((pass + 1) * 8)) << ((pass + 1) * 8) : 0ull;
-  int need = K;
-  const int one = n > 0 ? 1 : 0;  // a run-time 1: a literal makes ptxas emit ATOMS.POPC.INC inside a loop that peels one address per trip
-  for (; pass >= 0; --pass) {
-    const int shift = pass * 8;
-    if (tid < 256) ds->hist[tid] = 0;
-    __syncthreads();
-    for (int q = tid; q < n; q += D_THREADS) {
-      const u64 k = buf[q];
-      if (pass == 7 || (k >> (shift + 8)) == (prefix >> (shift + 8))) atomicAdd(&ds->hist[(int)((k >> shift) & 255ull)], one);
-    }
-    __syncthreads();
-    if (tid < 32) {  // one warp: bins 255 .. 0, eight per lane, highest bins in lane 0
-      int c[8], local = 0;
-#pragma unroll
-      for (int b = 0; b < 8; ++b) { c[b] = ds->hist[255 - (tid * 8 + b)]; local += c[b]; }
-      int incl = local;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, incl, off);
-        if (tid >= off) incl += t;
-      }
-      int cum = incl - local;  // keys in higher bins
-#pragma unroll
-      for (int b = 0; b < 8; ++b) {
-        if (cum < need && cum + c[b] >= need) { ds->digit = 255 - (tid * 8 + b); ds->need = need - cum; ds->bincnt = c[b]; }
-        cum += c[b];
-      }
-    }
-    __syncthreads();
-    prefix |= ((u64)ds->digit) << shift;
-    need = ds->need;
-    const int bincnt = ds->bincnt;
-    __syncthreads();
-    if (bincnt == need) break;  // the whole bin survives: every key with this prefix is kept
-  }
-  const u64 thr = prefix;  // undecided low digits are zero: the smallest key the kept bins can hold
+  const auto sel_key = [&](int q, u64& key) {
+    key = buf[q];
+    return true;
+  };
+  const u64 thr = radix_select<u64, 8, true>(CtaSelect<D_THREADS, 256>(ds->sel), n, K, sel_key).thr;
   // compaction through registers (n <= 8 * D_THREADS is guaranteed by the host-side cap)
   u64 keep[8];
 #pragma unroll
@@ -662,58 +616,9 @@ constexpr int S_CTAS = 6;             // CTAs per SM its registers are bounded f
 constexpr int S_CAP = 4 * D_THREADS;  // the longest candidate list the select kernel decides (the K1-D kernel's key buffer)
 constexpr int S_ILP = 12;             // candidates per lane in flight while the keys are built (C5: ~430 per column)
 // shared memory of one select warp: its radix histogram, then the keys of a list of up to sel_cap candidates (the handle's
-// bound, <= S_CAP: sized from the expected list lengths at create time, so that more warps fit on an SM)
-__host__ __device__ __forceinline__ int k1d_select_warp_bytes(int sel_cap) { return 256 * 4 + sel_cap * 8; }
-
-// One warp: the K-th largest key of buf[0..n), so that exactly the K largest keys are >= it (0 when n <= K: nothing is
-// cut).  Keys are distinct and non-zero.  d_select's MSB-first radix select with 8-bit digits on one warp and its own
-// histogram: it starts below the leading digits that every key shares and stops as soon as a whole bin is taken.
-__device__ u64 w_select(const u64* buf, int* hist, int n, int K) {
-  const int lane = threadIdx.x & 31;
-  if (n <= K) return 0ull;
-  u64 o = 0ull, a = ~0ull;
-  for (int q = lane; q < n; q += 32) { const u64 k = buf[q]; o |= k; a &= k; }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) { o |= __shfl_xor_sync(0xffffffffu, o, off); a &= __shfl_xor_sync(0xffffffffu, a, off); }
-  const u64 diff = o ^ a;
-  int pass = diff ? (63 - __clzll((long long)diff)) >> 3 : 0;
-  u64 prefix = pass < 7 ? (o >> ((pass + 1) * 8)) << ((pass + 1) * 8) : 0ull;
-  int need = K;
-  const int one = n > 0 ? 1 : 0;  // a run-time 1, as in d_select
-  for (; pass >= 0; --pass) {
-    const int shift = pass * 8;
-    for (int b = lane; b < 256; b += 32) hist[b] = 0;
-    __syncwarp();
-    for (int q = lane; q < n; q += 32) {
-      const u64 k = buf[q];
-      if (pass == 7 || (k >> (shift + 8)) == (prefix >> (shift + 8))) atomicAdd(&hist[(int)((k >> shift) & 255ull)], one);
-    }
-    __syncwarp();
-    int c[8], local = 0;  // bins 255 .. 0, eight per lane, highest bins in lane 0
-#pragma unroll
-    for (int b = 0; b < 8; ++b) { c[b] = hist[255 - (lane * 8 + b)]; local += c[b]; }
-    int incl = local;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, incl, off);
-      if (lane >= off) incl += t;
-    }
-    int cum = incl - local, digit = -1, rest = 0, bincnt = 0;
-#pragma unroll
-    for (int b = 0; b < 8; ++b) {
-      if (cum < need && cum + c[b] >= need) { digit = 255 - (lane * 8 + b); rest = need - cum; bincnt = c[b]; }
-      cum += c[b];
-    }
-    const int src = __ffs(__ballot_sync(0xffffffffu, digit >= 0)) - 1;
-    digit = __shfl_sync(0xffffffffu, digit, src);
-    need = __shfl_sync(0xffffffffu, rest, src);
-    bincnt = __shfl_sync(0xffffffffu, bincnt, src);
-    prefix |= ((u64)digit) << shift;
-    __syncwarp();  // every lane has read the histogram before the next pass clears it
-    if (bincnt == need) break;
-  }
-  return prefix;
-}
+// bound, <= S_CAP: sized from the expected list lengths at create time, so that more warps fit on an SM), rounded to 16
+// bytes so that every warp's histogram stays 16-byte aligned (select.cuh reads it as int4)
+__host__ __device__ __forceinline__ int k1d_select_warp_bytes(int sel_cap) { return 256 * 4 + (sel_cap * 8 + 15) / 16 * 16; }
 
 // One warp per column of the work list: keys from the column's own and mirror lists, the decision rule of sim_k1d_kernel's
 // collected path, the K best, emit -- or the column goes to the redo list (all columns when the call has fallen back).
@@ -779,7 +684,12 @@ __global__ void __launch_bounds__(32 * S_WARPS, S_CTAS) sim_k1d_select_kernel(co
     return;
   }
   __syncwarp();
-  const u64 thr = w_select(keys, hist, n_have, K);
+  const auto sel_key = [&](int q, u64& key) {
+    key = keys[q];
+    return true;
+  };
+  // the K-th largest key, so that exactly the K largest keys are >= it (0 when n_have == K: nothing is cut)
+  const u64 thr = n_have > K ? radix_select<u64, 8, true>(WarpSelect{hist}, n_have, K, sel_key).thr : 0ull;
   // emit while compacting: the kept keys of every 32 take the next output slots in lane order
   const size_t out_base = (size_t)lc * K;
   int kept = 0;

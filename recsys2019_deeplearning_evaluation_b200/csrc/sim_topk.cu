@@ -35,6 +35,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "select.cuh"
 
 namespace b200 {
 namespace sim {

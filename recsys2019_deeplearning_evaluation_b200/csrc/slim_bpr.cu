@@ -26,6 +26,7 @@
 
 #include "common.cuh"
 #include "sampler.cuh"
+#include "select.cuh"
 
 namespace b200 {
 namespace slim {
@@ -436,22 +437,18 @@ __global__ void __launch_bounds__(256) slim_tree_slot_kernel(const Params p, con
 // through topK_selection_from_list pyx:954-1031.  A row holding more than K cells keeps the K largest by value; the reference
 // sorts the column-ordered list with a stable qsort on the value, so among equal values the HIGHER columns survive:
 // key = (orderable value << 32) | column, keep the K largest keys.  Dropped cells vanish from the structure (a later touch
-// creates them again with value 0).  One warp per row: 8-bit radix select over the 64-bit keys, read from the row in
-// global memory (L1/L2-resident across the passes), stopping at the first digit whose bin is kept whole.
-__device__ __forceinline__ unsigned tree_orderable(float v) {
-  const unsigned b = __float_as_uint(v);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ u64 tree_cut_key(u64 cell, float v) { return ((u64)tree_orderable(v) << 32) | (cell & 0xFFFFFFFFull); }
+// creates them again with value 0).  One warp per row: radix select (select.cuh, 8-bit digits) over the 64-bit keys, read
+// from the row in global memory (L1/L2-resident across the passes).
+__device__ __forceinline__ u64 tree_cut_key(u64 cell, float v) { return ((u64)orderable(v) << 32) | (cell & 0xFFFFFFFFull); }
 
 constexpr int CUT_THREADS = 256;
 // thr[r]: the row keeps the cells whose cut key is >= thr[r]; cnt[r]: how many
 __global__ void __launch_bounds__(CUT_THREADS) slim_tree_cut_select_kernel(const u64* __restrict__ key, const float* __restrict__ val,
                                                                            const long long* __restrict__ rowptr, int n, int K, u64* thr,
                                                                            long long* cnt) {
-  __shared__ unsigned hist[CUT_THREADS / 32][256];
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  unsigned* h = hist[wib];
+  __shared__ __align__(16) int hist[CUT_THREADS / 32][256];
+  const int lane = threadIdx.x & 31;
+  const WarpSelect g{hist[threadIdx.x >> 5]};
   const int w = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   const int n_warps = (int)(((long long)gridDim.x * blockDim.x) >> 5);
   for (int row = w; row < n; row += n_warps) {
@@ -460,48 +457,12 @@ __global__ void __launch_bounds__(CUT_THREADS) slim_tree_cut_select_kernel(const
       if (lane == 0) { thr[row] = 0ull; cnt[row] = hi - lo; }
       continue;
     }
-    u64 prefix = 0, mask = 0;
-    unsigned need = (unsigned)K;
-    for (int shift = 56; shift >= 0; shift -= 8) {
-      for (int b = lane; b < 256; b += 32) h[b] = 0u;
-      __syncwarp();
-      for (long long t = lo + lane; t < hi; t += 32) {
-        const u64 k = tree_cut_key(key[t], val[t]);
-        if ((k & mask) == prefix) atomicAdd(&h[(int)((k >> shift) & 255u)], 1u);
-      }
-      __syncwarp();
-      // the bin holding the need-th largest key: lane l owns bins [8l, 8l + 8)
-      unsigned loc = 0;
-#pragma unroll
-      for (int b = 0; b < 8; ++b) loc += h[lane * 8 + b];
-      unsigned incl = loc;  // sum over the lanes >= this one
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const unsigned v = __shfl_down_sync(0xffffffffu, incl, o);
-        if (lane + o < 32) incl += v;
-      }
-      const unsigned above = incl - loc;
-      const unsigned owner = __ffs(__ballot_sync(0xffffffffu, above < need && need <= incl)) - 1;
-      int digit = 0;
-      unsigned rest = 0, bin = 0;
-      if (lane == (int)owner) {
-        unsigned cum = above;
-        for (int b = 7; b >= 0; --b) {
-          const unsigned c = h[lane * 8 + b];
-          if (cum + c >= need) { digit = lane * 8 + b; rest = need - cum; bin = c; break; }
-          cum += c;
-        }
-      }
-      digit = __shfl_sync(0xffffffffu, digit, owner);
-      rest = __shfl_sync(0xffffffffu, rest, owner);
-      bin = __shfl_sync(0xffffffffu, bin, owner);
-      __syncwarp();
-      prefix |= (u64)digit << shift;
-      mask |= 0xFFull << shift;
-      need = rest;
-      if (bin == need) break;  // every key of this bin is kept (the keys are distinct: at the last digit bin == need == 1)
-    }
-    if (lane == 0) { thr[row] = prefix; cnt[row] = K; }  // keys are kept iff (key & mask) >= prefix, i.e. key >= prefix
+    const auto sel_key = [&](int q, u64& k) {
+      k = tree_cut_key(key[lo + q], val[lo + q]);
+      return true;
+    };
+    const u64 t = radix_select<u64, 8, false>(g, (int)(hi - lo), K, sel_key).thr;
+    if (lane == 0) { thr[row] = t; cnt[row] = K; }
   }
 }
 
