@@ -27,6 +27,7 @@ extern "C" {
 #define B200_E_NOMEM (-3)   /* device or host allocation failed */
 #define B200_E_UNSUPPORTED (-4)
 #define B200_E_SINGULAR (-5)    /* the matrix to invert is exactly singular (np.linalg.LinAlgError) */
+#define B200_E_NOT_SPD (-6)     /* a Cholesky factorisation met a non-positive pivot and has no fallback */
 
 const char* b200_last_error(void);
 int b200_version(void);
@@ -426,6 +427,25 @@ int b200_debug_gemm_device(int kind, int M, int N, int K, float alpha, const flo
  * that path: 3 * 8 * n_pad^2 bytes besides d_G and d_B.  A singular matrix returns B200_E_SINGULAR. */
 int b200_ease_from_gram_device(const float* d_G, int n_items, const int32_t* d_urm_indices, int64_t nnz, float l2_norm,
                                float* h_B, float* d_B, void* stream);
+/* EASE_R fit inside one buffer, for catalogues whose b200_ease_from_gram_device footprint (d_G, d_B and 3 + 2 n_pad^2
+ * floats of its own) does not fit on the device.  d_A: [n_pad, n_pad] row-major fp32, n_pad = n_items rounded up to a
+ * multiple of 128, with X^T X in its top-left n_items x n_items block (the rest is overwritten).  The call sets the
+ * popularity diagonal + l2_norm and the identity padding, inverts in place (LAPACK potrf -> trtri -> lauum: blocked
+ * Cholesky, L := L^-1 right to left, P := L^-T L^-1 top to bottom, each O(n^3) product on the 3xTF32 tensor cores with
+ * K ranges of at most 512), writes B[i, j] = P[i, j] / (-P[j, j]), B[j, j] = 0 over the lower triangle of P, and compacts
+ * the rows so that on return the first n_items^2 floats of d_A are B as a contiguous [n_items, n_items] array.  About
+ * n^3 flops in all (n^3 / 3 per stage).  Device memory besides d_A: b200_ease_inplace_workspace_bytes, O(n_pad * 128).
+ * There is no fp64 LU fallback (it needs 24 * n_pad^2 more bytes): a Gram that is not positive definite (explicit ratings
+ * at a small l2_norm) returns B200_E_NOT_SPD with d_A overwritten. */
+int b200_ease_inplace_device(float* d_A, int n_items, const int32_t* d_urm_indices, int64_t nnz, float l2_norm, void* stream);
+/* every device byte b200_ease_inplace_device allocates besides d_A (an upper bound: workspaces already grown by an
+ * earlier call are reused) */
+int b200_ease_inplace_workspace_bytes(int n_items, int64_t* bytes);
+/* TEST HOOK: the stages of the in-place inverse on a symmetric positive definite [n_pad, n_pad] fp32 matrix at d_A (n_pad
+ * a multiple of 128): op 0 leaves the Cholesky factor L in the lower triangle (the blocks above the diagonal keep their
+ * input); op 1 then L^-1 (strict upper triangle zero); op 2 then P = L^-T L^-1 in the lower triangle.  B200_E_NOT_SPD on a
+ * non-positive pivot. */
+int b200_ease_inplace_debug_device(int op, float* d_A, int n_pad, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K4: implicit ALS half epoch  (hot path iii)

@@ -114,6 +114,9 @@ SIGNATURES = {
     "b200_debug_dgemm_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, c_void,
                                                ctypes.c_int, c_void, ctypes.c_int, ctypes.c_double, c_void, ctypes.c_int, c_void]),
     "b200_ease_from_gram_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, ctypes.c_int64, ctypes.c_float, c_void, c_void, c_void]),
+    "b200_ease_inplace_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, ctypes.c_int64, ctypes.c_float, c_void]),
+    "b200_ease_inplace_workspace_bytes": (ctypes.c_int, [ctypes.c_int, c_i64_p]),
+    "b200_ease_inplace_debug_device": (ctypes.c_int, [ctypes.c_int, c_void, ctypes.c_int, c_void]),
     "b200_feature_weighting_device": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int64, c_void, c_void, c_void,
                                                      ctypes.c_float, ctypes.c_float, c_void]),
     "b200_eval_accumulate_device": (ctypes.c_int, [c_void, ctypes.c_int, c_void, c_void, ctypes.c_int, c_void, c_void, c_void, c_void,
@@ -139,6 +142,10 @@ _lib = None
 
 class B200Error(RuntimeError):
     pass
+
+
+class NotPositiveDefiniteError(B200Error):
+    """B200_E_NOT_SPD: a Cholesky factorisation without a fallback met a non-positive pivot."""
 
 
 def load():
@@ -168,6 +175,8 @@ def check(rc):
         raise MemoryError(msg)
     if rc == -5:
         raise np.linalg.LinAlgError(msg)
+    if rc == -6:
+        raise NotPositiveDefiniteError(msg)
     raise B200Error("libb200rec error %d: %s" % (rc, msg))
 
 

@@ -16,6 +16,8 @@
 // The popularity diagonal is a count, below sum r^2 on explicit ratings, so there G can be indefinite.  When the Cholesky
 // meets a non-positive pivot, G is inverted again in fp64 by the pivoted LU of lu_inverse.cu (what np.linalg.inv does);
 // an fp32 LU of these systems (cond up to ~1e7) would be far from the reference.
+// Catalogues whose footprint here (G, B and 5 n_pad^2 floats) does not fit take b200_ease_inplace_device: the same
+// Cholesky, then trtri and lauum in place and an in-place finish, all inside one n_pad^2 buffer (no LU fallback there).
 #include <algorithm>
 #include <vector>
 
@@ -149,28 +151,24 @@ void gemm(cudaStream_t st, int M, int N, int K, float alpha, const float* A, int
   count_launch();
 }
 
-// In-place inverse of a symmetric positive definite n_pad x n_pad matrix (n_pad multiple of 128, row-major, device).
-// Returns 0 with A^{-1} (full symmetric matrix) in d_A, or the 1-based position of the first non-positive pivot inside a
-// diagonal block (the factorisation runs to the end, no inverse is formed).  d_work: 2 * n_pad * n_pad floats.
-int spd_inverse(float* d_A, int n_pad, float* d_work, cudaStream_t st) {
+// 1. Right-looking blocked Cholesky (lower) of the n_pad x n_pad matrix at d_A in place, A = L L^T: every diagonal block is
+// factored (strict upper triangle zeroed) and its inverse written to inv_blocks (n_pad / NB blocks of NB x NB); the blocks
+// above the diagonal keep their stale input values.  panel: n_pad x NB floats.  Returns 0, or the 1-based position of the
+// first non-positive pivot inside a diagonal block (the factorisation runs to the end).
+int cholesky(float* d_A, int n_pad, float* inv_blocks, float* panel, cudaStream_t st) {
   const int nblk = n_pad / NB;
-  const long long nn = (long long)n_pad * n_pad;
-  float* Linv = d_work;        // n_pad x n_pad
-  float* panel = d_work + nn;  // n_pad x NB  (first part of the second workspace)
-  DevBuf<float> inv_blocks((size_t)nblk * NB * NB);
   DevBuf<int> info(1);
   B200_CUDA(cudaMemsetAsync(info.get(), 0, sizeof(int), st));
   B200_CUDA(cudaFuncSetAttribute(potrf_inv_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, NB * (NB + 1) * 4));
-  // ---- 1. blocked Cholesky (lower), A = L L^T
   for (int k = 0; k < nblk; ++k) {
     float* Akk = d_A + (long long)k * NB * n_pad + (long long)k * NB;
-    potrf_inv_block_kernel<<<1, 256, NB * (NB + 1) * 4, st>>>(Akk, n_pad, inv_blocks.get() + (size_t)k * NB * NB, info.get());
+    potrf_inv_block_kernel<<<1, 256, NB * (NB + 1) * 4, st>>>(Akk, n_pad, inv_blocks + (size_t)k * NB * NB, info.get());
     count_launch();
     const int rem = n_pad - (k + 1) * NB;
     if (rem > 0) {
       float* A21 = Akk + (long long)NB * n_pad;
       // panel = A21 * inv(L11)^T
-      gemm<false, true, false>(st, rem, NB, NB, 1.f, A21, n_pad, 0, inv_blocks.get() + (size_t)k * NB * NB, NB, 0, 0.f, panel, NB, 0, 1);
+      gemm<false, true, false>(st, rem, NB, NB, 1.f, A21, n_pad, 0, inv_blocks + (size_t)k * NB * NB, NB, 0, 0.f, panel, NB, 0, 1);
       copy_block_kernel<<<div_up((long long)rem * NB, 256), 256, 0, st>>>(panel, NB, A21, n_pad, rem, NB);
       count_launch();
       // A22 -= L21 * L21^T
@@ -181,6 +179,19 @@ int spd_inverse(float* d_A, int n_pad, float* d_work, cudaStream_t st) {
   int h_info = 0;
   B200_CUDA(cudaMemcpyAsync(&h_info, info.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
   B200_CUDA(cudaStreamSynchronize(st));
+  return h_info;
+}
+
+// In-place inverse of a symmetric positive definite n_pad x n_pad matrix (n_pad multiple of 128, row-major, device).
+// Returns 0 with A^{-1} (full symmetric matrix) in d_A, or the 1-based position of the first non-positive pivot inside a
+// diagonal block (the factorisation runs to the end, no inverse is formed).  d_work: 2 * n_pad * n_pad floats.
+int spd_inverse(float* d_A, int n_pad, float* d_work, cudaStream_t st) {
+  const int nblk = n_pad / NB;
+  const long long nn = (long long)n_pad * n_pad;
+  float* Linv = d_work;        // n_pad x n_pad
+  float* panel = d_work + nn;  // n_pad x NB  (first part of the second workspace)
+  DevBuf<float> inv_blocks((size_t)nblk * NB * NB);
+  const int h_info = cholesky(d_A, n_pad, inv_blocks.get(), panel, st);
   if (h_info != 0) return h_info;
   // ---- 2. Linv = L^{-1}: diagonal blocks, then one block diagonal at a time
   B200_CUDA(cudaMemsetAsync(Linv, 0, sizeof(float) * (size_t)nn, st));
@@ -203,6 +214,127 @@ int spd_inverse(float* d_A, int n_pad, float* d_work, cudaStream_t st) {
   // ---- 3. A^{-1} = Linv^T * Linv  (k >= max(i, j) only)
   gemm<true, false, true>(st, n_pad, n_pad, n_pad, 1.f, Linv, n_pad, 0, Linv, n_pad, 0, 0.f, d_A, n_pad, 0, 1);
   B200_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// In-place EASE fit: the whole inverse and the finish inside the one n_pad x n_pad buffer (LAPACK potrf -> trtri -> lauum).
+// The only O(n^3) products with a K range of more than NB are split into K chunks of KW, so the packed operands of gemm
+// stay at 2 * n_pad * KW floats each instead of growing with n_pad^2.
+constexpr int KW = 4 * NB;
+
+// A[r, c] = 0 for c > r: the blocks above the diagonal still hold G after cholesky(), and the K-chunked trtri products
+// read the part of them inside a chunk (which must be the zeros of the triangular factor).  One CTA per row.
+__global__ void zero_upper_kernel(float* A, int n_pad) {
+  const long long r = blockIdx.x;
+  for (int c = (int)r + 1 + threadIdx.x; c < n_pad; c += blockDim.x) A[r * n_pad + c] = 0.f;
+}
+
+__global__ void zero_block_kernel(float* dst, int ldd, int rows, int cols) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (long long)rows * cols) return;
+  dst[(g / cols) * ldd + g % cols] = 0.f;
+}
+
+__global__ void get_diag_kernel(const float* __restrict__ A, int ldp, int n, float* d) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n) d[j] = A[(long long)j * ldp + j];
+}
+
+// In-place EASE finish on the lower triangle of P (stride ldp), d = diag P saved beforehand: B[i, j] = P[i, j] / (-d[j]),
+// B[j, j] = 0.  One CTA owns the 32 x 32 tile pair (I, J), (J, I) with I >= J: it reads the lower-triangle values of
+// tile (I, J) into shared memory, then writes both tiles (P symmetric: P[j, i] = P[i, j]).  No CTA reads a tile another
+// CTA writes.  grid = (T, T), T = ceil(n / 32); the CTAs with J > I exit.
+__global__ void __launch_bounds__(256) ease_finish_inplace_kernel(float* A, int ldp, int n, const float* __restrict__ d) {
+  __shared__ float t[32][33];
+  const int I = blockIdx.y, J = blockIdx.x;
+  if (J > I) return;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  for (int r = ty; r < 32; r += 8) {
+    const int i = I * 32 + r, j = J * 32 + tx;
+    t[r][tx] = (i < n && j < n && i >= j) ? A[(long long)i * ldp + j] : 0.f;
+  }
+  __syncthreads();
+  for (int r = ty; r < 32; r += 8) {
+    {  // tile (I, J)
+      const int i = I * 32 + r, j = J * 32 + tx;
+      if (i < n && j < n) A[(long long)i * ldp + j] = i == j ? 0.f : (i > j ? t[r][tx] : t[tx][r]) / (-d[j]);
+    }
+    if (I != J) {  // tile (J, I): P[i, j] = P[j, i] = t[tx][r]
+      const int i = J * 32 + r, j = I * 32 + tx;
+      if (i < n && j < n) A[(long long)i * ldp + j] = t[tx][r] / (-d[j]);
+    }
+  }
+}
+
+// 2. L := L^{-1} in place (LAPACK trtri, lower, non-unit), block columns right to left: X21 = -X22 L21 X11 with
+// X11 = inv_blocks[j] and X22 (the trailing block, already inverted) read in K chunks of KW.  The strict upper triangle
+// must be zero (zero_upper_kernel).  panel: n_pad x NB.
+void trtri_inplace(float* d_A, int n_pad, const float* inv_blocks, float* panel, cudaStream_t st) {
+  const int nblk = n_pad / NB;
+  for (int k = 0; k < nblk; ++k)  // the diagonal blocks become X_kk; the L_kk values are not read again
+    copy_block_kernel<<<div_up((long long)NB * NB, 256), 256, 0, st>>>(inv_blocks + (size_t)k * NB * NB, NB,
+                                                                       d_A + (long long)k * NB * n_pad + (long long)k * NB, n_pad, NB, NB);
+  count_launch(nblk);
+  for (int j = nblk - 2; j >= 0; --j) {
+    const int r0 = (j + 1) * NB, rem = n_pad - r0;
+    float* A21 = d_A + (long long)r0 * n_pad + (long long)j * NB;
+    // panel = L21 X11
+    gemm<false, false, false>(st, rem, NB, NB, 1.f, A21, n_pad, 0, inv_blocks + (size_t)j * NB * NB, NB, 0, 0.f, panel, NB, 0, 1);
+    // X21 = -X22 panel: the chunk of columns [k0, k0 + kw) of X22 only reaches rows >= k0 (X22 is lower triangular)
+    for (int k0 = r0; k0 < n_pad; k0 += KW) {
+      const int kw = std::min(KW, n_pad - k0);
+      gemm<false, false, false>(st, n_pad - k0, NB, kw, -1.f, d_A + (long long)k0 * n_pad + k0, n_pad, 0,
+                                panel + (long long)(k0 - r0) * NB, NB, 0, k0 == r0 ? 0.f : 1.f,
+                                d_A + (long long)k0 * n_pad + (long long)j * NB, n_pad, 0, 1);
+    }
+  }
+}
+
+// 3. P := X^T X in place on the lower triangle (LAPACK lauum), block rows top to bottom: for block row i,
+// A(i, 0:i+1) = X_ii^T A(i, 0:i+1) + X(i+1:, i)^T X(i+1:, 0:i+1).  The rows below i still hold X when row i is formed,
+// and the first product packs its operands before it overwrites them.  The blocks above the diagonal are not written
+// except the upper half of the diagonal blocks; only the lower triangle of P is meaningful.
+void lauum_inplace(float* d_A, int n_pad, cudaStream_t st) {
+  const int nblk = n_pad / NB;
+  for (int i = 0; i < nblk; ++i) {
+    const int N = (i + 1) * NB;
+    float* Ai0 = d_A + (long long)i * NB * n_pad;
+    gemm<true, false, false>(st, NB, N, NB, 1.f, Ai0 + (long long)i * NB, n_pad, 0, Ai0, n_pad, 0, 0.f, Ai0, n_pad, 0, 1);
+    for (int k0 = (i + 1) * NB; k0 < n_pad; k0 += KW) {
+      const int kw = std::min(KW, n_pad - k0);
+      const float* Ak0 = d_A + (long long)k0 * n_pad;
+      gemm<true, false, false>(st, NB, N, kw, 1.f, Ak0 + (long long)i * NB, n_pad, 0, Ak0, n_pad, 0, 1.f, Ai0, n_pad, 0, 1);
+    }
+  }
+}
+
+// Device bytes ease_inplace allocates besides the matrix: inv_blocks + panel, the packed operands of gemm (at most
+// 2 * n_pad * min(KW, n_pad) floats each), popularity counts, diag P, the compaction stage (NB rows of n) and the pivot flag.
+long long ease_inplace_workspace(int n) {
+  const long long n_pad = ((n + NB - 1) / NB) * (long long)NB;
+  return 4 * (2 * n_pad * NB + 2 * 2 * n_pad * std::min<long long>(KW, n_pad) + 2 * (long long)n + (long long)NB * n) + 4;
+}
+
+// Stages of ease_inplace on an SPD n_pad x n_pad matrix: 0 the Cholesky factor, 1 + L^{-1}, 2 + P = L^{-T} L^{-1}.
+// Returns the pivot position of cholesky() (0 when positive definite; later stages are skipped otherwise).
+int inverse_inplace(float* d_A, int n_pad, int last_stage, cudaStream_t st) {
+  DevBuf<float> inv_blocks((size_t)n_pad * NB), panel((size_t)n_pad * NB);
+  // the largest packed operand of the stages (K = NB, or a K chunk of at most min(KW, n_pad)): grow the workspaces once
+  const size_t pack = (size_t)2 * n_pad * std::min(KW, n_pad);
+  if (g_pack_a.n < pack || g_pack_b.n < pack) {
+    B200_CUDA(cudaStreamSynchronize(st));
+    if (g_pack_a.n < pack) g_pack_a.alloc(pack);
+    if (g_pack_b.n < pack) g_pack_b.alloc(pack);
+  }
+  const int info = cholesky(d_A, n_pad, inv_blocks.get(), panel.get(), st);
+  if (info != 0 || last_stage < 1) return info;
+  zero_upper_kernel<<<n_pad, 256, 0, st>>>(d_A, n_pad);
+  count_launch();
+  trtri_inplace(d_A, n_pad, inv_blocks.get(), panel.get(), st);
+  if (last_stage >= 2) lauum_inplace(d_A, n_pad, st);
+  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaStreamSynchronize(st));  // inv_blocks and panel are freed on return
   return 0;
 }
 
@@ -289,6 +421,83 @@ int b200_ease_from_gram_device(const float* d_G, int n_items, const int32_t* d_u
     B200_CUDA(cudaGetLastError());
     if (h_B) B200_CUDA(cudaMemcpyAsync(h_B, out, sizeof(float) * (size_t)n * n, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
+  });
+}
+
+}  // extern "C"
+
+extern "C" {
+
+/* In-place EASE_R fit: d_A [n_pad, n_pad] fp32 (n_pad = n_items rounded up to 128) holds X^T X in its top-left
+ * n_items x n_items block; on return its first n_items^2 floats are B as a contiguous [n_items, n_items] array. */
+int b200_ease_inplace_device(float* d_A, int n_items, const int32_t* d_urm_indices, int64_t nnz, float l2_norm, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(d_A && n_items > 0 && (nnz == 0 || d_urm_indices), "b200_ease_inplace: NULL argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int n = n_items, n_pad = ((n + NB - 1) / NB) * NB;
+    // identity padding: rows >= n and columns >= n are zero, then the diagonal (EASE_R_Recommender.py:62-63)
+    if (n_pad > n) {
+      zero_block_kernel<<<div_up((long long)n * (n_pad - n), 256), 256, 0, st>>>(d_A + n, n_pad, n, n_pad - n);
+      count_launch();
+      B200_CUDA(cudaMemsetAsync(d_A + (long long)n * n_pad, 0, sizeof(float) * (size_t)(n_pad - n) * n_pad, st));
+    }
+    {
+      DevBuf<int> cnt((size_t)n);
+      B200_CUDA(cudaMemsetAsync(cnt.get(), 0, sizeof(int) * (size_t)n, st));
+      if (nnz > 0) { col_count_kernel<<<sm_count() * 8, 256, 0, st>>>(d_urm_indices, nnz, cnt.get()); count_launch(); }
+      set_diag_kernel<<<div_up(n_pad, 256), 256, 0, st>>>(d_A, n, n_pad, cnt.get(), l2_norm);
+      count_launch();
+      B200_CUDA(cudaStreamSynchronize(st));
+    }
+    const int info = inverse_inplace(d_A, n_pad, 2, st);
+    if (info != 0) {
+      set_error("b200_ease_inplace: X^T X + diag is not positive definite (pivot %d of a diagonal block); the fp64 LU "
+                "inverse needs %lld more device bytes", info, 24LL * n_pad * n_pad);
+      throw CudaFail{B200_E_NOT_SPD};
+    }
+    {
+      DevBuf<float> d((size_t)n);
+      get_diag_kernel<<<div_up(n, 256), 256, 0, st>>>(d_A, n_pad, n, d.get());
+      const unsigned T = div_up(n, 32);
+      ease_finish_inplace_kernel<<<dim3(T, T), dim3(32, 8), 0, st>>>(d_A, n_pad, n, d.get());
+      count_launch(2);
+      B200_CUDA(cudaGetLastError());
+      B200_CUDA(cudaStreamSynchronize(st));
+    }
+    if (n_pad > n) {
+      // rows in order from stride n_pad to stride n through a stage of NB rows: the destination of rows [a, a + NB)
+      // ends at (a + NB) n <= (a + NB) n_pad, where the sources not yet staged begin
+      DevBuf<float> stage((size_t)NB * n);
+      for (int a = 0; a < n; a += NB) {
+        const int rows = std::min(NB, n - a);
+        copy_block_kernel<<<div_up((long long)rows * n, 256), 256, 0, st>>>(d_A + (long long)a * n_pad, n_pad, stage.get(), n, rows, n);
+        copy_block_kernel<<<div_up((long long)rows * n, 256), 256, 0, st>>>(stage.get(), n, d_A + (long long)a * n, n, rows, n);
+        count_launch(2);
+      }
+      B200_CUDA(cudaGetLastError());
+      B200_CUDA(cudaStreamSynchronize(st));
+    }
+  });
+}
+
+int b200_ease_inplace_workspace_bytes(int n_items, int64_t* bytes) {
+  return guarded([&] {
+    B200_REQUIRE(n_items > 0 && bytes, "b200_ease_inplace_workspace_bytes: n_items must be positive");
+    *bytes = ease_inplace_workspace(n_items);
+  });
+}
+
+/* TEST HOOK: the stages of the in-place inverse on an SPD [n_pad, n_pad] matrix (n_pad a multiple of 128):
+ * op 0 the Cholesky factor, op 1 then L^{-1} (trtri), op 2 then P = L^{-T} L^{-1} (lauum). */
+int b200_ease_inplace_debug_device(int op, float* d_A, int n_pad, void* stream) {
+  return guarded([&] {
+    B200_REQUIRE(op >= 0 && op <= 2 && d_A && n_pad > 0 && n_pad % NB == 0,
+                 "b200_ease_inplace_debug: op must be 0, 1 or 2 and n_pad a positive multiple of %d", NB);
+    const int info = inverse_inplace(d_A, n_pad, op, (cudaStream_t)stream);
+    if (info != 0) {
+      set_error("b200_ease_inplace_debug: matrix is not positive definite (pivot %d of a diagonal block)", info);
+      throw CudaFail{B200_E_NOT_SPD};
+    }
   });
 }
 

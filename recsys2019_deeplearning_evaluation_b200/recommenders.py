@@ -652,11 +652,46 @@ class SLIM_BPR_Cython(BaseItemSimilarityMatrixRecommender, Incremental_Training_
         self.W_sparse = sps.csr_matrix(W, dtype=np.float32)
 
 
+EASE_GRAM_SLAB_ROWS = 1024  # rows of X^T X the in-place EASE_R fit computes per similarity-kernel call
+# URM copies the in-place fit counts on the device: the similarity handle keeps the URM by rows and by columns with their
+# per-entry tables (at most three CSR-sized copies), and the recommender uploads its own CSR for the popularity counts
+EASE_URM_COPIES = 4
+
+
+def ease_urm_bytes(URM):
+    """Device bytes of one CSR copy of `URM` (int32 row pointers and column indices, fp32 values)."""
+    return 4 * (URM.shape[0] + 1) + 8 * int(URM.nnz)
+
+
+def ease_inplace_for_device(n_items, free_bytes, urm_bytes=0):
+    """Whether EASE_R_Recommender.fit takes the in-place path (b200_ease_inplace_device) on a device with `free_bytes`
+    free.  The default path's peak is X^T X and B (n_items^2 fp32 each) plus, inside b200_ease_from_gram_device, the padded
+    copy, Linv and the panel (3 n_pad^2) and the packed operands of the final Linv^T Linv product (2 n_pad^2):
+    4 * (2 n^2 + 5 n_pad^2) bytes.  The in-place path needs one n_pad^2 fp32 buffer, the call's workspace
+    (b200_ease_inplace_workspace_bytes), one Gram slab of EASE_GRAM_SLAB_ROWS rows and EASE_URM_COPIES times `urm_bytes`,
+    the device size of one CSR copy of the URM (ease_urm_bytes): the similarity handle's copies while the Gram is built,
+    then the recommender's own upload.  True only when the default path does not fit and the in-place path does: a
+    catalogue whose default footprint fits in `free_bytes` keeps the default path, and one that fits neither takes the
+    default path and fails with its out-of-memory error.  `free_bytes` is what the device reports: memory still held by
+    earlier work of the process (live tensors, the packed-operand workspaces an earlier default-path fit left grown,
+    2 n_pad^2 floats) counts as used."""
+    n = int(n_items)
+    n_pad = -(-n // 128) * 128
+    ws = ctypes.c_int64()
+    _lib.check(_lib.load().b200_ease_inplace_workspace_bytes(n, ctypes.byref(ws)))
+    default = 4 * (2 * n * n + 5 * n_pad * n_pad)
+    inplace = 4 * n_pad * n_pad + int(ws.value) + 4 * min(n, EASE_GRAM_SLAB_ROWS) * n + EASE_URM_COPIES * int(urm_bytes)
+    return default > int(free_bytes) and inplace <= int(free_bytes)
+
+
 class EASE_R_Recommender(BaseItemSimilarityMatrixRecommender):
     """EASE_R/EASE_R_Recommender.py:36-106.  Gram through the dense mode of the similarity kernel, inverse through the
     fp32 blocked-Cholesky kernels of csrc/ease.cu, or -- when G + diag is not positive definite, as on explicit ratings at
     small l2_norm -- through the fp64 pivoted LU of csrc/lu_inverse.cu; `topK=None` keeps the dense B on the device for
-    scoring.  A singular G raises np.linalg.LinAlgError("Singular matrix") like the reference's np.linalg.inv."""
+    scoring.  A singular G raises np.linalg.LinAlgError("Singular matrix") like the reference's np.linalg.inv.
+    A catalogue too large for that path's device memory but small enough for one n_pad^2 buffer is fitted in place
+    (ease_inplace_for_device, b200_ease_inplace_device); there an indefinite G + diag raises MemoryError, since the fp64
+    LU does not fit."""
     RECOMMENDER_NAME = "EASE_R_Recommender"
 
     def fit(self, topK=None, l2_norm=1e3, normalize_matrix=False, verbose=True):
@@ -670,15 +705,23 @@ class EASE_R_Recommender(BaseItemSimilarityMatrixRecommender):
             self.URM_train = sps.csr_matrix(X.dot(sps.diags(1.0 / cn)), dtype=np.float32)
             self._d_urm = None
         n = self.n_items
-        G = self._gram_device()
-        _, d_idx, _ = self._urm_device()
-        B = torch.empty((n, n), dtype=torch.float32, device=G.device)
-        try:
-            _lib.check(self._lib.b200_ease_from_gram_device(G.data_ptr(), n, d_idx.data_ptr(), self.URM_train.nnz, float(l2_norm),
-                                                            None, B.data_ptr(), _stream()))
-        except np.linalg.LinAlgError as e:
-            raise np.linalg.LinAlgError("Singular matrix") from e
-        del G
+        # the in-place path builds X^T X itself: a subclass with its own _gram_device (dist.make_sharded_ease, whose Gram
+        # is an all-reduce every rank must join) keeps the default path whatever its rank's free memory
+        own_gram = type(self)._gram_device is EASE_R_Recommender._gram_device
+        torch.cuda.empty_cache()  # blocks torch holds but does not use count as free
+        free_bytes = torch.cuda.mem_get_info()[0]
+        if own_gram and ease_inplace_for_device(n, free_bytes, ease_urm_bytes(self.URM_train)):
+            B = self._fit_inplace(float(l2_norm), free_bytes)
+        else:
+            G = self._gram_device()
+            _, d_idx, _ = self._urm_device()
+            B = torch.empty((n, n), dtype=torch.float32, device=G.device)
+            try:
+                _lib.check(self._lib.b200_ease_from_gram_device(G.data_ptr(), n, d_idx.data_ptr(), self.URM_train.nnz,
+                                                                float(l2_norm), None, B.data_ptr(), _stream()))
+            except np.linalg.LinAlgError as e:
+                raise np.linalg.LinAlgError("Singular matrix") from e
+            del G
         if topK is None:  # :75-78: dense W, scores = URM[users] . W
             self._d_B = B
             self.W_sparse = B.cpu().numpy()
@@ -686,6 +729,30 @@ class EASE_R_Recommender(BaseItemSimilarityMatrixRecommender):
             from .slim_bpr_epoch import dense_topk_to_sparse
             self._d_B = None
             self.W_sparse = sps.csr_matrix(dense_topk_to_sparse(B, n, topK, along_columns=True, mode=0), dtype=np.float32)
+
+    def _fit_inplace(self, l2_norm, free_bytes):
+        """B as an [n_items, n_items] view of one [n_pad, n_pad] fp32 tensor: X^T X is written into it slab by slab (the
+        dense mode of the similarity kernel, EASE_GRAM_SLAB_ROWS rows at a time), the similarity handle is freed, and
+        b200_ease_inplace_device inverts and finishes in place."""
+        import torch
+        from .similarity import Compute_Similarity_Cython
+        n = self.n_items
+        n_pad = -(-n // 128) * 128
+        A = torch.empty((n_pad, n_pad), dtype=torch.float32, device=torch.device("cuda", torch.cuda.current_device()))
+        sim = Compute_Similarity_Cython(self.URM_train, shrink=0, topK=n if n > 2048 else 0, normalize=False, similarity="cosine")
+        for lo in range(0, n, EASE_GRAM_SLAB_ROWS):
+            hi = min(n, lo + EASE_GRAM_SLAB_ROWS)
+            A[lo:hi, :n].copy_(sim.compute_dense_device(lo, hi))  # symmetric: orientation is irrelevant
+        sim._dealloc()
+        _, d_idx, _ = self._urm_device()
+        try:
+            _lib.check(self._lib.b200_ease_inplace_device(A.data_ptr(), n, d_idx.data_ptr(), self.URM_train.nnz, l2_norm, _stream()))
+        except _lib.NotPositiveDefiniteError as e:
+            lu_bytes = 4 * 2 * n * n + 24 * n_pad * n_pad
+            raise MemoryError("EASE_R_Recommender: X^T X + diag is not positive definite for {} items (explicit ratings at a "
+                              "small l2_norm); its fp64 LU inverse needs {} bytes of device memory and {} are free".format(
+                                  n, lu_bytes, int(free_bytes))) from e
+        return A.view(-1)[:n * n].view(n, n)
 
     def _gram_device(self, rows=None):
         """X^T X (EASE_R_Recommender.py:55-56) as a dense [n_items, n_items] fp32 CUDA tensor, from all users or from the
