@@ -387,6 +387,25 @@ int b200_cand_topn_device(const int32_t* d_users, int n_block, const int32_t* d_
  * ------------------------------------------------------------------------------------------------ */
 int b200_slim_enet_device(const float* d_G, const float* d_diag, int n_items, int64_t n_users, double l1_ratio, double alpha,
                           int positive_only, int max_iter, float tol, float* d_coef_T, int32_t* d_n_iter, void* stream);
+/* The same solve with positive_only on a non-negative URM, against a sparse Gram matrix and with no n_items^2 buffer:
+ * d_gram_ptr [n_items + 1] (int64), d_gram_col (ascending per row) and d_gram_val hold X^T X as a CSR WITHOUT its
+ * diagonal (b200_gram_slab_compact_device).  Item j visits only the support of row j; the coordinates outside it never
+ * act when G >= 0 and w >= 0, so the same coordinates are applied in the same order as above.  Instead of a coefficient
+ * line, item j's min(nnz - 1, topK) largest non-zero weights (ties to the ascending index) go to row j of the
+ * [n_items, topK] table d_top_idx / d_top_val (-1 / 0 past d_top_cnt[j]), as b200_dense_topk_device mode 2 would select
+ * them from d_coef_T.  Device memory besides the arguments: b200_slim_enet_workspace_bytes. */
+int b200_slim_enet_sparse_device(const int64_t* d_gram_ptr, const int32_t* d_gram_col, const float* d_gram_val, const float* d_diag,
+                                 int n_items, int64_t n_users, double l1_ratio, double alpha, int max_iter, float tol, int topK,
+                                 int32_t* d_top_idx, float* d_top_val, int32_t* d_top_cnt, int32_t* d_n_iter, void* stream);
+/* The workspace both solves allocate on a device with n_sms SMs: the per-CTA vectors w, H and q when 3 * n_items * 4 bytes
+ * exceed 200 KB of shared memory (min(n_items, n_sms) * 3 * n_items floats), else 0. */
+int b200_slim_enet_workspace_bytes(int n_items, int n_sms, int64_t* bytes);
+/* One slab of rows [row0, row0 + rows) of a dense [n, n] Gram matrix (d_slab, [rows, n] row-major) as CSR rows, without
+ * the diagonal.  Count pass (d_row_nnz non-NULL, d_row_start NULL): d_row_nnz[r] = the off-diagonal non-zeros of row r.
+ * Fill pass (d_row_start [rows + 1] the rows' starts, d_row_nnz NULL): their ascending column ids and values go to
+ * d_col / d_val at those positions. */
+int b200_gram_slab_compact_device(const float* d_slab, int rows, int n, int row0, int64_t* d_row_nnz, const int64_t* d_row_start,
+                                  int32_t* d_col, float* d_val, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K5: EASE^R closed form  (hot path iii)

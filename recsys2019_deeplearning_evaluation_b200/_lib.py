@@ -72,6 +72,12 @@ SIGNATURES = {
     "b200_slim_tree_cells": (ctypes.c_int, [c_void, ctypes.POINTER(ctypes.c_int64)]),
     "b200_slim_enet_device": (ctypes.c_int, [c_void, c_void, ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_double, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_float, c_void, c_void, c_void]),
+    "b200_slim_enet_sparse_device": (ctypes.c_int, [c_void, c_void, c_void, c_void, ctypes.c_int, ctypes.c_int64, ctypes.c_double,
+                                                    ctypes.c_double, ctypes.c_int, ctypes.c_float, ctypes.c_int, c_void, c_void, c_void,
+                                                    c_void, c_void]),
+    "b200_slim_enet_workspace_bytes": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, c_i64_p]),
+    "b200_gram_slab_compact_device": (ctypes.c_int, [c_void, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_void, c_void, c_void, c_void,
+                                                     c_void]),
     "b200_asysvd_create": (ctypes.c_int, [ctypes.POINTER(c_void), ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, c_void, c_void, c_void,
                                           ctypes.c_int, ctypes.c_double, ctypes.c_float, ctypes.c_int, ctypes.c_float, ctypes.c_float,
                                           ctypes.c_float, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void, c_void,

@@ -25,12 +25,6 @@ typedef unsigned long long u64;
 constexpr int THREADS = 256;
 constexpr int BINS = 2048;
 
-// orderable() maps +NaN above +inf and -NaN below -inf; every NaN is moved to one end instead, by mode
-__device__ __forceinline__ u64 line_key(float v, int qi, bool nan_high) {
-  const unsigned o = v != v ? (nan_high ? 0xFFFFFFFFu : 0u) : orderable(v);
-  return (((u64)o) << 32) | (u64)(0xFFFFFFFFu - (unsigned)qi);
-}
-
 // SPARSE: line l is the segment [ptr[l], ptr[l+1]) of (sidx, M); its cells are the stored entries and the implicit
 // zeros of a length-n_inner line.  Residency: 8 CTAs per SM for compressed lines (32 registers: the grid of sm_count * 8
 // is resident at once), 6 for dense ones (40 registers).
@@ -67,7 +61,7 @@ __global__ void __launch_bounds__(THREADS, SPARSE ? 8 : 6)
     const int nzero = n_inner_dense - nnz;
     int keep;  // how many non-zero cells survive
     if (mode == 0) keep = min(K, nnz);                                           // similarityMatrixTopK
-    else if (mode == 2) keep = max(0, min(K, nnz - 1));                          // SLIMElasticNetRecommender.py:103
+    else if (mode == 2) keep = drop_last_keep(K, nnz);                           // SLIMElasticNetRecommender.py:103
     else keep = min(K, npos) + min(nneg + nnan, max(0, K - npos - nzero));        // zeros outrank negatives, NaN last
     keep = min(keep, K);  // nzero < 0 when a compressed line holds more entries than n
     u64 thr = 0;

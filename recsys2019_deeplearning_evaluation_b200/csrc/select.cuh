@@ -26,6 +26,17 @@ __device__ __forceinline__ u64 orderable(double v) {
   return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
 }
 
+// The key of value v at index qi in a line of the top-K selections (dense_topk.cu, the sparse SLIM ElasticNet solve): the
+// value bits, then ~index so that ties go to the ascending index.  orderable() maps +NaN above +inf and -NaN below -inf;
+// every NaN is moved to one end instead, by mode.
+__device__ __forceinline__ u64 line_key(float v, int qi, bool nan_high) {
+  const unsigned o = v != v ? (nan_high ? 0xFFFFFFFFu : 0u) : orderable(v);
+  return (((u64)o) << 32) | (u64)(0xFFFFFFFFu - (unsigned)qi);
+}
+
+// How many of a line's nnz non-zero values SLIM ElasticNet keeps: min(nnz - 1, K), SLIMElasticNetRecommender.py:103
+__device__ __forceinline__ int drop_last_keep(int K, int nnz) { return max(0, min(K, nnz - 1)); }
+
 // What the select needs of a key type: its width, the digit nb bits wide at bit sh, the test against the prefix fixed so
 // far, and fixing one more digit of the prefix.
 template <typename Key> struct KeyBits;

@@ -570,12 +570,83 @@ class MatrixFactorization_AsySVD_Cython(_MatrixFactorization_Cython):
         return USER_factors
 
 
+def slim_enet_dense_bytes(n_items, topK, n_sms, urm_bytes=0):
+    """Device bytes of SLIMElasticNetRecommender.fit on the dense path, summed over its buffers: the Gram matrix X^T X and
+    coefT (n_items^2 fp32 each), the solve's workspace beyond 200 KB of shared-memory vectors
+    (b200_slim_enet_workspace_bytes on a device with `n_sms` SMs), the [n_items, min(topK, n_items)] top-K table (int32
+    index and fp32 value per cell, an int32 count per line) and EASE_URM_COPIES times `urm_bytes` (ease_urm_bytes), the URM
+    copies of the similarity handle that builds the Gram matrix."""
+    n = int(n_items)
+    ws = ctypes.c_int64()
+    _lib.check(_lib.load().b200_slim_enet_workspace_bytes(n, int(n_sms), ctypes.byref(ws)))
+    k = min(int(topK), n)
+    return 8 * n * n + int(ws.value) + 8 * n * k + 4 * n + EASE_URM_COPIES * int(urm_bytes)
+
+
+def slim_enet_sparse_for_device(n_items, free_bytes, positive_only, nonnegative, topK, n_sms, urm_bytes=0):
+    """Whether SLIMElasticNetRecommender.fit solves against a sparse Gram matrix (b200_slim_enet_sparse_device): only when
+    the dense path's footprint (slim_enet_dense_bytes) exceeds `free_bytes`, positive_only is set and the URM has no
+    negative value -- the conditions under which a coordinate outside the support of its item's row of X^T X never acts.
+    Every other fit keeps the dense path, a catalogue too large for it included (with its out-of-memory error).  Whether
+    the sparse Gram itself fits is only known once its non-zeros are counted; the fit raises MemoryError when it does
+    not."""
+    if not (positive_only and nonnegative):
+        return False
+    return slim_enet_dense_bytes(n_items, topK, n_sms, urm_bytes) > int(free_bytes)
+
+
+def gram_csr_device(URM):
+    """X^T X of `URM` as a CSR on the device WITHOUT its diagonal: (row_ptr int64 [n_items + 1], col int32 ascending per
+    row, val fp32).  The dense mode of the similarity kernel computes it EASE_GRAM_SLAB_ROWS rows at a time, twice: the first
+    pass counts each row's non-zeros, one host read gives nnz, the second recomputes the slabs and compacts them
+    (b200_gram_slab_compact_device).  The values are the dense Gram matrix's bits; the peak is the CSR plus one slab.
+    Raises MemoryError when the CSR and the solve's workspace do not fit in the free device memory."""
+    import torch
+    from .similarity import Compute_Similarity_Cython
+    lib = _lib.load()
+    n = URM.shape[1]
+    dev = torch.device("cuda", torch.cuda.current_device())
+    sim = Compute_Similarity_Cython(URM, shrink=0, topK=n if n > 2048 else 0, normalize=False, similarity="cosine")
+    try:
+        ptr = torch.zeros((n + 1,), dtype=torch.int64, device=dev)
+        for lo in range(0, n, EASE_GRAM_SLAB_ROWS):
+            hi = min(n, lo + EASE_GRAM_SLAB_ROWS)
+            S = sim.compute_dense_device(lo, hi)  # symmetric: orientation is irrelevant
+            _lib.check(lib.b200_gram_slab_compact_device(S.data_ptr(), hi - lo, n, lo, ptr[lo + 1:].data_ptr(), None, None, None,
+                                                         _stream()))
+            del S
+        ptr = torch.cumsum(ptr, 0)
+        nnz = int(ptr[-1])
+        ws = ctypes.c_int64()
+        _lib.check(lib.b200_slim_enet_workspace_bytes(n, torch.cuda.get_device_properties(dev).multi_processor_count, ctypes.byref(ws)))
+        need = 8 * nnz + int(ws.value)
+        torch.cuda.empty_cache()
+        free = torch.cuda.mem_get_info()[0]
+        if need > free:
+            raise MemoryError("SLIMElasticNetRecommender: X^T X of {} items has {} non-zeros off its diagonal; its CSR and the "
+                              "solve's workspace need {} bytes of device memory and {} are free".format(n, nnz, need, int(free)))
+        col = torch.empty((max(nnz, 1),), dtype=torch.int32, device=dev)
+        val = torch.empty((max(nnz, 1),), dtype=torch.float32, device=dev)
+        for lo in range(0, n, EASE_GRAM_SLAB_ROWS):
+            hi = min(n, lo + EASE_GRAM_SLAB_ROWS)
+            S = sim.compute_dense_device(lo, hi)
+            _lib.check(lib.b200_gram_slab_compact_device(S.data_ptr(), hi - lo, n, lo, None, ptr[lo:].data_ptr(), col.data_ptr(),
+                                                         val.data_ptr(), _stream()))
+            del S
+    finally:
+        sim._dealloc()
+    return ptr, col, val
+
+
 class SLIMElasticNetRecommender(BaseItemSimilarityMatrixRecommender):
     """SLIM_ElasticNet/SLIMElasticNetRecommender.py:20-148.  The reference fits one scikit-learn ElasticNet per item on the URM
     with that item's column zeroed (recomputing X^T X each time); here the Gram matrix is formed once on the device (the dense
     mode of the similarity kernel, as for EASE_R) and csrc/slim_enet.cu runs the Gram-matrix coordinate descent of all items,
     one CTA per item, with sklearn's stopping rule in cyclic coordinate order (the reference's order is random and unseeded:
-    its own runs differ from each other by as much as this differs from them, tests/test_oracle_elasticnet.py)."""
+    its own runs differ from each other by as much as this differs from them, tests/test_oracle_elasticnet.py).
+    A catalogue whose dense footprint (X^T X and the coefficients, 8 n_items^2 bytes) exceeds the free device memory is
+    solved against a sparse X^T X when positive_only is set and the URM has no negative value (slim_enet_sparse_for_device):
+    the same coordinate descent over each item's support, with the top-K taken inside the solve."""
     RECOMMENDER_NAME = "SLIMElasticNetRecommender"
 
     def fit(self, l1_ratio=0.1, alpha=1.0, positive_only=True, topK=100, max_iter=100, tol=1e-4):
@@ -584,8 +655,14 @@ class SLIMElasticNetRecommender(BaseItemSimilarityMatrixRecommender):
             self.RECOMMENDER_NAME, l1_ratio)  # :43
         self.l1_ratio, self.positive_only, self.topK = l1_ratio, positive_only, topK
         n = self.n_items
-        G = EASE_R_Recommender._gram_device(self)  # the same X^T X (it only reads URM_train / n_items)
         X = self.URM_train
+        torch.cuda.empty_cache()  # blocks torch holds but does not use count as free
+        n_sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+        if slim_enet_sparse_for_device(n, torch.cuda.mem_get_info()[0], positive_only, bool((X.data >= 0).all()), topK, n_sms,
+                                       ease_urm_bytes(X)):
+            self._fit_sparse(float(l1_ratio), float(alpha), int(topK), int(max_iter), float(tol))
+            return
+        G = EASE_R_Recommender._gram_device(self)  # the same X^T X (it only reads URM_train / n_items)
         diag = torch.from_numpy(np.asarray(X.multiply(X).sum(axis=0), dtype=np.float32).ravel()).to(G.device)
         coefT = torch.empty((n, n), dtype=torch.float32, device=G.device)
         self._n_iter = torch.empty((n,), dtype=torch.int32, device=G.device)
@@ -598,6 +675,27 @@ class SLIMElasticNetRecommender(BaseItemSimilarityMatrixRecommender):
         # column j of W_sparse (:119-121)
         T = dense_topk_to_sparse(coefT, n, min(int(topK), n), along_columns=False, mode=2)
         self.W_sparse = sps.csr_matrix(T.T, dtype=np.float32)
+
+    def _fit_sparse(self, l1_ratio, alpha, topK, max_iter, tol):
+        """The fit against gram_csr_device's sparse X^T X: b200_slim_enet_sparse_device writes each item's top-K into an
+        [n_items, min(topK, n_items)] table, whose line j is column j of W_sparse."""
+        import torch
+        from .similarity import topk_table_to_csr
+        n = self.n_items
+        X = self.URM_train
+        ptr, col, val = gram_csr_device(X)
+        dev = ptr.device
+        diag = torch.from_numpy(np.asarray(X.multiply(X).sum(axis=0), dtype=np.float32).ravel()).to(dev)
+        k = min(topK, n)
+        idx = torch.empty((n, k), dtype=torch.int32, device=dev)
+        vals = torch.empty((n, k), dtype=torch.float32, device=dev)
+        cnt = torch.empty((n,), dtype=torch.int32, device=dev)
+        self._n_iter = torch.empty((n,), dtype=torch.int32, device=dev)
+        _lib.check(self._lib.b200_slim_enet_sparse_device(ptr.data_ptr(), col.data_ptr(), val.data_ptr(), diag.data_ptr(), n,
+                                                          self.n_users, l1_ratio, alpha, max_iter, tol, k, idx.data_ptr(),
+                                                          vals.data_ptr(), cnt.data_ptr(), self._n_iter.data_ptr(), _stream()))
+        del ptr, col, val
+        self.W_sparse = topk_table_to_csr(n, k, idx, vals, cnt)  # W[idx, line] = val
 
 
 class SLIM_BPR_Cython(BaseItemSimilarityMatrixRecommender, Incremental_Training_Early_Stopping):
@@ -652,7 +750,7 @@ class SLIM_BPR_Cython(BaseItemSimilarityMatrixRecommender, Incremental_Training_
         self.W_sparse = sps.csr_matrix(W, dtype=np.float32)
 
 
-EASE_GRAM_SLAB_ROWS = 1024  # rows of X^T X the in-place EASE_R fit computes per similarity-kernel call
+EASE_GRAM_SLAB_ROWS = 1024  # rows of X^T X the in-place EASE_R fit and gram_csr_device compute per similarity-kernel call
 # URM copies the in-place fit counts on the device: the similarity handle keeps the URM by rows and by columns with their
 # per-entry tables (at most three CSR-sized copies), and the recommender uploads its own CSR for the popularity counts
 EASE_URM_COPIES = 4
