@@ -1266,6 +1266,17 @@ bool k1d_pair_gate(b200_sim_s* h, const int* d_cnt, cudaStream_t st) {
   }
 }
 
+// The dynamic shared-memory limit is an attribute of the kernel, shared by every handle with the same formula and counter
+// type, each of which launches with a size of its own: raise it to this handle's size, never lower it (a handle built
+// later for a smaller catalogue would otherwise break the launches of a larger one still alive).
+template <typename Kernel>
+void raise_smem_limit(Kernel kernel, size_t bytes) {
+  cudaFuncAttributes fa{};
+  B200_CUDA(cudaFuncGetAttributes(&fa, kernel));
+  if ((size_t)fa.maxDynamicSharedSizeBytes < bytes)
+    B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+}
+
 void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, const float* h_data,
            const float* h_row_weights, cudaStream_t st) {
   const int n_rows = h->n_rows, n_cols = h->n_cols;
@@ -1457,7 +1468,7 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
   h->win = win;
   h->acc_words = std::max(win / cpw, SBINS) + 4;  // + the dummy cell the padded row segments point at (cell index `win`)
   h->smem_bytes = (size_t)h->acc_words * 4 + (size_t)cap * 8 + staging + (size_t)n_win * (MAXTILES + 1) * 4;
-  B200_CUDA(cudaFuncSetAttribute(kernel_for(h->formula, h->binary, h->pack), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_bytes));
+  raise_smem_limit(kernel_for(h->formula, h->binary, h->pack), h->smem_bytes);
   h->tileB.alloc((size_t)n_win * (MAXTILES + 1));
   tile_bounds_kernel<<<div_up((long long)n_win * (MAXTILES + 1), 128), 128, 0, st>>>(h->BN.get(), n_cols, n_win, win, tile, h->tileB.get());
   count_launch();
@@ -1586,7 +1597,7 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
       B200_CUDA(cudaMemcpyAsync(h->h_old2new.data(), h->old2new.get(), sizeof(int) * (size_t)n_cols, cudaMemcpyDeviceToHost, st));
       B200_CUDA(cudaMemcpyAsync(h->h_csc_ptr.data(), h->csc_ptr.get(), sizeof(int) * ((size_t)n_cols + 1), cudaMemcpyDeviceToHost, st));
       B200_CUDA(cudaStreamSynchronize(st));
-      B200_CUDA(cudaFuncSetAttribute(k1d_kernel_for(h->formula), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem1_bytes));
+      raise_smem_limit(k1d_kernel_for(h->formula), h->smem1_bytes);
       // the whole unified L1 / shared array as shared memory: without it the driver sizes the carve-out for ONE block and the
       // second CTA of an SM never becomes resident
       B200_CUDA(cudaFuncSetAttribute(k1d_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
@@ -1603,7 +1614,7 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
           h->ctas_up = ctas;
       if (h->ctas_up > 0 && !k1d_pair_gate(h, cnt_new.get(), st)) h->ctas_up = 0;
       if (h->ctas_up > 0) {
-        B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_up_bytes));
+        raise_smem_limit(sim_k1d_upper_kernel, h->smem_up_bytes);
         B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         // the launch passes this handle's size; the limit is the same for every handle that shares the kernel
         h->smem_sel_bytes = (size_t)S_WARPS * k1d_select_warp_bytes(h->sel_cap);
@@ -1919,11 +1930,12 @@ int b200_sim_compute_peers_device(b200_sim_t h, int start_col, int end_col, int 
 
 int b200_sim_compute_dense_device(b200_sim_t h, int start_col, int end_col, float* d_out, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(h != nullptr && d_out != nullptr, "b200_sim_compute_dense: NULL argument");
+    B200_REQUIRE(h != nullptr, "b200_sim_compute_dense: NULL handle");
     B200_REQUIRE(h->formula != F_EUCLID, "b200_sim_compute_dense: the euclidean similarity has no dense output mode");
     B200_REQUIRE(0 <= start_col && start_col <= end_col && end_col <= h->n_cols, "b200_sim_compute_dense: bad column range [%d,%d)",
                  start_col, end_col);
-    if (end_col == start_col) return;
+    if (end_col == start_col) return;  // an empty range has an empty output, which may well be a NULL pointer
+    B200_REQUIRE(d_out != nullptr, "b200_sim_compute_dense: NULL output");
     cudaStream_t st = (cudaStream_t)stream;
     B200_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * (size_t)(end_col - start_col) * (size_t)h->n_cols, st));
     launch_topk(h, start_col, end_col, nullptr, nullptr, nullptr, d_out, st);

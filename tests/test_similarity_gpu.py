@@ -282,3 +282,18 @@ def test_k1c_empty_columns_topk_exceeds_candidates(force_k1c):
     X.eliminate_zeros()
     W, sim, _ = _check(X, topK=100, shrink=0, similarity="cosine")
     assert W[:, 5].nnz == 0 and W[5, :].nnz == 0
+
+
+def test_k1c_handle_built_later_for_fewer_columns(force_k1c):
+    """Two live handles launch the same nibble and window kernels, the one built later with less shared memory (fewer
+    columns): each kernel's shared-memory limit is the launching handle's, so the first handle still computes."""
+    X1 = synth_urm(700, 3000, 0.01, seed=3, values="binary")
+    X2 = synth_urm(700, 300, 0.04, seed=3, values="binary")
+    kw = dict(topK=25, shrink=7, similarity="cosine")
+    sim1 = _gpu_cls()(X1, **kw)
+    sim2 = _gpu_cls()(X2, **kw)
+    assert _k1c_info(sim1)[0] == 1 and _k1c_info(sim2)[0] == 1
+    W1 = sim1.compute_similarity()
+    check_topk_against_dense(W1, SimilarityOracle(X1, **kw), np.arange(0, 3000, 7), rtol=RTOL)
+    W2 = sim2.compute_similarity()
+    check_topk_against_dense(W2, SimilarityOracle(X2, **kw), np.arange(300), rtol=RTOL)
