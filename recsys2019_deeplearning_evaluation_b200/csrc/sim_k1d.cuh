@@ -403,8 +403,9 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
 // on top of the upper pass, so the path only pays when the select kernel can decide nearly every column.
 
 // Launch shape of the upper pass: U_CTAS CTAs of U_THREADS threads per SM (half-window counters: 50 KB at 200 K columns),
-// so that several columns per SM are in different phases, and U_STEPS loads of 32 chunks in flight per warp.  The -D
-// overrides are for A/B builds (tools/build_variant.py).
+// so that several columns per SM are in different phases, and loads of 32 chunks issued U_STEPS at a time per warp, double
+// buffered: the next U_STEPS are in flight while the current ones are counted.  The -D overrides are for A/B builds
+// (tools/build_variant.py).
 #ifndef B200_U_THREADS
 #define B200_U_THREADS 256
 #endif
@@ -412,7 +413,7 @@ __global__ void __launch_bounds__(D_THREADS, 2) sim_k1d_kernel(const KParams p) 
 #define B200_U_CTAS 4
 #endif
 #ifndef B200_U_STEPS
-#define B200_U_STEPS 4
+#define B200_U_STEPS 3
 #endif
 #ifndef B200_U_STAGE
 #define B200_U_STAGE 1024
@@ -433,8 +434,20 @@ constexpr int OWN_SPILLED = (int)0x80000000u;
 
 struct K1DUpShared {
   int item, nibsum, ncand, nst;
+  int4 wi;  // worklist_up[item], fetched by thread 0 while the previous column was counted
   unsigned long long base;
 };
+
+// One gathered entry: cell t of the window is counted iff `ok`.  Counting is straight-line code: every entry issues one
+// fire-and-forget shared reduction on a 32-bit shared address (acc_s: the counters' base in the shared window), and an
+// entry that does not count adds 0 to word `lane` (distinct banks, inside acc + stage: U_STAGE >= 32).  Not a predicated
+// reduction: ptxas turns that back into a branch region per entry (BSSY / BRA / BSYNC) with the address math inside.
+static_assert(U_STAGE >= 32, "an entry that does not count adds 0 to shared word `lane`");
+__device__ __forceinline__ void k1d_up_count(unsigned acc_s, int lane, unsigned t, bool ok) {
+  // word t / 8, nibble t % 8: 1 << ((t << 2) & 31), the wrap of the funnel shift
+  const unsigned word = ok ? t >> 3 : (unsigned)lane, inc = ok ? __funnelshift_l(0u, 1u, t << 2) : 0u;
+  asm volatile("red.shared.add.u32 [%0], %1;" :: "r"(acc_s + (word << 2)), "r"(inc) : "memory");
+}
 
 __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const KParams p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -444,50 +457,79 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
   const int W = k1d_upper_words(n);
   unsigned* acc = reinterpret_cast<unsigned*>(smem_raw);
   unsigned* stage = acc + W;
+  const unsigned acc_s = (unsigned)__cvta_generic_to_shared(acc);
   for (int i = tid; i < W; i += U_THREADS) acc[i] = 0u;
   if (blockIdx.x == 0 && tid == 0 && p.fail_every > 0) atomicExch(p.pair_fail, 1);  // test hook: exercises the fallback
   long long prof_t = p.prof ? clock64() : 0;
+  // Work items are taken one column ahead: thread 0 takes the next one (and reads the fallback flag alongside) while the
+  // current column gathers, and loads its work item before the sweep, so a column starts with its descriptor loads.  Once
+  // the call has fallen back, the remaining columns are not worth gathering: the CTA stops.
+  if (tid == 0) {
+    const int it = atomicAdd(p.counter, 1);
+    us.item = *(volatile int*)p.pair_fail ? p.n_range : it;
+    if (us.item < p.n_range) us.wi = __ldg(p.worklist_up + us.item);
+    us.nibsum = 0; us.ncand = 0; us.nst = 0;
+  }
+  __syncthreads();
 
   for (;;) {
-    __syncthreads();
-    if (tid == 0) {
-      // once the call has fallen back, the remaining columns are not worth gathering
-      us.item = *(volatile int*)p.pair_fail ? p.n_range : atomicAdd(p.counter, 1);
-      us.nibsum = 0; us.ncand = 0; us.nst = 0;
-    }
-    __syncthreads();
+    // us.item / us.wi: written by thread 0 before a barrier (the one above, or the previous column's sweep barrier), and
+    // rewritten only after this column's gather barrier
     const int item = us.item;
     if (item >= p.n_range) break;
-    const int4 wi = __ldg(p.worklist_up + item);
+    const int4 wi = us.wi;
     const int col = wi.x, adds = wi.y, cs = wi.z, ce = wi.w;  // adds: the increments of the column's windows
     const int size_c = k1d_window_size(n, col);
+    int it_next = 0, failed = 0;
+    if (tid == 0) {
+      it_next = atomicAdd(p.counter, 1);
+      failed = *(volatile int*)p.pair_fail;
+    }
 
     // ---------------- gather over the row windows: cell t = j' - col - 1 of doubled-row index j', counted iff t < size_c,
     // which masks the entries of the first and last chunk outside the window; a gap of 0 is padding.  A window is half a
     // row on average (C5: ~8 chunks), so one row per warp load would leave most lanes idle and issue as many
     // loads and atomic instructions as the whole row; instead the 32 windows of a batch are one stream of chunks, every
     // lane of every load busy.  Rows with chunks sit compacted in the low lanes; lane r holds row r's [beg, end) in the
-    // stream, and the row of stream position f is the number of rows that end at or before f.
-    for (int k0 = cs + warp * 32; k0 < ce; k0 += U_WARPS * 32) {
-      const int nrows = min(32, ce - k0);
-      int2 seg = make_int2(0, 0);
-      if (lane < nrows) seg = __ldg(p.csc_win + k0 + lane);
-      const unsigned nz = __ballot_sync(0xffffffffu, seg.y > 0);
-      const int nr = __popc(nz);
-      const int src = lane < nr ? (int)__fns(nz, 0, lane + 1) : 0;
-      const int rstart = __shfl_sync(0xffffffffu, seg.x, src);
-      const int sy = __shfl_sync(0xffffffffu, seg.y, src);
-      const int rn = lane < nr ? sy : 0;
-      int end = rn;
+    // stream, and the row of stream position f is the number of rows that end at or before f.  A warp's batches are one
+    // pipeline: the loads of its next U_STEPS steps (and the descriptors of its next batch) are in flight while it counts
+    // the current ones.  A position past the batch's stream loads nothing and decodes as {col, no gaps}: t = -1, never
+    // counted.
+    {
+      const unsigned sz = (unsigned)size_c;
+      int k0 = cs + warp * 32;
+      const auto desc = [&](int k) {
+        int2 s = make_int2(0, 0);
+        if (k + lane < ce) s = __ldg(p.csc_win + k + lane);
+        return s;
+      };
+      int rstart = 0, beg = 0, end = 0, nr = 0, total = 0, b0 = 0;  // the open batch, and its next stream position
+      const auto open = [&](int2 seg) {
+        const unsigned nz = __ballot_sync(0xffffffffu, seg.y > 0);
+        nr = __popc(nz);
+        const int src = lane < nr ? (int)__fns(nz, 0, lane + 1) : 0;
+        rstart = __shfl_sync(0xffffffffu, seg.x, src);
+        const int sy = __shfl_sync(0xffffffffu, seg.y, src);
+        const int rn = lane < nr ? sy : 0;
+        end = rn;
 #pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, end, off);
-        if (lane >= off) end += t;
+        for (int off = 1; off < 32; off <<= 1) {
+          const int t = __shfl_up_sync(0xffffffffu, end, off);
+          if (lane >= off) end += t;
+        }
+        beg = end - rn;
+        total = __shfl_sync(0xffffffffu, end, 31);
+        b0 = 0;
+      };
+      bool live = k0 < ce;  // the warp has steps left to issue
+      int2 seg_next = make_int2(0, 0);
+      if (live) {
+        const int2 seg = desc(k0);
+        seg_next = desc(k0 + U_WARPS * 32);
+        open(seg);
       }
-      const int beg = end - rn;
-      const int total = __shfl_sync(0xffffffffu, end, 31);
-      for (int b0 = 0; b0 < total; b0 += 32 * U_STEPS) {
-        int4 v[U_STEPS];
+      // loads the next U_STEPS steps of the stream into v, then moves on to the next batch if this one is done
+      const auto issue = [&](int4 (&v)[U_STEPS]) {
 #pragma unroll
         for (int q = 0; q < U_STEPS; ++q) {
           const int base = b0 + 32 * q, f = base + lane;
@@ -495,22 +537,49 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
           const unsigned ends = __reduce_or_sync(0xffffffffu, (lane < nr && end > base && end - base < 32) ? (1u << (end - base)) : 0u);
           const int row = (__popc(before) + __popc(ends & ((2u << lane) - 1u))) & 31;
           const int rb = __shfl_sync(0xffffffffu, beg, row), rs = __shfl_sync(0xffffffffu, rstart, row);
-          if (f < total) v[q] = __ldg(p.csr_idx1 + (size_t)rs + (f - rb));
+          v[q] = f < total ? __ldg(p.csr_idx1 + (size_t)rs + (f - rb)) : make_int4(col, 0, 0, 0);
         }
-#pragma unroll
-        for (int q = 0; q < U_STEPS; ++q) {
-          if (b0 + 32 * q + lane < total) {
-            unsigned t = (unsigned)(v[q].x - col - 1);
-            if (t < (unsigned)size_c) atomicAdd(&acc[t >> 3], 1u << ((t & 7) << 2));
-#pragma unroll
-            for (int e = 0; e < K1D_GAPS; ++e) {
-              const unsigned g = (unsigned)k1d_gap(v[q], e);
-              t += g;
-              if (g && t < (unsigned)size_c) atomicAdd(&acc[t >> 3], 1u << ((t & 7) << 2));
-            }
+        b0 += 32 * U_STEPS;
+        if (b0 >= total) {
+          k0 += U_WARPS * 32;
+          live = k0 < ce;
+          if (live) {
+            const int2 seg = seg_next;
+            seg_next = desc(k0 + U_WARPS * 32);
+            open(seg);
           }
         }
+      };
+      const auto count = [&](const int4 (&v)[U_STEPS]) {
+#pragma unroll
+        for (int q = 0; q < U_STEPS; ++q) {
+          unsigned t = (unsigned)(v[q].x - col - 1);
+          k1d_up_count(acc_s, lane, t, t < sz);
+#pragma unroll
+          for (int e = 0; e < K1D_GAPS; ++e) {
+            const unsigned g = (unsigned)k1d_gap(v[q], e);
+            t += g;
+            k1d_up_count(acc_s, lane, t, g != 0u && t < sz);
+          }
+        }
+      };
+      int4 va[U_STEPS], vb[U_STEPS];
+      bool have_a = live;
+      if (live) issue(va);
+      while (have_a) {
+        const bool have_b = live;
+        if (live) issue(vb);
+        count(va);
+        if (!have_b) break;
+        have_a = live;
+        if (live) issue(va);
+        count(vb);
       }
+    }
+    int4 wi_next = make_int4(0, 0, 0, 0);
+    if (tid == 0) {
+      it_next = failed ? p.n_range : it_next;
+      if (it_next < p.n_range) wi_next = __ldg(p.worklist_up + it_next);
     }
     __syncthreads();
     PROF_MARK(8);
@@ -565,6 +634,7 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
       ns = __reduce_add_sync(0xffffffffu, ns);
       if (lane == 0 && ns) atomicAdd(&us.nibsum, ns);
     }
+    if (tid == 0) { us.item = it_next; us.wi = wi_next; }  // every thread read this column's before the barrier above
     __syncthreads();
     const int nst = us.nst;
     if (tid == 0) {
@@ -582,6 +652,8 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
         p.own[base + t] = cd;
         atomicAdd(p.deg + (cd >> 4), 1);
       }
+    // every thread read nst before the barrier above; the next column's sweep counts after its first barrier
+    if (tid == 0) { us.nibsum = 0; us.ncand = 0; us.nst = 0; }
     PROF_MARK(9);
   }
 }
