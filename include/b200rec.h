@@ -132,7 +132,8 @@ int b200_sim_debug_set_cap(b200_sim_t h, int cap);
  * [0] stage  [1] accumulate  [2] bootstrap histogram  [3] scan+clear  [4] evaluate+compact  [5] select
  * [6] emit (window kernel); the bitmap kernel reports [1] accumulate  [2] level >= 3  [3] level 2  [4] level 1  [6] emit+clear;
  * its pair path reports [8] upper-pass gather  [9] upper-pass sweep + own-list write  [10] select kernel: keys + decision
- * [11] select kernel: select + emit (one warp per column: lane 0's clock, summed over warps).  enable!=0 turns counting on for later launches; out16 (nullable) receives and resets
+ * [11] select kernel: select + emit (one warp per column: lane 0's clock, summed over warps), and two counts of its
+ * exchange: [12] runs reserved in the bucket buffer (one per CTA and destination tile)  [13] cells written there.  enable!=0 turns counting on for later launches; out16 (nullable) receives and resets
  * the counters. */
 int b200_sim_debug_phase_cycles(b200_sim_t h, int enable, uint64_t* out16);
 
@@ -142,6 +143,13 @@ int b200_sim_debug_phase_cycles(b200_sim_t h, int enable, uint64_t* out16);
  * because a counter overflowed).  set_fail_every > 0 makes it hand back every n-th local column (exercises the redo path);
  * 0 switches that off. */
 int b200_sim_debug_k1c(b200_sim_t h, int set_fail_every, int* enabled, int* ctas_per_sm, int* n_bitmap_cols, int* n_window_cols);
+
+/* TEST HOOK for the exchange of that kernel's pair path: set_tile_log2 >= 0 (0..12) makes its destination tiles
+ * 2^set_tile_log2 columns wide from the next pair-path call on (a width whose tiles would not fit the bucket histogram is
+ * doubled); tile_log2 (nullable) receives the width the last pair-path call used (0 before the first one).
+ * deg and mir_off (nullable, n_cols + 1 values each) receive the per-column mirror counts, which are zero between calls,
+ * and the mirror-list offsets of the last pair-path call. */
+int b200_sim_debug_pair_lists(b200_sim_t h, int set_tile_log2, int* tile_log2, int32_t* deg, int32_t* mir_off);
 
 /* duration in milliseconds of the last top-K kernel launched through this handle, measured with CUDA
  * events on the launching stream (bench.py roofline leg) */

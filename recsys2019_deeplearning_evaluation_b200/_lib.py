@@ -39,6 +39,7 @@ SIGNATURES = {
     "b200_sim_debug_set_cap": (ctypes.c_int, [c_void, ctypes.c_int]),
     "b200_sim_debug_phase_cycles": (ctypes.c_int, [c_void, ctypes.c_int, ctypes.POINTER(ctypes.c_uint64)]),
     "b200_sim_debug_k1c": (ctypes.c_int, [c_void, ctypes.c_int, c_int_p, c_int_p, c_int_p, c_int_p]),
+    "b200_sim_debug_pair_lists": (ctypes.c_int, [c_void, ctypes.c_int, c_int_p, c_void, c_void]),
     "b200_sim_last_kernel_ms": (ctypes.c_int, [c_void, c_float_p]),
     "b200_sim_col_work": (ctypes.c_int, [c_void, c_void]),
     "b200_sim_work": (ctypes.c_int, [c_void, ctypes.c_int, ctypes.c_int, c_i64_p]),

@@ -658,28 +658,137 @@ __global__ void __launch_bounds__(U_THREADS, U_CTAS) sim_k1d_upper_kernel(const 
   }
 }
 
-// Exchange (after the exclusive scan of deg into mir_off): every cell (i, j, count) of the own lists (one warp per column
-// i) and of the loose list into the mirror list of j as (i << 4 | count).  Counting deg back down leaves it zero for the
-// next call; after a fallback nothing is exchanged and deg is cleared.  Launched with n_cols warps.
-__global__ void k1d_pair_scatter_kernel(const KParams p) {
-  const long long t0 = blockIdx.x * (long long)blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
-  if (*p.pair_fail) {
-    for (long long q = t0; q <= p.n_cols; q += nt) p.deg[q] = 0;
-    return;
-  }
-  const int i = (int)(t0 >> 5), lane = threadIdx.x & 31;
-  if (i < p.n_cols) {
-    const int s = p.own_off[i], n = p.own_n[i] & ~OWN_SPILLED;
-    for (int t = lane; t < n; t += 32) {
-      const unsigned cd = p.own[s + t], j = cd >> 4;
-      p.mir[p.mir_off[j] + atomicSub(p.deg + j, 1) - 1] = ((unsigned)i << 4) | (cd & 15u);
+// Exchange (after the exclusive scan of deg into mir_off): every cell (i, j, count) of the own lists and of the loose list
+// goes into the mirror list of j as (i << 4 | count), as a transpose by destination tile in two kernels whose writes stay
+// local.  Tile t is the columns [t << tile_log2, (t + 1) << tile_log2), so the tile of a cell is j >> tile_log2 (no
+// lookup), and its mirror region is [mir_off[c0], mir_off[c1]): columns are never split.
+//   bucket: per CTA, a batch of X_BATCH source columns and a share of the loose list: a shared histogram over the
+//           destination tiles, ONE returning global atomicAdd per (CTA, tile) on the tile's fill counter to reserve a run,
+//           the cells grouped by tile in shared memory, then stored as runs of (j - c0 << 32 | i << 4 | count) into
+//           `bucket`, which has the same offsets as mir: tile t's cells fill exactly its mirror region.  A run's stores
+//           are issued together, so its sectors are complete in L2 before they are evicted (stored cell by cell as the
+//           batch is read, they were not: the kernel took 1.3-2.3 ms at C5).  A batch larger than the stage is
+//           stored cell by cell;
+//   place:  one CTA per tile ranks its cells per destination column with shared-memory counters (started at the
+//           columns' offsets in the region) and writes them into a shared copy of the region, which it then stores to mir
+//           with coalesced full-sector writes (a region longer than X_STAGE is written to mir directly).  It zeroes deg
+//           (spent: zero for the next call, also after a fallback, where nothing else runs) and tile_fill.
+constexpr int X_THREADS = 512;     // threads of the bucket and place kernels
+#ifndef B200_X_BATCH
+#define B200_X_BATCH 32
+#endif
+constexpr int X_BATCH = B200_X_BATCH;  // source columns per bucket CTA (C5: ~6.9 K cells over 3 125 tiles; -D for A/B builds)
+constexpr int X_ILP = 4;           // cells per lane in flight
+constexpr int X_TILE_LOG2 = 6;     // default tile: 64 columns (C5: ~14 K cells, a 55 KB region)
+constexpr int X_MAX_TILES = 12288; // the bucket kernel's per-tile arrays' bound (2 x 48 KB): wider tiles on larger catalogues
+constexpr int X_BSTAGE = 10240;    // cells of a batch the bucket kernel groups in shared memory (80 KB: two CTAs per SM at C5)
+constexpr int X_STAGE = 24576;     // region cells the place kernel stages in shared memory (96 KB: two CTAs per SM)
+
+// Hands every cell of the bucket CTA's batch to fn(source column i, cell (j << 4 | count)): a warp per source column with
+// X_ILP own-list loads in flight per lane, then the CTA's share of the loose list.
+template <class Fn>
+__device__ __forceinline__ void k1d_batch_cells(const KParams& p, Fn fn) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c1 = min(p.n_cols, (int)(blockIdx.x + 1) * X_BATCH);
+  for (int i = blockIdx.x * X_BATCH + warp; i < c1; i += X_THREADS / 32) {
+    const int so = p.own_off[i], n = p.own_n[i] & ~OWN_SPILLED;
+    for (int t0 = 0; t0 < n; t0 += 32 * X_ILP) {
+      unsigned cd[X_ILP];
+#pragma unroll
+      for (int q = 0; q < X_ILP; ++q) {
+        const int t = t0 + 32 * q + lane;
+        cd[q] = t < n ? p.own[so + t] : 0u;
+      }
+#pragma unroll
+      for (int q = 0; q < X_ILP; ++q)
+        if (t0 + 32 * q + lane < n) fn(i, cd[q]);
     }
   }
-  const long long nl = (long long)min(*p.n_loose, (u64)p.loose_cap);
-  for (long long q = t0; q < nl; q += nt) {
-    const u64 e = p.loose[q];
-    const unsigned cd = (unsigned)e, j = cd >> 4;
-    p.mir[p.mir_off[j] + atomicSub(p.deg + j, 1) - 1] = ((unsigned)(e >> 32) << 4) | (cd & 15u);
+  const long long nl = (long long)min(*p.n_loose, (u64)p.loose_cap), G = gridDim.x;
+  for (long long q = nl * blockIdx.x / G + threadIdx.x; q < nl * (blockIdx.x + 1) / G; q += X_THREADS) {
+    const u64 c = p.loose[q];
+    fn((int)(c >> 32), (unsigned)c);
+  }
+}
+
+__global__ void __launch_bounds__(X_THREADS, 2) k1d_pair_bucket_kernel(const KParams p) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ int n_batch;
+  u64* stage = reinterpret_cast<u64*>(smem_raw);  // the batch's cells (j << 32 | i << 4 | count), grouped by tile
+  const int L = p.tile_log2, n_tiles = ((p.n_cols - 1) >> L) + 1;
+  // per destination tile: cells, then (run start in the bucket) - (start of the tile's group in the stage)
+  int* hist = reinterpret_cast<int*>(stage + X_BSTAGE);
+  int* next = hist + n_tiles;  // per destination tile: the next slot of its group
+  if (*p.pair_fail) return;
+  for (int t = threadIdx.x; t < n_tiles; t += X_THREADS) hist[t] = 0;
+  if (threadIdx.x == 0) n_batch = 0;
+  __syncthreads();
+  k1d_batch_cells(p, [&](int, unsigned cd) { atomicAdd(&hist[cd >> (4 + L)], 1); });
+  __syncthreads();
+  for (int t = threadIdx.x; t < n_tiles; t += X_THREADS) {
+    const int c = hist[t];
+    if (!c) continue;
+    const int g = p.mir_off[t << L] + atomicAdd(p.tile_fill + t, c), s = atomicAdd(&n_batch, c);
+    hist[t] = g - s;
+    next[t] = s;
+    if (p.prof) { atomicAdd(p.prof + 12, 1ull); atomicAdd(p.prof + 13, (unsigned long long)c); }  // runs and cells
+  }
+  __syncthreads();
+  const bool staged = n_batch <= X_BSTAGE;
+  const unsigned mask = (1u << L) - 1u;
+  k1d_batch_cells(p, [&](int i, unsigned cd) {
+    const unsigned j = cd >> 4, lo = ((unsigned)i << 4) | (cd & 15u);
+    const int r = atomicAdd(&next[j >> L], 1);
+    if (staged) stage[r] = ((u64)j << 32) | lo;
+    else p.bucket[hist[j >> L] + r] = ((u64)(j & mask) << 32) | lo;
+  });
+  if (!staged) return;
+  __syncthreads();
+  for (int k = threadIdx.x; k < n_batch; k += X_THREADS) {
+    const u64 e = stage[k];
+    const unsigned j = (unsigned)(e >> 32);
+    p.bucket[hist[j >> L] + k] = ((u64)(j & mask) << 32) | (unsigned)e;
+  }
+}
+
+// Persistent: CTA b places tiles b, b + gridDim.x, ...
+__global__ void __launch_bounds__(X_THREADS, 2) k1d_pair_place_kernel(const KParams p) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int L = p.tile_log2;
+  int* rank = reinterpret_cast<int*>(smem_raw);                      // per column of the tile: its next region position
+  unsigned* stage = reinterpret_cast<unsigned*>(rank + (1 << L));    // the region
+  const bool failed = *p.pair_fail;
+  const int n_tiles = ((p.n_cols - 1) >> L) + 1;
+  for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    const int c0 = t << L, nc = min(1 << L, p.n_cols - c0);
+    for (int k = threadIdx.x; k < nc; k += X_THREADS) p.deg[c0 + k] = 0;
+    if (failed) continue;
+    const int base = p.mir_off[c0], size = p.mir_off[c0 + nc] - base;
+    if (size == 0) continue;
+    for (int k = threadIdx.x; k < nc; k += X_THREADS) rank[k] = p.mir_off[c0 + k] - base;
+    if (threadIdx.x == 0) p.tile_fill[t] = 0;  // its cells are exactly the region's: size of them
+    __syncthreads();
+    const bool staged = size <= X_STAGE;
+    const u64* cells = p.bucket + base;
+    for (int k0 = 0; k0 < size; k0 += X_THREADS * X_ILP) {
+      u64 e[X_ILP];
+#pragma unroll
+      for (int q = 0; q < X_ILP; ++q) {
+        const int k = k0 + q * X_THREADS + threadIdx.x;
+        e[q] = k < size ? cells[k] : 0ull;
+      }
+#pragma unroll
+      for (int q = 0; q < X_ILP; ++q)
+        if (k0 + q * X_THREADS + threadIdx.x < size) {
+          const int r = atomicAdd(&rank[(int)(e[q] >> 32)], 1);
+          if (staged) stage[r] = (unsigned)e[q]; else p.mir[base + r] = (unsigned)e[q];
+        }
+    }
+    __syncthreads();
+    if (staged) {
+      for (int k = threadIdx.x; k < size; k += X_THREADS) p.mir[base + k] = stage[k];
+      __syncthreads();  // the region is stored before the next tile overwrites it
+    }
   }
 }
 

@@ -112,8 +112,9 @@ struct KParams {
   // window-work order; the own lists (column i's count >= 3 cells (j << 4 | count), j in i's window, one contiguous run per column:
   // start and length by column), their capacity and fill; the loose list of (i << 32 | j << 4 | count) cells that did not fit
   // a column's stage, its capacity and fill; the per-column mirror counts (deg) and offsets and the mirror lists built from
-  // them ((i << 4 | count) in the list of j); the flag that sends the whole call down the K1-D kernel, and the columns that
-  // the select kernel hands to the K1-D kernel
+  // them ((i << 4 | count) in the list of j) through the exchange's destination tiles (2^tile_log2 columns each, fill
+  // counters, bucket buffer); the flag that sends the whole call down the K1-D kernel, and the columns that the
+  // select kernel hands to the K1-D kernel
   const int2* __restrict__ csc_win;
   const int4* __restrict__ worklist_up;
   unsigned* own;
@@ -127,6 +128,9 @@ struct KParams {
   int* deg;
   const int* __restrict__ mir_off;
   unsigned* mir;
+  int tile_log2;
+  int* tile_fill;
+  u64* bucket;
   int* pair_fail;
   int sel_cap;  // the longest list the select kernel decides (its per-warp key buffer)
   int4* wl_redo;
@@ -1126,16 +1130,19 @@ struct b200_sim_s {
   std::vector<unsigned long long> h_work;  // by ORIGINAL column index
   // K1-D pair path (sim_k1d.cuh): row windows, the upper pass's work list (every column), own lists (capacity from the
   // expected pair count) with their per-column start and length, loose list, mirror lists (deg: per-column counts, zero
-  // between calls), control words (own and loose fill, fallback flag, redo count), redo list, scan scratch (all allocated
-  // by the first call that takes the path), the select kernel's level bounds, upper-pass geometry
+  // between calls), the exchange's bucket buffer and destination tiles (fill counters: zero between calls; the columns
+  // per tile requested, normally 2^X_TILE_LOG2, and the ones in use), control words (own and loose fill, fallback flag,
+  // redo count), redo list, scan scratch (all allocated by the first call that takes the path), the select kernel's level
+  // bounds, upper-pass geometry
   DevBuf<int2> csc_win;
   DevBuf<int4> worklist_up, wl_redo;
   DevBuf<unsigned> own, mir;
-  DevBuf<u64> loose;
+  DevBuf<u64> loose, bucket;
   long long pair_cap = 0, loose_cap = 0;
   double pairs_expected = 0.0;
   float lvl_b1 = 0.f, lvl_b2 = 0.f;
-  DevBuf<int> own_off, own_n, deg, mir_off, pair_ctl;
+  DevBuf<int> own_off, own_n, deg, mir_off, pair_ctl, tile_fill;
+  int tile_log2_req = X_TILE_LOG2, tile_log2 = 0;
   DevBuf<unsigned char> scan_tmp;
   size_t scan_tmp_bytes = 0, smem_up_bytes = 0, smem_sel_bytes = 0;
   int ctas_up = 0, sel_cap = 0;
@@ -1824,12 +1831,14 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.csc_win = h->csc_win.get(); p.worklist_up = h->worklist_up.get();
   if (pair_path && h->own.n == 0) {
     // first call on the pair path: the own lists hold twice the expected pairs (a fuller list sets the fallback flag), the
-    // loose list (cells past a column's stage: rare) a quarter of that, the mirror lists both; positions stay below 2^31
+    // loose list (cells past a column's stage: rare) a quarter of that, the mirror lists and the exchange's bucket buffer
+    // both; positions stay below 2^31
     h->pair_cap = std::min<long long>((long long)(2.0 * h->pairs_expected) + (1 << 16), (1ll << 30) - 1);
     h->loose_cap = h->pair_cap / 4 + (1 << 16);
     h->own.alloc((size_t)h->pair_cap);
     h->loose.alloc((size_t)h->loose_cap);
     h->mir.alloc((size_t)(h->pair_cap + h->loose_cap));
+    h->bucket.alloc((size_t)(h->pair_cap + h->loose_cap));
     h->own_off.alloc((size_t)h->n_cols);
     h->own_n.alloc((size_t)h->n_cols);
     h->deg.alloc((size_t)h->n_cols + 1);
@@ -1840,18 +1849,32 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, h->scan_tmp_bytes, h->deg.get(), h->mir_off.get(), h->n_cols + 1, st));
     h->scan_tmp.alloc(h->scan_tmp_bytes + 16);
   }
+  if (pair_path && h->tile_fill.n == 0) {
+    // destination tiles of the exchange: the requested columns per tile, doubled while the bucket kernel's per-tile arrays
+    // would not fit (C5: 3 125 tiles of 64 columns)
+    h->tile_log2 = h->tile_log2_req;
+    while (((h->n_cols - 1) >> h->tile_log2) + 1 > X_MAX_TILES) ++h->tile_log2;
+    const size_t nt = (size_t)((h->n_cols - 1) >> h->tile_log2) + 1;
+    h->tile_fill.alloc(nt);
+    B200_CUDA(cudaMemsetAsync(h->tile_fill.get(), 0, sizeof(int) * nt, st));
+    raise_smem_limit(k1d_pair_bucket_kernel, sizeof(u64) * X_BSTAGE + 2 * sizeof(int) * nt);
+    raise_smem_limit(k1d_pair_place_kernel, sizeof(int) * (((size_t)1 << h->tile_log2) + X_STAGE));
+    B200_CUDA(cudaFuncSetAttribute(k1d_pair_place_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    B200_CUDA(cudaFuncSetAttribute(k1d_pair_bucket_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  }
   p.own = h->own.get(); p.own_off = h->own_off.get(); p.own_n = h->own_n.get(); p.pair_cap = h->pair_cap;
   p.n_own = reinterpret_cast<u64*>(h->pair_ctl.get());
   p.pair_fail = h->pair_ctl.get() + 2; p.n_redo = h->pair_ctl.get() + 3;
   p.loose = h->loose.get(); p.n_loose = reinterpret_cast<u64*>(h->pair_ctl.get() + 4); p.loose_cap = h->loose_cap;
   p.deg = h->deg.get(); p.mir_off = h->mir_off.get(); p.mir = h->mir.get(); p.wl_redo = h->wl_redo.get();
+  p.tile_log2 = h->tile_log2; p.tile_fill = h->tile_fill.get(); p.bucket = h->bucket.get();
   p.sel_cap = h->sel_cap;
   p.lvl_b1 = h->lvl_b1; p.lvl_b2 = h->lvl_b2;
   B200_CUDA(cudaEventRecord(h->ev0, st));
   if (pair_path) {
-    // upper pass (own lists, deg) -> exchange (mirror lists) -> select; the select kernel's redo list (every column after a
-    // fallback) goes through the K1-D kernel, which hands its overflowed columns to the window kernel as below.  No host
-    // round trip.
+    // upper pass (own lists, deg) -> scan -> exchange (bucket, place: mirror lists) -> select; the select kernel's redo
+    // list (every column after a fallback) goes through the K1-D kernel, which hands its overflowed columns to the window
+    // kernel as below.  No host round trip.
     B200_CUDA(cudaMemcpyAsync(h->fail.get(), &h->n_dense_last, sizeof(int), cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaMemsetAsync(h->pair_ctl.get(), 0, 6 * sizeof(int), st));
     KParams q = p;
@@ -1861,7 +1884,8 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     B200_CUDA(cudaGetLastError());
     size_t tb = h->scan_tmp_bytes;
     B200_CUDA(cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), tb, h->deg.get(), h->mir_off.get(), h->n_cols + 1, st));
-    k1d_pair_scatter_kernel<<<div_up((long long)h->n_cols * 32, 256), 256, 0, st>>>(q);
+    k1d_pair_bucket_kernel<<<div_up(h->n_cols, X_BATCH), X_THREADS, sizeof(u64) * X_BSTAGE + 2 * sizeof(int) * h->tile_fill.n, st>>>(q);
+    k1d_pair_place_kernel<<<2 * h->n_sm, X_THREADS, sizeof(int) * (((size_t)1 << h->tile_log2) + X_STAGE), st>>>(q);
     B200_CUDA(cudaGetLastError());
     k1d_select_kernel_for(h->formula)<<<div_up(n_sparse, S_WARPS), 32 * S_WARPS, h->smem_sel_bytes, st>>>(q);
     B200_CUDA(cudaGetLastError());
@@ -1870,7 +1894,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     q.n_range_dev = p.n_redo;
     k1d_kernel_for(h->formula)<<<std::min(n_sparse, h->n_sm * h->ctas_per_sm), D_THREADS, h->smem1_bytes, st>>>(q);
     B200_CUDA(cudaGetLastError());
-    count_launch(6);
+    count_launch(7);
     B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
     p.n_range_dev = h->fail.get();
   } else if (n_sparse > 0) {
@@ -1996,6 +2020,25 @@ int b200_sim_debug_k1c(b200_sim_t h, int set_fail_every, int* enabled, int* ctas
         B200_CUDA(cudaDeviceSynchronize());
         B200_CUDA(cudaMemcpy(n_window_cols, h->fail.get(), sizeof(int), cudaMemcpyDeviceToHost));
       }
+    }
+  });
+}
+
+int b200_sim_debug_pair_lists(b200_sim_t h, int set_tile_log2, int* tile_log2, int32_t* deg, int32_t* mir_off) {
+  return guarded([&] {
+    B200_REQUIRE(h != nullptr, "b200_sim_debug_pair_lists: NULL handle");
+    if (set_tile_log2 >= 0) {
+      B200_REQUIRE(set_tile_log2 <= 12, "b200_sim_debug_pair_lists: tile_log2 must be in [0, 12]");
+      h->tile_log2_req = set_tile_log2;
+      h->tile_fill.release();  // the next pair-path call sizes the tiles again
+    }
+    if (tile_log2) *tile_log2 = h->tile_log2;
+    if (deg || mir_off) {
+      B200_REQUIRE(h->deg.n > 0, "b200_sim_debug_pair_lists: no call has taken the pair path yet");
+      B200_CUDA(cudaDeviceSynchronize());
+      const size_t bytes = sizeof(int) * ((size_t)h->n_cols + 1);
+      if (deg) B200_CUDA(cudaMemcpy(deg, h->deg.get(), bytes, cudaMemcpyDeviceToHost));
+      if (mir_off) B200_CUDA(cudaMemcpy(mir_off, h->mir_off.get(), bytes, cudaMemcpyDeviceToHost));
     }
   });
 }

@@ -45,6 +45,9 @@ if sys.argv[1] == "--child":
     print("%-10s kernel ms %s  checksum %s  cycles/col stage=%.0f mac=%.0f boot=%.0f scan=%.0f eval=%.0f select=%.0f emit=%.0f"
           "  pair path: upper-gather=%.0f upper-sweep=%.0f sel-keys=%.0f sel-emit=%.0f" % (
               sys.argv[3], " ".join("%.2f" % m for m in ms), chk, *cyc[:7], *cyc[8:12]), flush=True)
+    if cyc[12] > 0:
+        print("%-10s exchange: %d runs for %d cells, mean run %.1f cells" % (sys.argv[3], cyc[12] * n, cyc[13] * n, cyc[13] / cyc[12]),
+              flush=True)
     # device time per kernel of one call (a profiled run of its own): the gather / exchange / select split
     from torch.profiler import profile, ProfilerActivity
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
