@@ -313,8 +313,10 @@ enum b200_topk_mode { B200_TOPK_NONZERO = 0, B200_TOPK_ZEROS_OUTRANK = 1,
                       B200_TOPK_NONZERO_DROP_LAST = 2 };
 int b200_dense_topk_device(const float* d_matrix, int n, int K, int along_columns, int mode, int32_t* d_idx,
                            float* d_val, int32_t* d_cnt, void* stream);
-/* mode 0 over the lines of a rectangular dense matrix (line l starts at l * stride_line, its cells are stride_inner apart);
- * reported positions are cell index + index_offset -- the per-row top-K of one column slab of a sharded matrix */
+/* mode 0 or 1 over the lines of a rectangular dense matrix (line l starts at l * stride_line, its cells are stride_inner
+ * apart); reported positions are cell index + index_offset.  Mode 0: the per-row top-K of one column slab of a sharded
+ * matrix.  Mode 1 counts the zeros of a line among its n_inner cells, so its lines must be whole rows (a slab of the rows
+ * of a dense similarity, P3alpha / RP3beta with topK > 2048). */
 int b200_dense_topk_rect_device(const float* d_matrix, int n_lines, int n_inner, int64_t stride_line, int64_t stride_inner,
                                 int index_offset, int K, int mode, int32_t* d_idx, float* d_val, int32_t* d_cnt, void* stream);
 /* the same selection over the lines of a compressed sparse n x n matrix on the device (CSC columns or CSR rows):

@@ -125,7 +125,9 @@ int b200_dense_topk_rect_device(const float* d_matrix, int n_lines, int n_inner,
   return guarded([&] {
     B200_REQUIRE(d_matrix && d_idx && d_val && d_cnt, "b200_dense_topk_rect: NULL argument");
     B200_REQUIRE(n_lines > 0 && n_inner > 0 && K > 0, "b200_dense_topk_rect: bad shape");
-    B200_REQUIRE(mode == 0, "b200_dense_topk_rect: only the non-zero mode (the zeros of the other shards are not visible here)");
+    // mode 1 counts a line's zeros among its n_inner cells, so it is only right for whole lines (a slab of full rows), never
+    // for a column slab of a sharded matrix, whose other shards' zeros are not visible here
+    B200_REQUIRE(mode == 0 || mode == 1, "b200_dense_topk_rect: mode must be 0 or 1 (got %d)", mode);
     dtk::topk_lines_kernel<false><<<std::min(n_lines, sm_count() * 8), dtk::THREADS, 0, (cudaStream_t)stream>>>(
         d_matrix, nullptr, nullptr, n_lines, n_inner, (long long)stride_line, (long long)stride_inner, K, mode, d_idx, d_val, d_cnt, index_offset);
     B200_CUDA(cudaGetLastError());

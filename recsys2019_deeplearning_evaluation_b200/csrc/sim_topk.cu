@@ -754,7 +754,13 @@ __device__ void process_column(const KParams& p, int col, int target, int out_ba
         if (!load_cells<BINARY, PACK>(acci, iv, d)) continue;
         if (count_signs) {
 #pragma unroll
-          for (int c = 0; c < CPV; ++c) { cpos += d[c] > 0.f; cneg += d[c] < 0.f; }
+          for (int c = 0; c < CPV; ++c) {
+            // the sign of the similarity, not of the dot product: the scaled product is 0 where A_i or B_j is 0, and such
+            // a cell is one of the zeros that outrank the negatives (every other formula keeps the sign of d)
+            float s = d[c];
+            if (F == F_SCALE && s != 0.f) s = sim_value<F>(p, s, Ai, __int_as_float(__ldg(p.BN + win_lo + iv * CPV + c).x));
+            cpos += s > 0.f; cneg += s < 0.f;
+          }
         }
         float keepv[CPV];
         float dmax = NEG ? -d[0] : d[0];

@@ -5,7 +5,8 @@ The reference computes, per 200-row block, `Piu[block] * Pui` densified, scales 
 diagonal, keeps the topK of every ROW with a full argsort, optionally L1-normalises the rows and finally applies a
 COLUMN top-K (`similarityMatrixTopK`).  Here the product + row top-K is one pass of the similarity kernel in its
 "scale" formula (SURVEY.md Appendix A closed form): value[i, j] = (1/deg_i)^alpha * deg_j^-beta * sum_{u in item i}
-(r_uj / rowsum_u)^alpha; the column top-K runs on the device over the CSC of the result.
+(r_uj / rowsum_u)^alpha; the column top-K runs on the device over the CSC of the result.  A topK above the kernel's
+candidate buffer (2048) takes the kernel's dense mode instead, one slab of targets at a time, with a dense row top-K.
 Element-wise preparation of Pui (O(nnz)) stays on the host like the reference's sklearn `normalize`/`power` calls.
 Ties in either top-K resolve to the ascending index (the reference's argsort order is unspecified, App. A quirk 11).
 """
@@ -16,6 +17,9 @@ import scipy.sparse as sps
 
 from . import _lib
 from .similarity import _as_csr_f32, topk_table_to_csr
+
+SELECT_MAX_K = 2048  # the largest topK the window kernel's candidate buffer selects
+DENSE_SLAB_CELLS = 1 << 26  # topK > SELECT_MAX_K: cells of one dense slab of targets (256 MB of fp32)
 
 
 def _row_l1_normalize(M):
@@ -51,20 +55,16 @@ def sparse_column_topk(W, k):
     return topk_table_to_csr(n, k, idx, val, cnt)  # line = column, idx = row: entries stay in place
 
 
-def p3_similarity(URM_train, topK=100, alpha=1.0, beta=0.0, min_rating=0, implicit=False, normalize_similarity=False):
-    """Returns W_sparse (CSR float32, row i = item i's outgoing weights) as the reference's fit() leaves it.
-    beta=0 -> P3alpha, beta>0 -> RP3beta.  The recommender classes apply `min_rating` / `implicit` to their own
-    URM_train first (the reference mutates it, P3alphaRecommender.py:47-51); the arguments here serve direct callers and
-    work on a private copy."""
-    import torch
-    lib = _lib.load()
+def scaled_inputs(URM_train, alpha=1.0, beta=0.0, min_rating=0, implicit=False):
+    """The arguments of b200_sim_create_scaled for p3_similarity: Pui (CSR float32, the row-normalised URM to the power
+    alpha), A (float32, (1/deg_i)^alpha, 0 for an item nobody rated) and B (float32, deg_j^-beta, or 1 when beta == 0)."""
     URM = _as_csr_f32(URM_train).copy()
     if min_rating > 0:  # P3alphaRecommender.py:47-51
         URM.data[URM.data < min_rating] = 0
         URM.eliminate_zeros()
         if implicit:
             URM.data = np.ones(URM.data.size, dtype=np.float32)
-    n_users, n_items = URM.shape
+    n_items = URM.shape[1]
     Pui = _row_l1_normalize(URM)
     deg = np.bincount(URM.indices, minlength=n_items).astype(np.float64)  # X_bool.sum(axis=1)
     A = np.zeros(n_items, np.float64)
@@ -76,20 +76,45 @@ def p3_similarity(URM_train, topK=100, alpha=1.0, beta=0.0, min_rating=0, implic
     if alpha != 1.0:  # :64-66
         Pui = Pui.power(alpha).astype(np.float32)
         A = np.power(A, alpha)
-    A32, B32 = np.ascontiguousarray(A, np.float32), np.ascontiguousarray(B, np.float32)
+    return Pui, np.ascontiguousarray(A, np.float32), np.ascontiguousarray(B, np.float32)
+
+
+def p3_similarity(URM_train, topK=100, alpha=1.0, beta=0.0, min_rating=0, implicit=False, normalize_similarity=False):
+    """Returns W_sparse (CSR float32, row i = item i's outgoing weights) as the reference's fit() leaves it.
+    beta=0 -> P3alpha, beta>0 -> RP3beta.  The recommender classes apply `min_rating` / `implicit` to their own
+    URM_train first (the reference mutates it, P3alphaRecommender.py:47-51); the arguments here serve direct callers and
+    work on a private copy."""
+    import torch
+    lib = _lib.load()
+    Pui, A32, B32 = scaled_inputs(URM_train, alpha, beta, min_rating, implicit)
+    n_users, n_items = Pui.shape
     K = int(min(topK, n_items)) if topK is not False else n_items
+    dense = K > SELECT_MAX_K
     h = ctypes.c_void_p()
     indptr, indices, data = (np.ascontiguousarray(Pui.indptr, np.int32), np.ascontiguousarray(Pui.indices, np.int32),
                              np.ascontiguousarray(Pui.data, np.float32))
     _lib.check(lib.b200_sim_create_scaled(ctypes.byref(h), n_users, n_items, Pui.nnz, _lib.ptr(indptr), _lib.ptr(indices),
-                                          _lib.ptr(data), _lib.ptr(A32), _lib.ptr(B32), K, None))
+                                          _lib.ptr(data), _lib.ptr(A32), _lib.ptr(B32), 1 if dense else K, None))
     try:
         dev = torch.device("cuda", torch.cuda.current_device())
         idx = torch.empty((n_items, K), dtype=torch.int32, device=dev)
         val = torch.empty((n_items, K), dtype=torch.float32, device=dev)
         cnt = torch.empty((n_items,), dtype=torch.int32, device=dev)
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _lib.check(lib.b200_sim_compute_device(h, 0, n_items, idx.data_ptr(), val.data_ptr(), cnt.data_ptr(), st))
+        if dense:
+            # topK beyond the window kernel's selection buffer: the dense mode of the same handle (the scaled values, the
+            # diagonal 0) one slab of targets at a time, then per target the K largest over all cells, zeros dropped
+            # (b200_dense_topk mode 1: zeros outrank negatives, ties to the ascending index, as in the window kernel)
+            rows = max(1, min(n_items, DENSE_SLAB_CELLS // n_items))
+            S = torch.empty((rows, n_items), dtype=torch.float32, device=dev)
+            for lo in range(0, n_items, rows):
+                m = min(rows, n_items - lo)
+                _lib.check(lib.b200_sim_compute_dense_device(h, lo, lo + m, S.data_ptr(), st))
+                _lib.check(lib.b200_dense_topk_rect_device(S.data_ptr(), m, n_items, n_items, 1, 0, K, 1, idx[lo].data_ptr(),
+                                                           val[lo].data_ptr(), cnt[lo:].data_ptr(), st))
+            del S
+        else:
+            _lib.check(lib.b200_sim_compute_device(h, 0, n_items, idx.data_ptr(), val.data_ptr(), cnt.data_ptr(), st))
         T = topk_table_to_csr(n_items, K, idx, val, cnt)  # T[j, i] = value of target i towards j
     finally:
         lib.b200_sim_destroy(h)
