@@ -1006,3 +1006,312 @@ __global__ void k1d_upper_worklist_kernel(const int* __restrict__ perm, const un
   const int c = perm[k];
   wl[k] = make_int4(c, (int)(unsigned)work[k], csc_ptr[c], csc_ptr[c + 1]);
 }
+
+// ------------------------------------------------------------------------------------------------------
+// Host side: a handle's K1-D and pair-path state, its set-up at create time (k1d_build) and its launches (k1d_launch).
+// They take the similarity handle, b200_sim_s in sim_topk.cu, which holds a K1DState and is defined after this header:
+// hence the template parameter.  What the kernels read lives in the handle's KParams `base`; this is the rest.
+// ------------------------------------------------------------------------------------------------------
+struct K1DState {
+  // routing: on by default for binary data with >= k1c_min_cols columns; whether the handle qualified; the expected hits per
+  // neighbour (gathered entries / n_cols) below which a column takes K1-D; the last launch's split of the columns
+  bool want_k1c = true, k1c = false;
+  double k1c_lambda = 0.75;
+  int k1c_min_cols = 32768;
+  int n_sparse_last = 0, n_dense_last = 0;
+  sim_kernel_t kernel = nullptr, select_kernel = nullptr;  // the instances of the handle's formula
+  // second row layout with one window, CSC-side row locations, norm tile bounds, redo count, work list, CTAs per SM and
+  // dynamic shared memory of the K1-D kernel; the new index and CSC range of every column, for the host's work lists
+  DevBuf<int4> csr_idx1, worklist;
+  DevBuf<int> col_adds, fail;
+  DevBuf<int2> csc_seg;
+  DevBuf<float> tbnd;
+  int ctas_per_sm = 0;
+  size_t smem1_bytes = 0;
+  std::vector<int> h_old2new, h_csc_ptr;
+  // pair path: row windows, the upper pass's work list (every column), own lists (capacity from the expected pair count)
+  // with their per-column start and length, loose list, mirror lists (deg: per-column counts, zero between calls), the
+  // exchange's bucket buffer and destination tiles (fill counters: zero between calls; the columns per tile requested,
+  // normally 2^X_TILE_LOG2), control words (own and loose fill, fallback flag, redo count), redo list, scan scratch (all
+  // allocated by the first call that takes the path: k1d_pair_buffers), upper-pass and select geometry
+  DevBuf<int2> csc_win;
+  DevBuf<int4> worklist_up, wl_redo;
+  DevBuf<unsigned> own, mir;
+  DevBuf<u64> loose, bucket;
+  double pairs_expected = 0.0;
+  DevBuf<int> own_off, own_n, deg, mir_off, pair_ctl, tile_fill;
+  int tile_log2_req = X_TILE_LOG2;
+  DevBuf<unsigned char> scan_tmp;
+  size_t scan_tmp_bytes = 0, smem_up_bytes = 0, smem_sel_bytes = 0;
+  int ctas_up = 0;
+  bool pair_path_last = false;  // the cached routing qualifies for the pair path
+};
+
+// Whether the K1-D pair path pays on this data.  It saves about half of a K1-D pass when the select kernel decides a column
+// itself, and costs a full K1-D pass more for every column it hands back, so it is taken only when at least 90 % of the
+// non-empty columns are expected to pass the select kernel's rule: with users drawn independently, column c has
+// n_cols * P(Poisson(lambda_c) >= 3) cells with count >= 3 (lambda_c = gathered entries off the diagonal / n_cols), which
+// must reach K, and
+// no count-2 / count-1 cell may reach the floor sim(3, largest norm term).  Sets the smallest norm terms of the neighbours
+// a count-1 / count-2 cell can have, the expected number of pairs (which sizes the pair list), and the longest list the
+// select kernel decides: the largest expected list plus six standard deviations (Poisson) and 32, in multiples of 8, at
+// most S_CAP.  A longer list is redone exactly; the bound only sizes the select kernel's shared memory, so that more of
+// its warps fit on an SM (C5: expected lists of 243 to 778, sel_cap 984, six CTAs per SM instead of three).
+template <class Handle>
+bool k1d_pair_gate(Handle* h, const int* d_cnt, cudaStream_t st) {
+  KParams& p = h->base;
+  const int n = p.n_cols;
+  std::vector<int> cnt((size_t)n);
+  std::vector<int2> bn((size_t)n);
+  std::vector<float> a((size_t)n);
+  B200_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaMemcpyAsync(bn.data(), h->BN.get(), sizeof(int2) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaMemcpyAsync(a.data(), h->A.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaStreamSynchronize(st));
+  auto bval = [&](int j) { float b; std::memcpy(&b, &bn[(size_t)j].x, sizeof b); return b; };
+  float b1 = FLT_MAX, b2 = FLT_MAX;
+  for (int j = 0; j < n; ++j) {
+    if (cnt[(size_t)j] >= 1) b1 = std::min(b1, bval(j));
+    if (cnt[(size_t)j] >= 2) b2 = std::min(b2, bval(j));
+  }
+  p.lvl_b1 = b1;
+  p.lvl_b2 = b2;
+  const float bmax = bval(n - 1);
+  long long nonempty = 0, pass = 0;
+  double cells = 0.0, est_max = 0.0;
+  with_formula<F_PROD, F_NONORM, F_JACCARD, F_DICE, F_TVERSKY>(h->formula, [&](auto f) {
+    constexpr int F = decltype(f)::value;
+    for (int c = 0; c < n; ++c) {
+      if (cnt[(size_t)c] == 0) continue;
+      ++nonempty;
+      const double lam = (double)(h->h_work[(size_t)bn[(size_t)c].y] - (unsigned long long)cnt[(size_t)c]) / (double)n;
+      const double est = (double)n * std::max(0.0, 1.0 - std::exp(-lam) * (1.0 + lam + 0.5 * lam * lam));
+      cells += est;
+      est_max = std::max(est_max, est);
+      const float ai = a[(size_t)c];
+      const float fl = sim_value<F>(p, 3.f, ai, bmax) * (1.f - 1e-6f);
+      if (est >= (double)p.K && fl > 0.f && !(sim_value<F>(p, 2.f, ai, b2) >= fl) && !(sim_value<F>(p, 1.f, ai, b1) >= fl)) ++pass;
+    }
+  });
+  h->k1d.pairs_expected = 0.5 * cells;
+  p.sel_cap = (int)std::min<double>(std::ceil((est_max + 6.0 * std::sqrt(est_max) + 32.0) / 8.0) * 8.0, (double)S_CAP);
+  return nonempty > 0 && (double)pass >= 0.9 * (double)nonempty;
+}
+
+// K1-D's part of the handle's set-up, for binary data whose formula K1-D serves: the row layout and its CSC-side locations,
+// the CTAs per SM that fit, the pair path's gate and its upper pass's work list.  Points h->base at the buffers it keeps.
+// d_cnt: users per column; d_csc_pos: the CSR position of every CSC entry; h->csr_idx is still the unpadded CSR.
+template <class Handle>
+void k1d_build(Handle* h, const int* d_cnt, const int* d_csc_pos, cudaStream_t st) {
+  K1DState& k = h->k1d;
+  KParams& b = h->base;
+  const int n_rows = h->n_rows, n_cols = b.n_cols;
+  const long long nnz = h->nnz;
+  with_formula<F_PROD, F_NONORM, F_JACCARD, F_DICE, F_TVERSKY>(h->formula, [&](auto f) {
+    k.kernel = sim_k1d_kernel<decltype(f)::value>;
+    k.select_kernel = sim_k1d_select_kernel<decltype(f)::value>;
+  });
+  const bool f_ok_c = h->formula == F_PROD || h->formula == F_NONORM || h->formula == F_JACCARD || h->formula == F_DICE ||
+                      (h->formula == F_TVERSKY && b.ta >= 0.f && b.tb >= 0.f);  // decreasing in the neighbour's norm term
+  if (!h->binary || !k.want_k1c || !f_ok_c || nnz == 0 || n_cols < k.k1c_min_cols) return;
+  DevBuf<unsigned long long> win_work;  // upper-pass work per new column, and the new column indices
+  DevBuf<int> win_iota;
+  {
+    // every row twice, back to back, for the pair path's windows -- once when the doubled layout might not fit 32-bit chunk
+    // positions: the K1-D kernel reads only the first copy, and the handle does not take the pair path.  A row never has
+    // more chunks than entries, so the bound on the entries that the four-per-chunk layout needed still covers every matrix,
+    // whatever its gaps
+    const int copies = 2 * (long long)nnz + 3ll * n_rows < (1ll << 31) ? 2 : 1;
+    DevBuf<int> len1((size_t)n_rows + 1), poff1((size_t)n_rows + 1);
+    B200_CUDA(cudaMemsetAsync(len1.get() + n_rows, 0, sizeof(int), st));
+    k1d_row_len_kernel<<<div_up(n_rows, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), n_rows, copies, n_cols, len1.get());
+    count_launch();
+    size_t tb1 = 0;
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb1, len1.get(), poff1.get(), n_rows + 1, st));
+    DevBuf<unsigned char> tmp1(tb1 + 16);
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(tmp1.get(), tb1, len1.get(), poff1.get(), n_rows + 1, st)); count_launch();
+    int total1 = 0;
+    B200_CUDA(cudaMemcpyAsync(&total1, poff1.get() + n_rows, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    k.csr_idx1.alloc((size_t)total1 + 2);
+    k1d_row_fill_kernel<<<div_up((long long)n_rows * 8, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), poff1.get(), n_rows,
+                                                                           copies, n_cols, k.csr_idx1.get()); count_launch();
+    k.col_adds.alloc((size_t)n_cols);
+    k.csc_seg.alloc((size_t)nnz + 2);
+    B200_CUDA(cudaMemsetAsync(k.csc_seg.get() + nnz, 0, 2 * sizeof(int2), st));
+    if (copies == 2) {
+      k.csc_win.alloc((size_t)nnz);
+      win_work.alloc((size_t)n_cols);
+      win_iota.alloc((size_t)n_cols);
+    }
+    k1d_csc_rows_kernel<<<div_up((long long)n_cols * 32, 256), 256, 0, st>>>(h->csc_ptr.get(), h->csc_idx.get(), h->csr_ptr.get(),
+                                                                             h->csr_idx.get(), d_csc_pos, poff1.get(),
+                                                                             k.csr_idx1.get(), n_cols, k.csc_seg.get(),
+                                                                             k.col_adds.get(), k.csc_win.get(), win_work.get(),
+                                                                             win_iota.get()); count_launch();
+    B200_CUDA(cudaStreamSynchronize(st));
+  }
+  // ---- geometry and eligibility
+  const int win1 = ((n_cols + 7) / 8) * 8;
+  b.ntile = (n_cols + (1 << D_TILE_LOG2) - 1) >> D_TILE_LOG2;
+  b.bm_words = ((win1 / 8 + 1) + 3) / 4 * 4;
+  const long long fixed = (long long)b.bm_words * 4 + ((long long)b.ntile + 1) * 4 + (long long)b.ntile * 4 + 32;
+  // two CTAs per SM when both fit (each CTA also pays its static shared memory and the 1 KB the hardware reserves)
+  cudaFuncAttributes fa{};
+  B200_CUDA(cudaFuncGetAttributes(&fa, k.kernel));
+  int dev = 0, sm_total = 0, max_smem = 0;
+  B200_CUDA(cudaGetDevice(&dev));
+  B200_CUDA(cudaDeviceGetAttribute(&sm_total, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+  B200_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const long long need_keys = (long long)b.K + (1ll << D_TILE_LOG2) + 128;  // a pruned buffer always takes one more tile
+  for (int ctas = 2; ctas >= 1 && !k.k1c; --ctas) {
+    long long avail = (long long)sm_total / ctas - (long long)fa.sharedSizeBytes - 1024;
+    avail = std::min<long long>(avail, (long long)max_smem - (long long)fa.sharedSizeBytes);
+    const long long keys = std::min<long long>((avail - fixed) / 8, 4 * D_THREADS);
+    if (keys >= need_keys) {
+      k.ctas_per_sm = ctas;
+      b.cap_d = (int)keys;
+      k.smem1_bytes = (size_t)(fixed + keys * 8);
+      k.k1c = true;
+    }
+  }
+  if (k.k1c) {
+    k.tbnd.alloc((size_t)b.ntile + 1);
+    k1d_tile_bounds_kernel<<<div_up(b.ntile + 1, 128), 128, 0, st>>>(h->BN.get(), n_cols, b.ntile, k.tbnd.get()); count_launch();
+    k.fail.alloc(1);
+    k.worklist.alloc((size_t)n_cols);
+    k.h_old2new.resize((size_t)n_cols);
+    k.h_csc_ptr.resize((size_t)n_cols + 1);
+    B200_CUDA(cudaMemcpyAsync(k.h_old2new.data(), h->old2new.get(), sizeof(int) * (size_t)n_cols, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaMemcpyAsync(k.h_csc_ptr.data(), h->csc_ptr.get(), sizeof(int) * ((size_t)n_cols + 1), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    raise_smem_limit(k.kernel, k.smem1_bytes);
+    // the whole unified L1 / shared array as shared memory: without it the driver sizes the carve-out for ONE block and the
+    // second CTA of an SM never becomes resident
+    B200_CUDA(cudaFuncSetAttribute(k.kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+
+    // pair path: needs the doubled row layout; the upper pass needs the half-window counters and the stage (up to U_CTAS
+    // CTAs per SM as they fit), and it only pays when the select kernel can decide most columns itself (k1d_pair_gate); its
+    // buffers are allocated by the first call that takes it
+    cudaFuncAttributes fu{};
+    B200_CUDA(cudaFuncGetAttributes(&fu, sim_k1d_upper_kernel));
+    k.smem_up_bytes = ((size_t)k1d_upper_words(n_cols) + U_STAGE) * 4;
+    k.ctas_up = 0;
+    for (int ctas = U_CTAS; ctas >= 1 && k.ctas_up == 0 && k.csc_win.n > 0; --ctas)
+      if ((long long)k.smem_up_bytes <= std::min<long long>((long long)sm_total / ctas - 1024, (long long)max_smem) - (long long)fu.sharedSizeBytes)
+        k.ctas_up = ctas;
+    if (k.ctas_up > 0 && !k1d_pair_gate(h, d_cnt, st)) k.ctas_up = 0;
+    if (k.ctas_up > 0) {
+      raise_smem_limit(sim_k1d_upper_kernel, k.smem_up_bytes);
+      B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+      // the launch passes this handle's size; the limit is the same for every handle that shares the kernel
+      k.smem_sel_bytes = (size_t)S_WARPS * k1d_select_warp_bytes(b.sel_cap);
+      B200_CUDA(cudaFuncSetAttribute(k.select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S_WARPS * k1d_select_warp_bytes(S_CAP)));
+      B200_CUDA(cudaFuncSetAttribute(k.select_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+      k.worklist_up.alloc((size_t)n_cols);
+      // the upper pass's longest-first order: every column by descending window work (empty columns do nothing there)
+      DevBuf<unsigned long long> keys_out((size_t)n_cols);
+      DevBuf<int> perm((size_t)n_cols);
+      size_t tb = 0;
+      B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
+      DevBuf<unsigned char> tmp(tb + 16);
+      B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
+      k1d_upper_worklist_kernel<<<div_up(n_cols, 256), 256, 0, st>>>(perm.get(), keys_out.get(), h->csc_ptr.get(), n_cols, k.worklist_up.get());
+      count_launch(5);
+      B200_CUDA(cudaStreamSynchronize(st));
+    }
+  }
+  if (!k.k1c) { k.csr_idx1.release(); k.csc_seg.release(); k.col_adds.release(); }
+  if (k.ctas_up == 0) k.csc_win.release();
+  b.tbnd = k.tbnd.get(); b.csr_idx1 = k.csr_idx1.get(); b.csc_seg = k.csc_seg.get(); b.col_adds = k.col_adds.get();
+  b.worklist = k.worklist.get(); b.fail = k.fail.get();
+  b.csc_win = k.csc_win.get(); b.worklist_up = k.worklist_up.get();
+}
+
+// The pair path's buffers, allocated by the first call that takes it, and its destination tiles, allocated again after
+// b200_sim_debug_pair_lists changed their width.  Points h->base at them, before the call copies its parameters from there.
+template <class Handle>
+void k1d_pair_buffers(Handle* h, cudaStream_t st) {
+  K1DState& k = h->k1d;
+  KParams& b = h->base;
+  const int n = b.n_cols;
+  if (k.own.n == 0) {
+    // the own lists hold twice the expected pairs (a fuller list sets the fallback flag), the loose list (cells past a
+    // column's stage: rare) a quarter of that, the mirror lists and the exchange's bucket buffer both; positions stay below
+    // 2^31
+    b.pair_cap = std::min<long long>((long long)(2.0 * k.pairs_expected) + (1 << 16), (1ll << 30) - 1);
+    b.loose_cap = b.pair_cap / 4 + (1 << 16);
+    k.own.alloc((size_t)b.pair_cap);
+    k.loose.alloc((size_t)b.loose_cap);
+    k.mir.alloc((size_t)(b.pair_cap + b.loose_cap));
+    k.bucket.alloc((size_t)(b.pair_cap + b.loose_cap));
+    k.own_off.alloc((size_t)n);
+    k.own_n.alloc((size_t)n);
+    k.deg.alloc((size_t)n + 1);
+    k.mir_off.alloc((size_t)n + 1);
+    k.pair_ctl.alloc(6);  // [0..1] own fill (64-bit), [2] fallback flag, [3] redo count, [4..5] loose fill (64-bit)
+    k.wl_redo.alloc((size_t)n);
+    B200_CUDA(cudaMemsetAsync(k.deg.get(), 0, sizeof(int) * ((size_t)n + 1), st));
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, k.scan_tmp_bytes, k.deg.get(), k.mir_off.get(), n + 1, st));
+    k.scan_tmp.alloc(k.scan_tmp_bytes + 16);
+    b.own = k.own.get(); b.own_off = k.own_off.get(); b.own_n = k.own_n.get();
+    b.n_own = reinterpret_cast<u64*>(k.pair_ctl.get());
+    b.pair_fail = k.pair_ctl.get() + 2; b.n_redo = k.pair_ctl.get() + 3;
+    b.loose = k.loose.get(); b.n_loose = reinterpret_cast<u64*>(k.pair_ctl.get() + 4);
+    b.deg = k.deg.get(); b.mir_off = k.mir_off.get(); b.mir = k.mir.get(); b.wl_redo = k.wl_redo.get(); b.bucket = k.bucket.get();
+  }
+  if (k.tile_fill.n == 0) {
+    // destination tiles of the exchange: the requested columns per tile, doubled while the bucket kernel's per-tile arrays
+    // would not fit (C5: 3 125 tiles of 64 columns)
+    b.tile_log2 = k.tile_log2_req;
+    while (((n - 1) >> b.tile_log2) + 1 > X_MAX_TILES) ++b.tile_log2;
+    const size_t nt = (size_t)((n - 1) >> b.tile_log2) + 1;
+    k.tile_fill.alloc(nt);
+    B200_CUDA(cudaMemsetAsync(k.tile_fill.get(), 0, sizeof(int) * nt, st));
+    raise_smem_limit(k1d_pair_bucket_kernel, sizeof(u64) * X_BSTAGE + 2 * sizeof(int) * nt);
+    raise_smem_limit(k1d_pair_place_kernel, sizeof(int) * (((size_t)1 << b.tile_log2) + X_STAGE));
+    B200_CUDA(cudaFuncSetAttribute(k1d_pair_place_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    B200_CUDA(cudaFuncSetAttribute(k1d_pair_bucket_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    b.tile_fill = k.tile_fill.get();
+  }
+}
+
+// K1-D's part of a launch: the n_sparse > 0 columns the routing sent to it, with the call's parameters p.  On the pair path
+// the upper pass (own lists, deg) -> scan -> exchange (bucket, place: mirror lists) -> select, and the select kernel's redo
+// list (every column after a fallback) goes through the K1-D kernel; otherwise the K1-D kernel takes the columns itself.
+// Either way the columns with an overflowed counter are appended to the window kernel's list, whose length the window
+// kernel then reads from the device (p.n_range_dev): no host round trip between the launches.
+template <class Handle>
+void k1d_launch(Handle* h, KParams& p, int n_sparse, bool pair_path, cudaStream_t st) {
+  K1DState& k = h->k1d;
+  const int n = p.n_cols, grid = std::min(n_sparse, h->n_sm * k.ctas_per_sm);
+  B200_CUDA(cudaMemcpyAsync(p.fail, &k.n_dense_last, sizeof(int), cudaMemcpyHostToDevice, st));
+  KParams q = p;
+  q.n_range = n_sparse;
+  if (pair_path) {
+    B200_CUDA(cudaMemsetAsync(k.pair_ctl.get(), 0, 6 * sizeof(int), st));
+    q.n_range = n;  // the upper pass's work list holds every column
+    sim_k1d_upper_kernel<<<std::min(n, h->n_sm * k.ctas_up), U_THREADS, k.smem_up_bytes, st>>>(q);
+    q.n_range = n_sparse;
+    B200_CUDA(cudaGetLastError());
+    size_t tb = k.scan_tmp_bytes;
+    B200_CUDA(cub::DeviceScan::ExclusiveSum(k.scan_tmp.get(), tb, k.deg.get(), k.mir_off.get(), n + 1, st));
+    k1d_pair_bucket_kernel<<<div_up(n, X_BATCH), X_THREADS, sizeof(u64) * X_BSTAGE + 2 * sizeof(int) * k.tile_fill.n, st>>>(q);
+    k1d_pair_place_kernel<<<2 * h->n_sm, X_THREADS, sizeof(int) * (((size_t)1 << p.tile_log2) + X_STAGE), st>>>(q);
+    B200_CUDA(cudaGetLastError());
+    k.select_kernel<<<div_up(n_sparse, S_WARPS), 32 * S_WARPS, k.smem_sel_bytes, st>>>(q);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemsetAsync(p.counter, 0, sizeof(int), st));
+    q.worklist = k.wl_redo.get();
+    q.n_range_dev = p.n_redo;
+    k.kernel<<<grid, D_THREADS, k.smem1_bytes, st>>>(q);
+    B200_CUDA(cudaGetLastError());
+    count_launch(7);
+  } else {
+    k.kernel<<<grid, D_THREADS, k.smem1_bytes, st>>>(q);
+    B200_CUDA(cudaGetLastError());
+    count_launch();
+  }
+  B200_CUDA(cudaMemsetAsync(p.counter, 0, sizeof(int), st));
+  p.n_range_dev = p.fail;
+}

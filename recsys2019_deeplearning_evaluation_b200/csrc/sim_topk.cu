@@ -32,6 +32,7 @@
 #include <cfloat>
 #include <cmath>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -899,6 +900,31 @@ __global__ void tile_bounds_kernel(const int2* __restrict__ BN, int n_cols, int 
   tileB[g] = __int_as_float(BN[j].x);
 }
 
+// ------------------------------------------------------------------------------------------------------
+// host helpers of the launch set-up, shared with sim_k1d.cuh
+// ------------------------------------------------------------------------------------------------------
+typedef void (*sim_kernel_t)(const KParams);
+
+// Calls fn(std::integral_constant<int, F>{}) for the formula F among Fs that equals f, so that fn can name the kernel
+// instance that serves f.  The last of Fs also serves every formula not listed.
+template <int F, int... Fs, class Fn>
+decltype(auto) with_formula(int f, Fn&& fn) {
+  if constexpr (sizeof...(Fs) == 0) return fn(std::integral_constant<int, F>{});
+  else if (f == F) return fn(std::integral_constant<int, F>{});
+  else return with_formula<Fs...>(f, fn);
+}
+
+// The dynamic shared-memory limit is an attribute of the kernel, shared by every handle with the same formula and counter
+// type, each of which launches with a size of its own: raise it to this handle's size, never lower it (a handle built
+// later for a smaller catalogue would otherwise break the launches of a larger one still alive).
+template <typename Kernel>
+void raise_smem_limit(Kernel kernel, size_t bytes) {
+  cudaFuncAttributes fa{};
+  B200_CUDA(cudaFuncGetAttributes(&fa, kernel));
+  if ((size_t)fa.maxDynamicSharedSizeBytes < bytes)
+    B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+}
+
 #include "sim_k1d.cuh"
 
 // ------------------------------------------------------------------------------------------------------
@@ -1099,60 +1125,27 @@ using namespace b200;
 using namespace b200::sim;
 
 struct b200_sim_s {
-  int n_rows = 0, n_cols = 0;
+  // the launch parameters that do not change from call to call: geometry, formula constants and the handle's buffers
+  KParams base{};
+  int n_rows = 0;
   long long nnz = 0;
-  int kind = 0, K = 0, normalize = 0;
-  float shrink = 0.f, asym_alpha = 0.5f, ta = 1.f, tb = 1.f;
+  int kind = 0, normalize = 0;
+  float asym_alpha = 0.5f;
   int formula = F_PROD;
-  bool binary = false, signed_data = false;
+  bool binary = false;
   bool pack = false;               // binary path with 16-bit counters (two cells per accumulator word)
   bool allow_pack = true;
-  int acc_words = 0;               // 4-byte words allocated for the accumulator window
-  int eu_mode = 1, eu_norm = 0, eu_avg = 0;  // euclidean: distance->similarity mode, normalize, normalize_avg_row
   bool scaled = false;             // P3alpha / RP3beta product: CSC values are 1, A and B come from the caller
   const float* h_A = nullptr;
   const float* h_B = nullptr;
-  int n_win = 1, win = 0, cap = 2048, cap_alloc = 2048;
+  sim_kernel_t kernel = nullptr;   // the window kernel of the formula and counter type
   size_t smem_bytes = 0;
   int n_sm = 0;
   DevBuf<int> csr_ptr, csr_idx, csc_ptr, csc_idx, split, old2new;
   DevBuf<int2> csr_ent, csc_ent, BN;
   DevBuf<float> A, tileB;
-  int lpu_log2 = 3;
-  // K1-D (binary path, large sparse catalogues): second row layout with one window, CSC-side row locations, norm tile
-  // bounds, ring / table geometry, routing threshold (expected hits per neighbour of a column) and last-launch statistics
-  bool want_k1c = true, k1c = false;
-  DevBuf<int4> csr_idx1;
-  DevBuf<int> col_adds, fail;
-  DevBuf<int2> csc_seg;
-  DevBuf<float> tbnd;
-  DevBuf<int4> worklist;
-  int bm_words = 0, cap_d = 0, fail_every = 0, ctas_per_sm = 0, ntile = 0;
-  size_t smem1_bytes = 0;
-  double k1c_lambda = 0.75;
-  int k1c_min_cols = 32768;
-  std::vector<int> h_old2new, h_csc_ptr;
-  int n_sparse_last = 0, n_dense_last = 0;
+  K1DState k1d;                    // binary path, large sparse catalogues (sim_k1d.cuh)
   std::vector<unsigned long long> h_work;  // by ORIGINAL column index
-  // K1-D pair path (sim_k1d.cuh): row windows, the upper pass's work list (every column), own lists (capacity from the
-  // expected pair count) with their per-column start and length, loose list, mirror lists (deg: per-column counts, zero
-  // between calls), the exchange's bucket buffer and destination tiles (fill counters: zero between calls; the columns
-  // per tile requested, normally 2^X_TILE_LOG2, and the ones in use), control words (own and loose fill, fallback flag,
-  // redo count), redo list, scan scratch (all allocated by the first call that takes the path), the select kernel's level
-  // bounds, upper-pass geometry
-  DevBuf<int2> csc_win;
-  DevBuf<int4> worklist_up, wl_redo;
-  DevBuf<unsigned> own, mir;
-  DevBuf<u64> loose, bucket;
-  long long pair_cap = 0, loose_cap = 0;
-  double pairs_expected = 0.0;
-  float lvl_b1 = 0.f, lvl_b2 = 0.f;
-  DevBuf<int> own_off, own_n, deg, mir_off, pair_ctl, tile_fill;
-  int tile_log2_req = X_TILE_LOG2, tile_log2 = 0;
-  DevBuf<unsigned char> scan_tmp;
-  size_t scan_tmp_bytes = 0, smem_up_bytes = 0, smem_sel_bytes = 0;
-  int ctas_up = 0, sel_cap = 0;
-  bool pair_path_last = false;  // the cached routing qualifies for the pair path
   DevBuf<int> counter, order;
   std::vector<int> h_order;  // cached LPT order for [order_lo, order_hi)
   int order_lo = -1, order_hi = -1;
@@ -1167,132 +1160,16 @@ namespace {
 
 constexpr int GRID1D = 132 * 8;  // grid-stride loops: 8 CTAs per SM of an H100
 
-typedef void (*sim_kernel_t)(const KParams);
-template <int F>
-sim_kernel_t kernel_of(bool binary, bool pack) {
-  if (binary && pack) return sim_topk_kernel<F, true, true>;
-  if (binary) return sim_topk_kernel<F, true, false>;
-  return sim_topk_kernel<F, false, false>;
-}
-sim_kernel_t kernel_for(int formula, bool binary, bool pack) {
-  switch (formula) {
-    case F_PROD: return kernel_of<F_PROD>(binary, pack);
-    case F_NONORM: return kernel_of<F_NONORM>(binary, pack);
-    case F_JACCARD: return kernel_of<F_JACCARD>(binary, pack);
-    case F_DICE: return kernel_of<F_DICE>(binary, pack);
-    case F_SCALE: return sim_topk_kernel<F_SCALE, false, false>;
-    case F_EUCLID: return kernel_of<F_EUCLID>(binary, pack);
-    default: return kernel_of<F_TVERSKY>(binary, pack);
-  }
-}
-
-sim_kernel_t k1d_kernel_for(int formula) {
-  switch (formula) {
-    case F_PROD: return sim_k1d_kernel<F_PROD>;
-    case F_NONORM: return sim_k1d_kernel<F_NONORM>;
-    case F_JACCARD: return sim_k1d_kernel<F_JACCARD>;
-    case F_DICE: return sim_k1d_kernel<F_DICE>;
-    default: return sim_k1d_kernel<F_TVERSKY>;
-  }
-}
-
-sim_kernel_t k1d_select_kernel_for(int formula) {
-  switch (formula) {
-    case F_PROD: return sim_k1d_select_kernel<F_PROD>;
-    case F_NONORM: return sim_k1d_select_kernel<F_NONORM>;
-    case F_JACCARD: return sim_k1d_select_kernel<F_JACCARD>;
-    case F_DICE: return sim_k1d_select_kernel<F_DICE>;
-    default: return sim_k1d_select_kernel<F_TVERSKY>;
-  }
-}
-
 int bits_for(long long n) {
   int b = 1;
   while ((1ll << b) < n) ++b;
   return b;
 }
 
-// Whether the K1-D pair path pays on this data.  It saves about half of a K1-D pass when the select kernel decides a column
-// itself, and costs a full K1-D pass more for every column it hands back, so it is taken only when at least 90 % of the
-// non-empty columns are expected to pass the select kernel's rule: with users drawn independently, column c has
-// n_cols * P(Poisson(lambda_c) >= 3) cells with count >= 3 (lambda_c = gathered entries off the diagonal / n_cols), which
-// must reach K, and
-// no count-2 / count-1 cell may reach the floor sim(3, largest norm term).  Sets the smallest norm terms of the neighbours
-// a count-1 / count-2 cell can have, the expected number of pairs (which sizes the pair list), and the longest list the
-// select kernel decides: the largest expected list plus six standard deviations (Poisson) and 32, in multiples of 8, at
-// most S_CAP.  A longer list is redone exactly; the bound only sizes the select kernel's shared memory, so that more of
-// its warps fit on an SM (C5: expected lists of 243 to 778, sel_cap 984, six CTAs per SM instead of three).
-template <int F>
-bool k1d_pair_gate_f(b200_sim_s* h, const KParams& p, const std::vector<int>& cnt, const std::vector<int2>& bn, const std::vector<float>& a) {
-  const int n = h->n_cols;
-  auto bval = [&](int j) { float b; std::memcpy(&b, &bn[(size_t)j].x, sizeof b); return b; };
-  float b1 = FLT_MAX, b2 = FLT_MAX;
-  for (int j = 0; j < n; ++j) {
-    if (cnt[(size_t)j] >= 1) b1 = std::min(b1, bval(j));
-    if (cnt[(size_t)j] >= 2) b2 = std::min(b2, bval(j));
-  }
-  h->lvl_b1 = b1;
-  h->lvl_b2 = b2;
-  const float bmax = bval(n - 1);
-  long long nonempty = 0, pass = 0;
-  double cells = 0.0, est_max = 0.0;
-  for (int c = 0; c < n; ++c) {
-    if (cnt[(size_t)c] == 0) continue;
-    ++nonempty;
-    const double lam = (double)(h->h_work[(size_t)bn[(size_t)c].y] - (unsigned long long)cnt[(size_t)c]) / (double)n;
-    const double est = (double)n * std::max(0.0, 1.0 - std::exp(-lam) * (1.0 + lam + 0.5 * lam * lam));
-    cells += est;
-    est_max = std::max(est_max, est);
-    const float ai = a[(size_t)c];
-    const float fl = sim_value<F>(p, 3.f, ai, bmax) * (1.f - 1e-6f);
-    if (est >= (double)h->K && fl > 0.f && !(sim_value<F>(p, 2.f, ai, b2) >= fl) && !(sim_value<F>(p, 1.f, ai, b1) >= fl)) ++pass;
-  }
-  h->pairs_expected = 0.5 * cells;
-  h->sel_cap = (int)std::min<double>(std::ceil((est_max + 6.0 * std::sqrt(est_max) + 32.0) / 8.0) * 8.0, (double)S_CAP);
-  return nonempty > 0 && (double)pass >= 0.9 * (double)nonempty;
-}
-
-// the formula constants of KParams
-void set_formula_params(KParams& p, const b200_sim_s* h) {
-  p.se = h->shrink + 1e-6f;
-  p.shrink_div = h->shrink != 0.f ? h->shrink : 1.f;
-  p.ta = h->ta; p.tb = h->tb;
-}
-
-bool k1d_pair_gate(b200_sim_s* h, const int* d_cnt, cudaStream_t st) {
-  const int n = h->n_cols;
-  std::vector<int> cnt((size_t)n);
-  std::vector<int2> bn((size_t)n);
-  std::vector<float> a((size_t)n);
-  B200_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  B200_CUDA(cudaMemcpyAsync(bn.data(), h->BN.get(), sizeof(int2) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  B200_CUDA(cudaMemcpyAsync(a.data(), h->A.get(), sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  B200_CUDA(cudaStreamSynchronize(st));
-  KParams p{};
-  set_formula_params(p, h);
-  switch (h->formula) {
-    case F_PROD: return k1d_pair_gate_f<F_PROD>(h, p, cnt, bn, a);
-    case F_NONORM: return k1d_pair_gate_f<F_NONORM>(h, p, cnt, bn, a);
-    case F_JACCARD: return k1d_pair_gate_f<F_JACCARD>(h, p, cnt, bn, a);
-    case F_DICE: return k1d_pair_gate_f<F_DICE>(h, p, cnt, bn, a);
-    default: return k1d_pair_gate_f<F_TVERSKY>(h, p, cnt, bn, a);
-  }
-}
-
-// The dynamic shared-memory limit is an attribute of the kernel, shared by every handle with the same formula and counter
-// type, each of which launches with a size of its own: raise it to this handle's size, never lower it (a handle built
-// later for a smaller catalogue would otherwise break the launches of a larger one still alive).
-template <typename Kernel>
-void raise_smem_limit(Kernel kernel, size_t bytes) {
-  cudaFuncAttributes fa{};
-  B200_CUDA(cudaFuncGetAttributes(&fa, kernel));
-  if ((size_t)fa.maxDynamicSharedSizeBytes < bytes)
-    B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-}
-
 void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, const float* h_data,
            const float* h_row_weights, cudaStream_t st) {
-  const int n_rows = h->n_rows, n_cols = h->n_cols;
+  KParams& b = h->base;
+  const int n_rows = h->n_rows, n_cols = b.n_cols;
   const long long nnz = h->nnz;
   const size_t nnz1 = (size_t)std::max<long long>(nnz, 1);
   h->n_sm = sm_count();
@@ -1370,7 +1247,7 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
                                                        h->old2new.get(), h->A.get(), h->BN.get(), cnt_new.get());
   count_launch();
   B200_CUDA(cudaStreamSynchronize(st));
-  h->signed_data = (hflags & 2) != 0;
+  b.eu_signed = (hflags & 2) != 0;
   h->binary = ((hflags & 1) == 0) && !h_row_weights && !h->scaled;
 
   // ---- CSR in the new numbering: relabel, then sort every row segment by the new index
@@ -1435,16 +1312,17 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
   } else {
     h->formula = h->normalize ? F_PROD : F_NONORM;
   }
+  b.signed_data = (b.eu_signed && h->formula != F_EUCLID) ? 1 : 0;  // euclidean similarities are never negative
 
   // ---- window geometry: the accumulator covers `win` neighbour columns; n_win passes per target column
   int dev = 0, max_smem = 0;
   B200_CUDA(cudaGetDevice(&dev));
   B200_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   int cap = 2048;
-  while (cap < 4 * h->K) cap <<= 1;
-  B200_REQUIRE(cap <= 8192, "topK=%d too large for the top-K kernel (max 2048); use the dense path", h->K);
-  h->cap = cap;
-  h->cap_alloc = cap;
+  while (cap < 4 * b.K) cap <<= 1;
+  B200_REQUIRE(cap <= 8192, "topK=%d too large for the top-K kernel (max 2048); use the dense path", b.K);
+  b.cap = cap;
+  b.cap_alloc = cap;
   const size_t staging = (size_t)STAGE_INTS * 4;
   // binary path: counts fit 15 bits when no column holds 32768 entries (a dot product is at most the shorter column)
   {
@@ -1477,11 +1355,17 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
   int win = (n_cols + n_win - 1) / n_win;
   win = (win + cpv - 1) / cpv * cpv;
   if (win < cpv) win = cpv;
-  h->n_win = n_win;
-  h->win = win;
-  h->acc_words = std::max(win / cpw, SBINS) + 4;  // + the dummy cell the padded row segments point at (cell index `win`)
-  h->smem_bytes = (size_t)h->acc_words * 4 + (size_t)cap * 8 + staging + (size_t)n_win * (MAXTILES + 1) * 4;
-  raise_smem_limit(kernel_for(h->formula, h->binary, h->pack), h->smem_bytes);
+  b.n_win = n_win;
+  b.win = win;
+  b.acc_cells = std::max(win / cpw, SBINS) + 4;  // + the dummy cell the padded row segments point at (cell index `win`)
+  h->smem_bytes = (size_t)b.acc_cells * 4 + (size_t)cap * 8 + staging + (size_t)n_win * (MAXTILES + 1) * 4;
+  const bool binary = h->binary, pack = h->pack;
+  h->kernel = with_formula<F_PROD, F_NONORM, F_JACCARD, F_DICE, F_SCALE, F_EUCLID, F_TVERSKY>(h->formula, [&](auto f) -> sim_kernel_t {
+    constexpr int F = decltype(f)::value;
+    if constexpr (F == F_SCALE) return sim_topk_kernel<F, false, false>;  // never binary: A and B are the caller's
+    else return binary ? (pack ? sim_topk_kernel<F, true, true> : sim_topk_kernel<F, true, false>) : sim_topk_kernel<F, false, false>;
+  });
+  raise_smem_limit(h->kernel, h->smem_bytes);
   h->tileB.alloc((size_t)n_win * (MAXTILES + 1));
   tile_bounds_kernel<<<div_up((long long)n_win * (MAXTILES + 1), 128), 128, 0, st>>>(h->BN.get(), n_cols, n_win, win, tile, h->tileB.get());
   count_launch();
@@ -1491,15 +1375,14 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     const double chunks = avg_seg / (h->binary ? 4.0 : 2.0) + 1.0;
     int l2 = 1;
     while (l2 < 5 && (1 << l2) < chunks) ++l2;
-    h->lpu_log2 = l2;
+    b.lpu_log2 = l2;
   }
   if (n_win > 1 || h->binary) {
     h->split.alloc((size_t)n_rows * (n_win + 1));
     const long long total = (long long)n_rows * (n_win + 1);
     split_kernel<<<div_up(total, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), n_rows, n_win, win, h->split.get()); count_launch();
   }
-  DevBuf<unsigned long long> win_work;  // K1-D upper-pass work per new column, and the new column indices
-  DevBuf<int> win_iota;
+  DevBuf<int> idx_pad, split_pad;
   if (h->binary) {  // padded, 16-byte aligned (row, window) segments
     const long long n_seg = (long long)n_rows * n_win;
     B200_REQUIRE((long long)nnz + 3 * n_seg < (1ll << 31), "matrix too large for 32-bit positions in the padded row layout");
@@ -1513,51 +1396,12 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     int total_pad = 0;
     B200_CUDA(cudaMemcpyAsync(&total_pad, poff.get() + n_seg, sizeof(int), cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    DevBuf<int> idx_pad((size_t)total_pad + 8), split_pad((size_t)n_rows * (n_win + 1));
+    idx_pad.alloc((size_t)total_pad + 8);
+    split_pad.alloc((size_t)n_rows * (n_win + 1));
     seg_pad_kernel<<<div_up(n_seg * 8, 256), 256, 0, st>>>(h->split.get(), h->csr_idx.get(), poff.get(), n_seg, n_win, win, total_pad,
                                                           idx_pad.get(), split_pad.get()); count_launch();
     B200_CUDA(cudaStreamSynchronize(st));
-    const bool f_ok_c = h->formula == F_PROD || h->formula == F_NONORM || h->formula == F_JACCARD || h->formula == F_DICE ||
-                        (h->formula == F_TVERSKY && h->ta >= 0.f && h->tb >= 0.f);  // decreasing in the neighbour's norm term
-    if (h->want_k1c && f_ok_c && nnz > 0 && n_cols >= h->k1c_min_cols) {
-      // K1-D layout (sim_k1d.cuh): every row twice, back to back, for the pair path's windows -- once when the doubled
-      // layout might not fit 32-bit chunk positions: the K1-D kernel reads only the first copy, and the handle does not take
-      // the pair path.  A row never has more chunks than entries, so the bound on the entries that the four-per-chunk layout
-      // needed still covers every matrix, whatever its gaps
-      const int copies = 2 * (long long)nnz + 3ll * n_rows < (1ll << 31) ? 2 : 1;
-      DevBuf<int> len1((size_t)n_rows + 1), poff1((size_t)n_rows + 1);
-      B200_CUDA(cudaMemsetAsync(len1.get() + n_rows, 0, sizeof(int), st));
-      k1d_row_len_kernel<<<div_up(n_rows, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), n_rows, copies, n_cols, len1.get());
-      count_launch();
-      size_t tb1 = 0;
-      B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb1, len1.get(), poff1.get(), n_rows + 1, st));
-      DevBuf<unsigned char> tmp1(tb1 + 16);
-      B200_CUDA(cub::DeviceScan::ExclusiveSum(tmp1.get(), tb1, len1.get(), poff1.get(), n_rows + 1, st)); count_launch();
-      int total1 = 0;
-      B200_CUDA(cudaMemcpyAsync(&total1, poff1.get() + n_rows, sizeof(int), cudaMemcpyDeviceToHost, st));
-      B200_CUDA(cudaStreamSynchronize(st));
-      h->csr_idx1.alloc((size_t)total1 + 2);
-      k1d_row_fill_kernel<<<div_up((long long)n_rows * 8, 256), 256, 0, st>>>(h->csr_ptr.get(), h->csr_idx.get(), poff1.get(), n_rows,
-                                                                             copies, n_cols, h->csr_idx1.get()); count_launch();
-      h->col_adds.alloc((size_t)n_cols);
-      h->csc_seg.alloc((size_t)nnz + 2);
-      B200_CUDA(cudaMemsetAsync(h->csc_seg.get() + nnz, 0, 2 * sizeof(int2), st));
-      if (copies == 2) {
-        h->csc_win.alloc((size_t)nnz);
-        win_work.alloc((size_t)n_cols);
-        win_iota.alloc((size_t)n_cols);
-      }
-      k1d_csc_rows_kernel<<<div_up((long long)n_cols * 32, 256), 256, 0, st>>>(h->csc_ptr.get(), h->csc_idx.get(), h->csr_ptr.get(),
-                                                                               h->csr_idx.get(), csc_pos.get(), poff1.get(),
-                                                                               h->csr_idx1.get(), n_cols, h->csc_seg.get(),
-                                                                               h->col_adds.get(), h->csc_win.get(), win_work.get(),
-                                                                               win_iota.get()); count_launch();
-      B200_CUDA(cudaStreamSynchronize(st));
-    }
-    h->csr_idx = std::move(idx_pad);
-    h->split = std::move(split_pad);
   }
-  csc_pos.release();
   // ---- per-column work (for LPT ordering and the bytes model), reported by ORIGINAL column index
   {
     DevBuf<unsigned long long> work((size_t)n_cols);
@@ -1572,83 +1416,72 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
     h->h_work.resize((size_t)n_cols);
     for (int c = 0; c < n_cols; ++c) h->h_work[(size_t)c] = w_new[(size_t)o2n[(size_t)c]];
   }
-  if (!h->binary) h->csr_idx.release();  // the AoS copy carries the indices
+  k1d_build(h, cnt_new.get(), csc_pos.get(), st);
+  csc_pos.release();
+  if (h->binary) {
+    h->csr_idx = std::move(idx_pad);
+    h->split = std::move(split_pad);
+  } else {
+    h->csr_idx.release();  // the AoS copy carries the indices
+  }
   h->counter.alloc(1);
   h->order.alloc((size_t)n_cols);
-  // ---- K1-D geometry and eligibility (sim_k1d.cuh)
-  h->k1c = false;
-  if (h->csc_seg.n > 0) {
-    const int win1 = ((n_cols + 7) / 8) * 8;
-    h->ntile = (n_cols + (1 << D_TILE_LOG2) - 1) >> D_TILE_LOG2;
-    h->bm_words = ((win1 / 8 + 1) + 3) / 4 * 4;
-    const long long fixed = (long long)h->bm_words * 4 + ((long long)h->ntile + 1) * 4 + (long long)h->ntile * 4 + 32;
-    // two CTAs per SM when both fit (each CTA also pays its static shared memory and the 1 KB the hardware reserves)
-    cudaFuncAttributes fa{};
-    B200_CUDA(cudaFuncGetAttributes(&fa, k1d_kernel_for(h->formula)));
-    int dev = 0, sm_total = 0;
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sm_total, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
-    const long long need_keys = (long long)h->K + (1ll << D_TILE_LOG2) + 128;  // a pruned buffer always takes one more tile
-    for (int ctas = 2; ctas >= 1 && !h->k1c; --ctas) {
-      long long avail = (long long)sm_total / ctas - (long long)fa.sharedSizeBytes - 1024;
-      avail = std::min<long long>(avail, (long long)max_smem - (long long)fa.sharedSizeBytes);
-      const long long keys = std::min<long long>((avail - fixed) / 8, 4 * D_THREADS);
-      if (keys >= need_keys) {
-        h->ctas_per_sm = ctas;
-        h->cap_d = (int)keys;
-        h->smem1_bytes = (size_t)(fixed + keys * 8);
-        h->k1c = true;
-      }
-    }
-    if (h->k1c) {
-      h->tbnd.alloc((size_t)h->ntile + 1);
-      k1d_tile_bounds_kernel<<<div_up(h->ntile + 1, 128), 128, 0, st>>>(h->BN.get(), n_cols, h->ntile, h->tbnd.get()); count_launch();
-      h->fail.alloc(1);
-      h->worklist.alloc((size_t)n_cols);
-      h->h_old2new.resize((size_t)n_cols);
-      h->h_csc_ptr.resize((size_t)n_cols + 1);
-      B200_CUDA(cudaMemcpyAsync(h->h_old2new.data(), h->old2new.get(), sizeof(int) * (size_t)n_cols, cudaMemcpyDeviceToHost, st));
-      B200_CUDA(cudaMemcpyAsync(h->h_csc_ptr.data(), h->csc_ptr.get(), sizeof(int) * ((size_t)n_cols + 1), cudaMemcpyDeviceToHost, st));
-      B200_CUDA(cudaStreamSynchronize(st));
-      raise_smem_limit(k1d_kernel_for(h->formula), h->smem1_bytes);
-      // the whole unified L1 / shared array as shared memory: without it the driver sizes the carve-out for ONE block and the
-      // second CTA of an SM never becomes resident
-      B200_CUDA(cudaFuncSetAttribute(k1d_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+  b.csr_ptr = h->csr_ptr.get(); b.csr_ent = h->csr_ent.get(); b.csr_idx = h->csr_idx.get();
+  b.split = h->split.get();
+  b.csc_ptr = h->csc_ptr.get(); b.csc_ent = h->csc_ent.get(); b.csc_idx = h->csc_idx.get();
+  b.A = h->A.get(); b.BN = h->BN.get(); b.tileB = h->tileB.get(); b.old2new = h->old2new.get();
+  b.order = h->order.get(); b.redo = h->order.get(); b.counter = h->counter.get();
+}
 
-      // pair path: needs the doubled row layout; the upper pass needs the half-window counters and the stage (up to U_CTAS
-      // CTAs per SM as they fit), and it only pays when the select kernel can decide most columns itself (k1d_pair_gate); its
-      // buffers are allocated by the first call that takes it
-      cudaFuncAttributes fu{};
-      B200_CUDA(cudaFuncGetAttributes(&fu, sim_k1d_upper_kernel));
-      h->smem_up_bytes = ((size_t)k1d_upper_words(n_cols) + U_STAGE) * 4;
-      h->ctas_up = 0;
-      for (int ctas = U_CTAS; ctas >= 1 && h->ctas_up == 0 && h->csc_win.n > 0; --ctas)
-        if ((long long)h->smem_up_bytes <= std::min<long long>((long long)sm_total / ctas - 1024, (long long)max_smem) - (long long)fu.sharedSizeBytes)
-          h->ctas_up = ctas;
-      if (h->ctas_up > 0 && !k1d_pair_gate(h, cnt_new.get(), st)) h->ctas_up = 0;
-      if (h->ctas_up > 0) {
-        raise_smem_limit(sim_k1d_upper_kernel, h->smem_up_bytes);
-        B200_CUDA(cudaFuncSetAttribute(sim_k1d_upper_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-        // the launch passes this handle's size; the limit is the same for every handle that shares the kernel
-        h->smem_sel_bytes = (size_t)S_WARPS * k1d_select_warp_bytes(h->sel_cap);
-        B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributeMaxDynamicSharedMemorySize, S_WARPS * k1d_select_warp_bytes(S_CAP)));
-        B200_CUDA(cudaFuncSetAttribute(k1d_select_kernel_for(h->formula), cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-        h->worklist_up.alloc((size_t)n_cols);
-        // the upper pass's longest-first order: every column by descending window work (empty columns do nothing there)
-        DevBuf<unsigned long long> keys_out((size_t)n_cols);
-        DevBuf<int> perm((size_t)n_cols);
-        size_t tb = 0;
-        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
-        DevBuf<unsigned char> tmp(tb + 16);
-        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tb, win_work.get(), keys_out.get(), win_iota.get(), perm.get(), n_cols, 0, 64, st));
-        k1d_upper_worklist_kernel<<<div_up(n_cols, 256), 256, 0, st>>>(perm.get(), keys_out.get(), h->csc_ptr.get(), n_cols, h->worklist_up.get());
-        count_launch(5);
-        B200_CUDA(cudaStreamSynchronize(st));
-      }
-    }
-  }
-  if (!h->k1c) { h->csr_idx1.release(); h->csc_seg.release(); h->col_adds.release(); }
-  if (h->ctas_up == 0) h->csc_win.release();
+}  // namespace
+
+namespace {
+
+// The steps every create entry point shares: the checks of the shape and the input arrays, the environment hooks, a new
+// handle that `init` fills with the fields of its kind (and may reject), build(); the handle is deleted when a step fails.
+template <class Init>
+int create(const char* fn, b200_sim_t* out, int64_t n_rows, int64_t n_cols, int64_t nnz, const int32_t* h_indptr,
+           const int32_t* h_indices, const float* h_data, int topK, float shrink, const float* h_row_weights, void* stream,
+           Init init) {
+  if (out) *out = nullptr;
+  b200_sim_s* h = nullptr;
+  int rc = guarded([&] {
+    B200_REQUIRE(out != nullptr, "%s: out is NULL", fn);
+    B200_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0, "%s: bad shape %lld x %lld nnz %lld", fn, (long long)n_rows,
+                 (long long)n_cols, (long long)nnz);
+    B200_REQUIRE(n_rows < (1ll << 31) - 1 && n_cols < (1ll << 31) - 1 && nnz < (1ll << 31) - 1, "%s: int32 index range exceeded", fn);
+    B200_REQUIRE(topK >= 1, "%s: topK must be >= 1", fn);
+    B200_REQUIRE(h_indptr && (nnz == 0 || (h_indices && h_data)), "%s: NULL input array", fn);
+    h = new b200_sim_s();
+    h->allow_pack = getenv("B200REC_NO_PACK") == nullptr;  // test hook: force 32-bit counters on the binary path
+    // K1-D routing: on by default for binary data with >= k1c_min_cols columns; B200REC_K1C=0 disables it, the other two
+    // variables are test hooks (small matrices, forced overflow -> redo path)
+    if (const char* e = getenv("B200REC_K1C")) h->k1d.want_k1c = atoi(e) != 0;
+    if (const char* e = getenv("B200REC_K1C_LAMBDA")) h->k1d.k1c_lambda = atof(e);
+    if (const char* e = getenv("B200REC_K1C_MINCOLS")) h->k1d.k1c_min_cols = atoi(e);
+    h->n_rows = (int)n_rows;
+    h->nnz = nnz;
+    KParams& b = h->base;
+    b.n_cols = (int)n_cols;
+    b.K = (int)std::min<int64_t>(topK, n_cols);
+    b.se = shrink + 1e-6f;
+    b.shrink_div = shrink != 0.f ? shrink : 1.f;
+    b.eu_shrink = shrink;
+    b.ta = b.tb = 1.f;
+    b.eu_mode = B200_EUCLID_LIN;
+    b.eu_div = 1.f;
+    init(h);
+    build(h, h_indptr, h_indices, h_data, h_row_weights, (cudaStream_t)stream);
+    h->h_A = h->h_B = nullptr;  // the caller's arrays, read by build() only
+    *out = h;
+  });
+  if (rc != B200_OK) delete h;
+  return rc;
+}
+
+void check_range(const b200_sim_s* h, int start_col, int end_col, const char* fn) {
+  B200_REQUIRE(0 <= start_col && start_col <= end_col && end_col <= h->base.n_cols, "%s: bad column range [%d,%d)", fn,
+               start_col, end_col);
 }
 
 }  // namespace
@@ -1659,92 +1492,42 @@ int b200_sim_create(b200_sim_t* out, int64_t n_rows, int64_t n_cols, int64_t nnz
                     const int32_t* h_indices, const float* h_data, int kind, int topK, float shrink, int normalize,
                     float asymmetric_alpha, float tversky_alpha, float tversky_beta, const float* h_row_weights,
                     void* stream) {
-  if (out) *out = nullptr;
-  b200_sim_s* h = nullptr;
-  int rc = guarded([&] {
-    B200_REQUIRE(out != nullptr, "b200_sim_create: out is NULL");
-    B200_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0, "b200_sim_create: bad shape %lld x %lld nnz %lld",
-                 (long long)n_rows, (long long)n_cols, (long long)nnz);
-    B200_REQUIRE(n_rows < (1ll << 31) - 1 && n_cols < (1ll << 31) - 1 && nnz < (1ll << 31) - 1,
-                 "b200_sim_create: int32 index range exceeded");
+  return create("b200_sim_create", out, n_rows, n_cols, nnz, h_indptr, h_indices, h_data, topK, shrink, h_row_weights, stream,
+                [&](b200_sim_s* h) {
     B200_REQUIRE(kind >= B200_SIM_COSINE && kind <= B200_SIM_TVERSKY, "b200_sim_create: unknown similarity kind %d", kind);
-    B200_REQUIRE(topK >= 1, "b200_sim_create: topK must be >= 1 (dense output goes through b200_sim_compute_dense)");
-    B200_REQUIRE(h_indptr && (nnz == 0 || (h_indices && h_data)), "b200_sim_create: NULL input array");
-    h = new b200_sim_s();
-    h->allow_pack = getenv("B200REC_NO_PACK") == nullptr;  // test hook: force 32-bit counters on the binary path
-    // K1-D routing: on by default for binary data with >= k1c_min_cols columns; B200REC_K1C=0 disables it, the other two
-    // variables are test hooks (small matrices, forced overflow -> redo path)
-    if (const char* e = getenv("B200REC_K1C")) h->want_k1c = atoi(e) != 0;
-    if (const char* e = getenv("B200REC_K1C_LAMBDA")) h->k1c_lambda = atof(e);
-    if (const char* e = getenv("B200REC_K1C_MINCOLS")) h->k1c_min_cols = atoi(e);
-    h->n_rows = (int)n_rows;
-    h->n_cols = (int)n_cols;
-    h->nnz = nnz;
     h->kind = kind;
-    h->K = (int)std::min<int64_t>(topK, n_cols);
     const bool set_kind = kind == B200_SIM_JACCARD || kind == B200_SIM_DICE || kind == B200_SIM_TVERSKY;
     h->normalize = set_kind ? 0 : (normalize != 0);
-    h->shrink = shrink;
     h->asym_alpha = asymmetric_alpha;
-    h->ta = tversky_alpha;
-    h->tb = tversky_beta;
-    build(h, h_indptr, h_indices, h_data, h_row_weights, (cudaStream_t)stream);
-    *out = h;
+    h->base.ta = tversky_alpha;
+    h->base.tb = tversky_beta;
   });
-  if (rc != B200_OK && h) delete h;
-  return rc;
 }
 
 int b200_sim_create_scaled(b200_sim_t* out, int64_t n_rows, int64_t n_cols, int64_t nnz, const int32_t* h_indptr,
                            const int32_t* h_indices, const float* h_data, const float* h_A, const float* h_B, int topK,
                            void* stream) {
-  if (out) *out = nullptr;
-  b200_sim_s* h = nullptr;
-  int rc = guarded([&] {
-    B200_REQUIRE(out && h_indptr && h_A && h_B && (nnz == 0 || (h_indices && h_data)), "b200_sim_create_scaled: NULL argument");
-    B200_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_sim_create_scaled: bad shape");
-    B200_REQUIRE(topK >= 1, "b200_sim_create_scaled: topK must be >= 1");
-    h = new b200_sim_s();
-    h->n_rows = (int)n_rows; h->n_cols = (int)n_cols; h->nnz = nnz;
+  return create("b200_sim_create_scaled", out, n_rows, n_cols, nnz, h_indptr, h_indices, h_data, topK, 0.f, nullptr, stream,
+                [&](b200_sim_s* h) {
+    B200_REQUIRE(h_A && h_B, "b200_sim_create_scaled: NULL argument");
     h->kind = B200_SIM_COSINE;
-    h->K = (int)std::min<int64_t>(topK, n_cols);
     h->scaled = true;
     h->h_A = h_A; h->h_B = h_B;
-    build(h, h_indptr, h_indices, h_data, nullptr, (cudaStream_t)stream);
-    h->h_A = h->h_B = nullptr;
-    *out = h;
   });
-  if (rc != B200_OK && h) delete h;
-  return rc;
 }
 
 int b200_sim_create_euclidean(b200_sim_t* out, int64_t n_rows, int64_t n_cols, int64_t nnz, const int32_t* h_indptr,
                               const int32_t* h_indices, const float* h_data, int topK, float shrink, int normalize,
                               int normalize_avg_row, int distance_mode, void* stream) {
-  if (out) *out = nullptr;
-  b200_sim_s* h = nullptr;
-  int rc = guarded([&] {
-    B200_REQUIRE(out && h_indptr && (nnz == 0 || (h_indices && h_data)), "b200_sim_create_euclidean: NULL argument");
-    B200_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0, "b200_sim_create_euclidean: bad shape %lld x %lld nnz %lld",
-                 (long long)n_rows, (long long)n_cols, (long long)nnz);
-    B200_REQUIRE(n_rows < (1ll << 31) - 1 && n_cols < (1ll << 31) - 1 && nnz < (1ll << 31) - 1,
-                 "b200_sim_create_euclidean: int32 index range exceeded");
-    B200_REQUIRE(topK >= 1, "b200_sim_create_euclidean: topK must be >= 1");
+  return create("b200_sim_create_euclidean", out, n_rows, n_cols, nnz, h_indptr, h_indices, h_data, topK, shrink, nullptr, stream,
+                [&](b200_sim_s* h) {
     B200_REQUIRE(distance_mode >= B200_EUCLID_EXP && distance_mode <= B200_EUCLID_LOG,
                  "b200_sim_create_euclidean: unknown similarity_from_distance_mode %d", distance_mode);
-    h = new b200_sim_s();
-    h->allow_pack = getenv("B200REC_NO_PACK") == nullptr;
-    h->n_rows = (int)n_rows; h->n_cols = (int)n_cols; h->nnz = nnz;
     h->kind = B200_SIM_EUCLIDEAN;
-    h->K = (int)std::min<int64_t>(topK, n_cols);
-    h->normalize = 0;
-    h->shrink = shrink;
-    h->eu_mode = distance_mode; h->eu_norm = normalize != 0; h->eu_avg = normalize_avg_row != 0;
-    build(h, h_indptr, h_indices, h_data, nullptr, (cudaStream_t)stream);
-    *out = h;
+    h->base.eu_mode = distance_mode;
+    h->base.eu_norm = normalize != 0;
+    h->base.eu_div = normalize_avg_row ? (float)h->n_rows : 1.f;
   });
-  if (rc != B200_OK && h) delete h;
-  return rc;
 }
 
 int b200_sim_destroy(b200_sim_t h) {
@@ -1758,11 +1541,11 @@ int b200_sim_destroy(b200_sim_t h) {
 int b200_sim_info(b200_sim_t h, int* K, int* n_windows, int* window_cells, int* binary_path, int* signed_data) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_info: NULL handle");
-    if (K) *K = h->K;
-    if (n_windows) *n_windows = h->n_win;
-    if (window_cells) *window_cells = h->win;
+    if (K) *K = h->base.K;
+    if (n_windows) *n_windows = h->base.n_win;
+    if (window_cells) *window_cells = h->base.win;
     if (binary_path) *binary_path = h->binary ? (h->pack ? 2 : 1) : 0;
-    if (signed_data) *signed_data = h->signed_data ? 1 : 0;
+    if (signed_data) *signed_data = h->base.eu_signed;
   });
 }
 
@@ -1770,8 +1553,9 @@ struct PeerOut { int* idx; float* val; int* cnt; };
 
 static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx, float* d_val, int32_t* d_cnt, float* d_dense,
                         cudaStream_t st, const PeerOut* peers = nullptr, int n_peers = 0) {
-  const int n_range = end_col - start_col;
-  const bool use_k1c = h->k1c && d_dense == nullptr;
+  K1DState& k = h->k1d;
+  const int n_cols = h->base.n_cols, n_range = end_col - start_col;
+  const bool use_k1c = k.k1c && d_dense == nullptr;
   // Routing + longest-processing-time-first order of the local columns (cached per range).  With K1-D the columns whose
   // expected hits per neighbour (gathered entries / n_cols) stay below k1c_lambda go to the nibble-counter kernel (`worklist`);
   // the rest -- and whatever that kernel hands back -- go to the window kernel (`order`).
@@ -1781,143 +1565,47 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     h->h_order.clear();
     int n_nonempty_dense = 0;
     for (int i = 0; i < n_range; ++i) {
-      const bool sp = use_k1c && w[i] > 0 && (double)w[i] <= h->k1c_lambda * (double)h->n_cols;
+      const bool sp = use_k1c && w[i] > 0 && (double)w[i] <= k.k1c_lambda * (double)n_cols;
       (sp ? sparse : h->h_order).push_back(i);
       if (!sp && w[i] > 0) ++n_nonempty_dense;
     }
     // the pair path needs every pair's pass in this call: the whole column range, every non-empty column on K1-D
-    h->pair_path_last = h->ctas_up > 0 && use_k1c && start_col == 0 && end_col == h->n_cols && n_nonempty_dense == 0 && !sparse.empty();
+    k.pair_path_last = k.ctas_up > 0 && use_k1c && start_col == 0 && end_col == n_cols && n_nonempty_dense == 0 && !sparse.empty();
     auto by_work = [w](int a, int b) { return w[a] > w[b]; };
     std::stable_sort(h->h_order.begin(), h->h_order.end(), by_work);
     std::stable_sort(sparse.begin(), sparse.end(), by_work);
-    h->n_dense_last = (int)h->h_order.size();
-    h->n_sparse_last = (int)sparse.size();
+    k.n_dense_last = (int)h->h_order.size();
+    k.n_sparse_last = (int)sparse.size();
     if (!h->h_order.empty())
       B200_CUDA(cudaMemcpyAsync(h->order.get(), h->h_order.data(), sizeof(int) * h->h_order.size(), cudaMemcpyHostToDevice, st));
     std::vector<int4> wl(sparse.size());
-    for (size_t k = 0; k < sparse.size(); ++k) {
-      const int cn = h->h_old2new[(size_t)(start_col + sparse[k])];
-      wl[k] = make_int4(cn, sparse[k], h->h_csc_ptr[(size_t)cn], h->h_csc_ptr[(size_t)cn + 1]);
+    for (size_t i = 0; i < sparse.size(); ++i) {
+      const int cn = k.h_old2new[(size_t)(start_col + sparse[i])];
+      wl[i] = make_int4(cn, sparse[i], k.h_csc_ptr[(size_t)cn], k.h_csc_ptr[(size_t)cn + 1]);
     }
-    if (!wl.empty()) B200_CUDA(cudaMemcpyAsync(h->worklist.get(), wl.data(), sizeof(int4) * wl.size(), cudaMemcpyHostToDevice, st));
+    if (!wl.empty()) B200_CUDA(cudaMemcpyAsync(k.worklist.get(), wl.data(), sizeof(int4) * wl.size(), cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaStreamSynchronize(st));
     h->order_lo = start_col;
     h->order_hi = end_col;
     h->order_k1c = use_k1c;
   }
-  const bool pair_path = h->pair_path_last && n_peers == 0;
-  const int n_sparse = use_k1c ? h->n_sparse_last : 0, n_dense = use_k1c ? h->n_dense_last : n_range;
+  const bool pair_path = k.pair_path_last && n_peers == 0;
+  const int n_sparse = use_k1c ? k.n_sparse_last : 0, n_dense = use_k1c ? k.n_dense_last : n_range;
   B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
-  KParams p;
-  p.n_cols = h->n_cols; p.K = h->K; p.n_win = h->n_win; p.win = h->win; p.cap = h->cap; p.cap_alloc = h->cap_alloc;
-  p.acc_cells = h->acc_words;
-  p.lpu_log2 = h->lpu_log2;
-  p.tileB = h->tileB.get();
-  set_formula_params(p, h);
-  p.csr_ptr = h->csr_ptr.get(); p.csr_ent = h->csr_ent.get(); p.csr_idx = h->csr_idx.get();
-  p.split = h->split.get();
-  p.csc_ptr = h->csc_ptr.get(); p.csc_ent = h->csc_ent.get(); p.csc_idx = h->csc_idx.get();
-  p.A = h->A.get(); p.BN = h->BN.get(); p.old2new = h->old2new.get();
+  if (pair_path) k1d_pair_buffers(h, st);
+  KParams p = h->base;
   p.col_begin = start_col; p.n_range = n_dense;
-  p.order = h->order.get();
-  p.counter = h->counter.get();
   p.n_out = 1 + n_peers;
   p.o_idx[0] = d_idx; p.o_val[0] = d_val; p.o_cnt[0] = d_cnt;
   for (int r = 0; r < n_peers; ++r) { p.o_idx[1 + r] = peers[r].idx; p.o_val[1 + r] = peers[r].val; p.o_cnt[1 + r] = peers[r].cnt; }
-  p.signed_data = (h->signed_data && h->formula != F_EUCLID) ? 1 : 0;  // euclidean similarities are never negative
-  p.eu_mode = h->eu_mode; p.eu_norm = h->eu_norm; p.eu_signed = h->signed_data ? 1 : 0;
-  p.eu_div = h->eu_avg ? (float)h->n_rows : 1.f;
-  p.eu_shrink = h->shrink;
   p.dense_out = d_dense;
   p.prof = h->prof_on ? h->prof.get() : nullptr;
-  p.bm_words = h->bm_words; p.cap_d = h->cap_d; p.fail_every = h->fail_every; p.ntile = h->ntile; p.tbnd = h->tbnd.get();
-  p.csr_idx1 = h->csr_idx1.get(); p.csc_seg = h->csc_seg.get(); p.col_adds = h->col_adds.get(); p.worklist = h->worklist.get();
-  p.redo = h->order.get(); p.fail = h->fail.get();
   p.n_range_dev = nullptr;
-  p.csc_win = h->csc_win.get(); p.worklist_up = h->worklist_up.get();
-  if (pair_path && h->own.n == 0) {
-    // first call on the pair path: the own lists hold twice the expected pairs (a fuller list sets the fallback flag), the
-    // loose list (cells past a column's stage: rare) a quarter of that, the mirror lists and the exchange's bucket buffer
-    // both; positions stay below 2^31
-    h->pair_cap = std::min<long long>((long long)(2.0 * h->pairs_expected) + (1 << 16), (1ll << 30) - 1);
-    h->loose_cap = h->pair_cap / 4 + (1 << 16);
-    h->own.alloc((size_t)h->pair_cap);
-    h->loose.alloc((size_t)h->loose_cap);
-    h->mir.alloc((size_t)(h->pair_cap + h->loose_cap));
-    h->bucket.alloc((size_t)(h->pair_cap + h->loose_cap));
-    h->own_off.alloc((size_t)h->n_cols);
-    h->own_n.alloc((size_t)h->n_cols);
-    h->deg.alloc((size_t)h->n_cols + 1);
-    h->mir_off.alloc((size_t)h->n_cols + 1);
-    h->pair_ctl.alloc(6);  // [0..1] own fill (64-bit), [2] fallback flag, [3] redo count, [4..5] loose fill (64-bit)
-    h->wl_redo.alloc((size_t)h->n_cols);
-    B200_CUDA(cudaMemsetAsync(h->deg.get(), 0, sizeof(int) * ((size_t)h->n_cols + 1), st));
-    B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, h->scan_tmp_bytes, h->deg.get(), h->mir_off.get(), h->n_cols + 1, st));
-    h->scan_tmp.alloc(h->scan_tmp_bytes + 16);
-  }
-  if (pair_path && h->tile_fill.n == 0) {
-    // destination tiles of the exchange: the requested columns per tile, doubled while the bucket kernel's per-tile arrays
-    // would not fit (C5: 3 125 tiles of 64 columns)
-    h->tile_log2 = h->tile_log2_req;
-    while (((h->n_cols - 1) >> h->tile_log2) + 1 > X_MAX_TILES) ++h->tile_log2;
-    const size_t nt = (size_t)((h->n_cols - 1) >> h->tile_log2) + 1;
-    h->tile_fill.alloc(nt);
-    B200_CUDA(cudaMemsetAsync(h->tile_fill.get(), 0, sizeof(int) * nt, st));
-    raise_smem_limit(k1d_pair_bucket_kernel, sizeof(u64) * X_BSTAGE + 2 * sizeof(int) * nt);
-    raise_smem_limit(k1d_pair_place_kernel, sizeof(int) * (((size_t)1 << h->tile_log2) + X_STAGE));
-    B200_CUDA(cudaFuncSetAttribute(k1d_pair_place_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    B200_CUDA(cudaFuncSetAttribute(k1d_pair_bucket_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-  }
-  p.own = h->own.get(); p.own_off = h->own_off.get(); p.own_n = h->own_n.get(); p.pair_cap = h->pair_cap;
-  p.n_own = reinterpret_cast<u64*>(h->pair_ctl.get());
-  p.pair_fail = h->pair_ctl.get() + 2; p.n_redo = h->pair_ctl.get() + 3;
-  p.loose = h->loose.get(); p.n_loose = reinterpret_cast<u64*>(h->pair_ctl.get() + 4); p.loose_cap = h->loose_cap;
-  p.deg = h->deg.get(); p.mir_off = h->mir_off.get(); p.mir = h->mir.get(); p.wl_redo = h->wl_redo.get();
-  p.tile_log2 = h->tile_log2; p.tile_fill = h->tile_fill.get(); p.bucket = h->bucket.get();
-  p.sel_cap = h->sel_cap;
-  p.lvl_b1 = h->lvl_b1; p.lvl_b2 = h->lvl_b2;
   B200_CUDA(cudaEventRecord(h->ev0, st));
-  if (pair_path) {
-    // upper pass (own lists, deg) -> scan -> exchange (bucket, place: mirror lists) -> select; the select kernel's redo
-    // list (every column after a fallback) goes through the K1-D kernel, which hands its overflowed columns to the window
-    // kernel as below.  No host round trip.
-    B200_CUDA(cudaMemcpyAsync(h->fail.get(), &h->n_dense_last, sizeof(int), cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemsetAsync(h->pair_ctl.get(), 0, 6 * sizeof(int), st));
-    KParams q = p;
-    q.n_range = h->n_cols;  // the upper pass's work list holds every column
-    sim_k1d_upper_kernel<<<std::min(h->n_cols, h->n_sm * h->ctas_up), U_THREADS, h->smem_up_bytes, st>>>(q);
-    q.n_range = n_sparse;
-    B200_CUDA(cudaGetLastError());
-    size_t tb = h->scan_tmp_bytes;
-    B200_CUDA(cub::DeviceScan::ExclusiveSum(h->scan_tmp.get(), tb, h->deg.get(), h->mir_off.get(), h->n_cols + 1, st));
-    k1d_pair_bucket_kernel<<<div_up(h->n_cols, X_BATCH), X_THREADS, sizeof(u64) * X_BSTAGE + 2 * sizeof(int) * h->tile_fill.n, st>>>(q);
-    k1d_pair_place_kernel<<<2 * h->n_sm, X_THREADS, sizeof(int) * (((size_t)1 << h->tile_log2) + X_STAGE), st>>>(q);
-    B200_CUDA(cudaGetLastError());
-    k1d_select_kernel_for(h->formula)<<<div_up(n_sparse, S_WARPS), 32 * S_WARPS, h->smem_sel_bytes, st>>>(q);
-    B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
-    q.worklist = h->wl_redo.get();
-    q.n_range_dev = p.n_redo;
-    k1d_kernel_for(h->formula)<<<std::min(n_sparse, h->n_sm * h->ctas_per_sm), D_THREADS, h->smem1_bytes, st>>>(q);
-    B200_CUDA(cudaGetLastError());
-    count_launch(7);
-    B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
-    p.n_range_dev = h->fail.get();
-  } else if (n_sparse > 0) {
-    // nibble-counter kernel first; columns with an overflowed counter are appended to the window kernel's list, whose length
-    // the window kernel then reads from the device (no host round trip between the two launches)
-    B200_CUDA(cudaMemcpyAsync(h->fail.get(), &h->n_dense_last, sizeof(int), cudaMemcpyHostToDevice, st));
-    KParams q = p;
-    q.n_range = n_sparse;
-    k1d_kernel_for(h->formula)<<<std::min(n_sparse, h->n_sm * h->ctas_per_sm), D_THREADS, h->smem1_bytes, st>>>(q);
-    B200_CUDA(cudaGetLastError());
-    count_launch();
-    B200_CUDA(cudaMemsetAsync(h->counter.get(), 0, sizeof(int), st));
-    p.n_range_dev = h->fail.get();
-  }
+  if (n_sparse > 0) k1d_launch(h, p, n_sparse, pair_path, st);  // the pair path implies n_sparse > 0
   if (n_dense > 0 || n_sparse > 0) {
     const int grid = n_sparse > 0 ? h->n_sm : std::min(n_dense, h->n_sm);
-    kernel_for(h->formula, h->binary, h->pack)<<<grid, THREADS, h->smem_bytes, st>>>(p);
+    h->kernel<<<grid, THREADS, h->smem_bytes, st>>>(p);
     B200_CUDA(cudaGetLastError());
     count_launch();
   }
@@ -1929,8 +1617,7 @@ int b200_sim_compute_device(b200_sim_t h, int start_col, int end_col, int32_t* d
                             void* stream) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_compute: NULL handle");
-    B200_REQUIRE(0 <= start_col && start_col <= end_col && end_col <= h->n_cols, "b200_sim_compute: bad column range [%d,%d)",
-                 start_col, end_col);
+    check_range(h, start_col, end_col, "b200_sim_compute");
     if (end_col == start_col) return;
     B200_REQUIRE(d_idx && d_val && d_cnt, "b200_sim_compute: NULL output");
     launch_topk(h, start_col, end_col, d_idx, d_val, d_cnt, nullptr, (cudaStream_t)stream);
@@ -1941,8 +1628,7 @@ int b200_sim_compute_peers_device(b200_sim_t h, int start_col, int end_col, int 
                                   int64_t val_offset, int64_t cnt_offset, void* stream) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_compute_peers: NULL handle");
-    B200_REQUIRE(0 <= start_col && start_col <= end_col && end_col <= h->n_cols, "b200_sim_compute_peers: bad column range [%d,%d)",
-                 start_col, end_col);
+    check_range(h, start_col, end_col, "b200_sim_compute_peers");
     B200_REQUIRE(n_tables >= 1 && n_tables <= B200_MAX_PEERS && d_tables != nullptr, "b200_sim_compute_peers: 1..%d tables", B200_MAX_PEERS);
     if (end_col == start_col) return;
     PeerOut out[B200_MAX_PEERS];
@@ -1950,8 +1636,8 @@ int b200_sim_compute_peers_device(b200_sim_t h, int start_col, int end_col, int 
       B200_REQUIRE(d_tables[r] != nullptr, "b200_sim_compute_peers: NULL table");
       int32_t* base = reinterpret_cast<int32_t*>(d_tables[r]);
       // rows are addressed by GLOBAL column: the range's first row sits at start_col
-      out[r].idx = base + idx_offset + (int64_t)start_col * h->K;
-      out[r].val = reinterpret_cast<float*>(base + val_offset) + (int64_t)start_col * h->K;
+      out[r].idx = base + idx_offset + (int64_t)start_col * h->base.K;
+      out[r].val = reinterpret_cast<float*>(base + val_offset) + (int64_t)start_col * h->base.K;
       out[r].cnt = base + cnt_offset + start_col;
     }
     launch_topk(h, start_col, end_col, out[0].idx, out[0].val, out[0].cnt, nullptr, (cudaStream_t)stream, out + 1, n_tables - 1);
@@ -1962,12 +1648,11 @@ int b200_sim_compute_dense_device(b200_sim_t h, int start_col, int end_col, floa
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_compute_dense: NULL handle");
     B200_REQUIRE(h->formula != F_EUCLID, "b200_sim_compute_dense: the euclidean similarity has no dense output mode");
-    B200_REQUIRE(0 <= start_col && start_col <= end_col && end_col <= h->n_cols, "b200_sim_compute_dense: bad column range [%d,%d)",
-                 start_col, end_col);
+    check_range(h, start_col, end_col, "b200_sim_compute_dense");
     if (end_col == start_col) return;  // an empty range has an empty output, which may well be a NULL pointer
     B200_REQUIRE(d_out != nullptr, "b200_sim_compute_dense: NULL output");
     cudaStream_t st = (cudaStream_t)stream;
-    B200_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * (size_t)(end_col - start_col) * (size_t)h->n_cols, st));
+    B200_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * (size_t)(end_col - start_col) * (size_t)h->base.n_cols, st));
     launch_topk(h, start_col, end_col, nullptr, nullptr, nullptr, d_out, st);
   });
 }
@@ -1975,16 +1660,15 @@ int b200_sim_compute_dense_device(b200_sim_t h, int start_col, int end_col, floa
 int b200_sim_compute(b200_sim_t h, int start_col, int end_col, int32_t* h_idx, float* h_val, int32_t* h_cnt) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_compute: NULL handle");
-    B200_REQUIRE(0 <= start_col && start_col <= end_col && end_col <= h->n_cols, "b200_sim_compute: bad column range [%d,%d)",
-                 start_col, end_col);
-    const size_t n_range = (size_t)(end_col - start_col);
+    check_range(h, start_col, end_col, "b200_sim_compute");
+    const size_t n_range = (size_t)(end_col - start_col), K = (size_t)h->base.K;
     if (n_range == 0) return;
-    DevBuf<int> d_idx(n_range * h->K), d_cnt(n_range);
-    DevBuf<float> d_val(n_range * h->K);
+    DevBuf<int> d_idx(n_range * K), d_cnt(n_range);
+    DevBuf<float> d_val(n_range * K);
     int rc = b200_sim_compute_device(h, start_col, end_col, d_idx.get(), d_val.get(), d_cnt.get(), nullptr);
     if (rc != B200_OK) throw CudaFail{rc};
-    B200_CUDA(cudaMemcpy(h_idx, d_idx.get(), sizeof(int) * n_range * h->K, cudaMemcpyDeviceToHost));
-    B200_CUDA(cudaMemcpy(h_val, d_val.get(), sizeof(float) * n_range * h->K, cudaMemcpyDeviceToHost));
+    B200_CUDA(cudaMemcpy(h_idx, d_idx.get(), sizeof(int) * n_range * K, cudaMemcpyDeviceToHost));
+    B200_CUDA(cudaMemcpy(h_val, d_val.get(), sizeof(float) * n_range * K, cudaMemcpyDeviceToHost));
     B200_CUDA(cudaMemcpy(h_cnt, d_cnt.get(), sizeof(int) * n_range, cudaMemcpyDeviceToHost));
   });
 }
@@ -1992,8 +1676,8 @@ int b200_sim_compute(b200_sim_t h, int start_col, int end_col, int32_t* h_idx, f
 int b200_sim_debug_set_cap(b200_sim_t h, int cap) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_debug_set_cap: NULL handle");
-    B200_REQUIRE(cap > h->K && cap <= h->cap_alloc, "b200_sim_debug_set_cap: cap must be in (K, %d]", h->cap_alloc);
-    h->cap = cap;
+    B200_REQUIRE(cap > h->base.K && cap <= h->base.cap_alloc, "b200_sim_debug_set_cap: cap must be in (K, %d]", h->base.cap_alloc);
+    h->base.cap = cap;
   });
 }
 
@@ -2016,15 +1700,16 @@ int b200_sim_debug_phase_cycles(b200_sim_t h, int enable, uint64_t* out16) {
 int b200_sim_debug_k1c(b200_sim_t h, int set_fail_every, int* enabled, int* ctas_per_sm, int* n_bitmap_cols, int* n_window_cols) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_debug_k1c: NULL handle");
-    if (set_fail_every >= 0 && h->k1c) h->fail_every = set_fail_every;  // 0 = off; n: every n-th local column is handed back
-    if (enabled) *enabled = h->k1c ? 1 : 0;
-    if (ctas_per_sm) *ctas_per_sm = h->k1c ? h->ctas_per_sm : 0;
-    if (n_bitmap_cols) *n_bitmap_cols = h->n_sparse_last;  // routing of the last launch
+    const K1DState& k = h->k1d;
+    if (set_fail_every >= 0 && k.k1c) h->base.fail_every = set_fail_every;  // 0 = off; n: every n-th local column is handed back
+    if (enabled) *enabled = k.k1c ? 1 : 0;
+    if (ctas_per_sm) *ctas_per_sm = k.k1c ? k.ctas_per_sm : 0;
+    if (n_bitmap_cols) *n_bitmap_cols = k.n_sparse_last;  // routing of the last launch
     if (n_window_cols) {
-      *n_window_cols = h->n_dense_last;
-      if (h->k1c && h->n_sparse_last > 0) {  // the nibble kernel's redo count is on the device
+      *n_window_cols = k.n_dense_last;
+      if (k.k1c && k.n_sparse_last > 0) {  // the nibble kernel's redo count is on the device
         B200_CUDA(cudaDeviceSynchronize());
-        B200_CUDA(cudaMemcpy(n_window_cols, h->fail.get(), sizeof(int), cudaMemcpyDeviceToHost));
+        B200_CUDA(cudaMemcpy(n_window_cols, k.fail.get(), sizeof(int), cudaMemcpyDeviceToHost));
       }
     }
   });
@@ -2033,18 +1718,20 @@ int b200_sim_debug_k1c(b200_sim_t h, int set_fail_every, int* enabled, int* ctas
 int b200_sim_debug_pair_lists(b200_sim_t h, int set_tile_log2, int* tile_log2, int32_t* deg, int32_t* mir_off) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_sim_debug_pair_lists: NULL handle");
+    K1DState& k = h->k1d;
     if (set_tile_log2 >= 0) {
       B200_REQUIRE(set_tile_log2 <= 12, "b200_sim_debug_pair_lists: tile_log2 must be in [0, 12]");
-      h->tile_log2_req = set_tile_log2;
-      h->tile_fill.release();  // the next pair-path call sizes the tiles again
+      k.tile_log2_req = set_tile_log2;
+      k.tile_fill.release();  // the next pair-path call sizes the tiles again
+      h->base.tile_fill = nullptr;
     }
-    if (tile_log2) *tile_log2 = h->tile_log2;
+    if (tile_log2) *tile_log2 = h->base.tile_log2;
     if (deg || mir_off) {
-      B200_REQUIRE(h->deg.n > 0, "b200_sim_debug_pair_lists: no call has taken the pair path yet");
+      B200_REQUIRE(k.deg.n > 0, "b200_sim_debug_pair_lists: no call has taken the pair path yet");
       B200_CUDA(cudaDeviceSynchronize());
-      const size_t bytes = sizeof(int) * ((size_t)h->n_cols + 1);
-      if (deg) B200_CUDA(cudaMemcpy(deg, h->deg.get(), bytes, cudaMemcpyDeviceToHost));
-      if (mir_off) B200_CUDA(cudaMemcpy(mir_off, h->mir_off.get(), bytes, cudaMemcpyDeviceToHost));
+      const size_t bytes = sizeof(int) * ((size_t)h->base.n_cols + 1);
+      if (deg) B200_CUDA(cudaMemcpy(deg, k.deg.get(), bytes, cudaMemcpyDeviceToHost));
+      if (mir_off) B200_CUDA(cudaMemcpy(mir_off, k.mir_off.get(), bytes, cudaMemcpyDeviceToHost));
     }
   });
 }
@@ -2061,14 +1748,14 @@ int b200_sim_last_kernel_ms(b200_sim_t h, float* ms) {
 int b200_sim_col_work(b200_sim_t h, int64_t* out_n_cols) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr && out_n_cols != nullptr, "b200_sim_col_work: NULL argument");
-    for (int c = 0; c < h->n_cols; ++c) out_n_cols[c] = (int64_t)h->h_work[(size_t)c];
+    for (int c = 0; c < h->base.n_cols; ++c) out_n_cols[c] = (int64_t)h->h_work[(size_t)c];
   });
 }
 
 int b200_sim_work(b200_sim_t h, int start_col, int end_col, int64_t* gathered_entries) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr && gathered_entries != nullptr, "b200_sim_work: NULL argument");
-    B200_REQUIRE(0 <= start_col && start_col <= end_col && end_col <= h->n_cols, "b200_sim_work: bad column range");
+    check_range(h, start_col, end_col, "b200_sim_work");
     unsigned long long s = 0;
     for (int c = start_col; c < end_col; ++c) s += h->h_work[(size_t)c];
     *gathered_entries = (int64_t)s;

@@ -56,6 +56,20 @@ def test_fails_loudly_without_cuda():
         Compute_Similarity_Cython(X, topK=5)
 
 
+def test_create_scaled_rejects_columns_past_int32():
+    """The column count is checked before it is narrowed to int, and before any CUDA call."""
+    from recsys2019_deeplearning_evaluation_b200 import _lib
+    L = _lib.load()
+    h = ctypes.c_void_p(1)
+    indptr = np.zeros(5, np.int32)
+    A = np.ones(1, np.float32)
+    B = np.ones(1, np.float32)
+    rc = L.b200_sim_create_scaled(ctypes.byref(h), 4, 2**31, 0, _lib.ptr(indptr), None, None, _lib.ptr(A), _lib.ptr(B), 5, None)
+    assert rc == -1
+    assert h.value is None
+    assert b"int32 index range exceeded" in L.b200_last_error()
+
+
 def test_argument_errors_mirror_the_reference():
     from recsys2019_deeplearning_evaluation_b200.similarity import Compute_Similarity_Cython, Compute_Similarity
     from recsys2019_deeplearning_evaluation_b200.synth import synth_urm

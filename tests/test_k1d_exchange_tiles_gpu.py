@@ -10,18 +10,12 @@ import ctypes
 import numpy as np
 import pytest
 
+from k1d_util import _lib, _phase_cycles, force_k1c  # noqa: F401 (fixture)
 from recsys2019_deeplearning_evaluation_b200.synth import synth_urm
 from test_k1d_exchange_gpu import K, KW, S_CAP, _designed
-from test_k1d_pairs_gpu import _lib, _phase_cycles
 
 pytestmark = pytest.mark.gpu
 
-
-@pytest.fixture
-def force_k1c(monkeypatch):
-    monkeypatch.setenv("B200REC_K1C_MINCOLS", "1")
-    monkeypatch.setenv("B200REC_K1C_LAMBDA", "1e9")  # every non-empty column goes to K1-D
-    yield monkeypatch
 
 
 def _handle(X, fail_every=0, **kw):

@@ -11,21 +11,15 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
+from k1d_util import _lib, _phase_cycles, force_k1c  # noqa: F401 (fixture)
 from oracle.similarity_oracle import SimilarityOracle, check_topk_against_dense
 from recsys2019_deeplearning_evaluation_b200.synth import synth_urm
-from test_k1d_pairs_gpu import _lib, _phase_cycles
 from test_k1d_window_gpu import _designed
 
 pytestmark = pytest.mark.gpu
 
 KW = dict(topK=20, shrink=1000, similarity="cosine")  # the shrink keeps sim(3, largest norm) above every count-2 / count-1 cell
 
-
-@pytest.fixture
-def force_k1c(monkeypatch):
-    monkeypatch.setenv("B200REC_K1C_MINCOLS", "1")
-    monkeypatch.setenv("B200REC_K1C_LAMBDA", "1e9")  # every non-empty column goes to K1-D
-    yield monkeypatch
 
 
 def _check(X, monkeypatch, cols):

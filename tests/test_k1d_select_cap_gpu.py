@@ -8,20 +8,14 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
+from k1d_util import _full_vs_parts, _phase_cycles, force_k1c  # noqa: F401 (fixture)
 from recsys2019_deeplearning_evaluation_b200.synth import synth_urm
-from test_k1d_pairs_gpu import _full_vs_parts, _phase_cycles
 
 pytestmark = pytest.mark.gpu
 
 K = 50
 KW = dict(topK=K, shrink=1000, similarity="cosine")  # the shrink keeps sim(3, largest norm) above every count-2 / count-1 cell
 
-
-@pytest.fixture
-def force_k1c(monkeypatch):
-    monkeypatch.setenv("B200REC_K1C_MINCOLS", "1")
-    monkeypatch.setenv("B200REC_K1C_LAMBDA", "1e9")  # every non-empty column goes to K1-D
-    yield monkeypatch
 
 
 def _sel_cap(X):

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
+from k1d_util import force_k1c  # noqa: F401 (fixture)
 from oracle.similarity_oracle import EuclideanOracle, SimilarityOracle, check_topk_against_dense
 from recsys2019_deeplearning_evaluation_b200.dist import balanced_ranges
 from recsys2019_deeplearning_evaluation_b200.synth import synth_urm
@@ -252,12 +253,6 @@ def test_peers_candidate_overflow_rescan():
 
     _check_peer_route(make, X, exact=False, oracle=SimilarityOracle(X, **kw))
 
-
-@pytest.fixture
-def force_k1c(monkeypatch):
-    monkeypatch.setenv("B200REC_K1C_MINCOLS", "1")
-    monkeypatch.setenv("B200REC_K1C_LAMBDA", "1e9")  # every non-empty column goes to K1-D
-    yield monkeypatch
 
 
 def test_peers_k1d_with_redo(force_k1c):

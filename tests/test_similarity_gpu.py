@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
+from k1d_util import force_k1c  # noqa: F401 (fixture)
 from oracle.similarity_oracle import SimilarityOracle, check_topk_against_dense
 from recsys2019_deeplearning_evaluation_b200.synth import synth_urm
 
@@ -187,12 +188,6 @@ def _k1c_info(sim):
     _lib.check(_lib.load().b200_sim_debug_k1c(sim._h, -1, ctypes.byref(en), ctypes.byref(ctas), ctypes.byref(nb), ctypes.byref(nw)))
     return en.value, ctas.value, nb.value, nw.value
 
-
-@pytest.fixture
-def force_k1c(monkeypatch):
-    monkeypatch.setenv("B200REC_K1C_MINCOLS", "1")
-    monkeypatch.setenv("B200REC_K1C_LAMBDA", "1e9")  # every non-empty column goes to the nibble kernel first
-    yield monkeypatch
 
 
 @pytest.mark.parametrize("kind", ["cosine", "asymmetric", "jaccard", "tanimoto", "dice", "tversky"])
