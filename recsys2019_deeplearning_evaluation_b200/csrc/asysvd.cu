@@ -17,13 +17,13 @@
 #include <algorithm>
 #include <vector>
 
+#include "adaptive.cuh"
 #include "common.cuh"
 #include "sampler.cuh"
 
 namespace b200 {
 namespace asy {
 
-enum SgdMode { SGD = 0, ADAGRAD = 1, RMSPROP = 2, ADAM = 3 };
 constexpr int THREADS = 1024;
 constexpr int WARPS = THREADS / 32;
 static_assert(WARPS == 32, "step (2) keeps one partial vector per lane");
@@ -46,13 +46,13 @@ struct Params {
 
 // pyx:838-876 on register copies of the state; c is the adagrad / rmsprop cache or adam's first moment, m2 adam's second moment
 __device__ __forceinline__ float adapt(const Params& p, float g, float& c, float& m2, float inv1, float inv2) {
-  if (p.sgd_mode == ADAGRAD) {
+  if (p.sgd_mode == B200_ADAGRAD) {
     c += g * g;
     return g / (sqrtf(c) + 1e-8f);
-  } else if (p.sgd_mode == RMSPROP) {
+  } else if (p.sgd_mode == B200_RMSPROP) {
     c = c * p.gamma + (1.f - p.gamma) * g * g;
     return g / (sqrtf(c) + 1e-8f);
-  } else if (p.sgd_mode == ADAM) {
+  } else if (p.sgd_mode == B200_ADAM) {
     c = c * p.beta1 + (1.f - p.beta1) * g;
     m2 = m2 * p.beta2 + (1.f - p.beta2) * g * g;
     return (c * inv1) / (sqrtf(m2 * inv2) + 1e-8f);
@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(THREADS) asysvd_sequential_kernel(const Params
       for (int off = 16; off > 0; off >>= 1) pred += __shfl_xor_sync(0xffffffffu, pred, off);
       if (lane == 0) {
         float inv1 = 1.f, inv2 = 1.f;
-        if (p.sgd_mode == ADAM) { inv1 = (float)(1.0 / (1.0 - b1p)); inv2 = (float)(1.0 / (1.0 - b2p)); s_inv1 = inv1; s_inv2 = inv2; }
+        if (p.sgd_mode == B200_ADAM) { inv1 = adam_correction(b1p); inv2 = adam_correction(b2p); s_inv1 = inv1; s_inv2 = inv2; }
         if (p.use_bias) pred += b_mu + b_u + b_i;  // pyx:458-461
         const float err = r - pred;  // pyx:468-471 with batch_size == 1
         s_err = err;
@@ -183,7 +183,7 @@ __global__ void __launch_bounds__(THREADS) asysvd_sequential_kernel(const Params
           p.bi[i] = b_i + p.lr * gi;
           p.bu[u] = b_u + p.lr * gu;
         }
-        if (p.sgd_mode == ADAM) { b1p *= (double)p.beta1; b2p *= (double)p.beta2; }  // per sample, pyx:544-547
+        if (p.sgd_mode == B200_ADAM) { b1p *= (double)p.beta1; b2p *= (double)p.beta2; }  // per sample, pyx:544-547
       }
     }
     ASY_MARK(4);
@@ -259,8 +259,7 @@ struct b200_asysvd_s {
   DevBuf<int> d_indptr, d_indices, su, si;
   DevBuf<float> sr, Y, X, bu, bi, mu, cY, cX, cbu, cbi, cmu, m2Y, m2X, m2bu, m2bi, m2mu;
   DevBuf<double> pow_out;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  bool timed = false;
+  EpochTimer timer;
   long long n_last = 0;
 };
 
@@ -305,7 +304,7 @@ int b200_asysvd_create(b200_asysvd_t* out, int64_t n_users, int64_t n_items, int
     B200_REQUIRE(out && h_indptr && h_indices && h_data && h_profile_factors && h_item_factors, "b200_asysvd_create: NULL argument");
     B200_REQUIRE(n_users > 0 && n_items > 0 && nnz > 0 && nnz < (1ll << 31) - 1, "b200_asysvd_create: bad shape");
     B200_REQUIRE(n_factors > 0 && n_factors <= 1024, "b200_asysvd_create: n_factors must be in [1, 1024] (got %d)", n_factors);
-    B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_asysvd_create: unknown sgd_mode %d", sgd_mode);
+    B200_REQUIRE(sgd_mode >= B200_SGD && sgd_mode <= B200_ADAM, "b200_asysvd_create: unknown sgd_mode %d", sgd_mode);
     h = new b200_asysvd_s();
     Params& p = h->p;
     const size_t f = (size_t)n_factors, fp = (f + 3) & ~(size_t)3, nf = (size_t)n_items * fp;
@@ -330,11 +329,11 @@ int b200_asysvd_create(b200_asysvd_t* out, int64_t n_users, int64_t n_items, int
     upload_rows(h->X, h_item_factors, (size_t)n_items, f, fp); p.X = h->X.get();
     zeros(h->bu, (size_t)n_users); zeros(h->bi, (size_t)n_items); zeros(h->mu, 1);  // pyx:184-186
     p.bu = h->bu.get(); p.bi = h->bi.get(); p.mu = h->mu.get();
-    if (sgd_mode != SGD) {  // pyx:248-270
+    if (sgd_mode != B200_SGD) {  // pyx:248-270
       zeros(h->cY, nf); zeros(h->cX, nf); zeros(h->cbu, (size_t)n_users); zeros(h->cbi, (size_t)n_items); zeros(h->cmu, 1);
       p.cY = h->cY.get(); p.cX = h->cX.get(); p.cbu = h->cbu.get(); p.cbi = h->cbi.get(); p.cmu = h->cmu.get();
     }
-    if (sgd_mode == ADAM) {
+    if (sgd_mode == B200_ADAM) {
       zeros(h->m2Y, nf); zeros(h->m2X, nf); zeros(h->m2bu, (size_t)n_users); zeros(h->m2bi, (size_t)n_items); zeros(h->m2mu, 1);
       p.m2Y = h->m2Y.get(); p.m2X = h->m2X.get(); p.m2bu = h->m2bu.get(); p.m2bi = h->m2bi.get(); p.m2mu = h->m2mu.get();
     }
@@ -343,8 +342,6 @@ int b200_asysvd_create(b200_asysvd_t* out, int64_t n_users, int64_t n_items, int
     p.su = h->su.get(); p.si = h->si.get(); p.sr = h->sr.get();
     h->pow_out.alloc(2);
     p.pow_out = h->pow_out.get();
-    B200_CUDA(cudaEventCreate(&h->ev0));
-    B200_CUDA(cudaEventCreate(&h->ev1));
     *out = h;
   });
   if (rc != B200_OK && h) delete h;
@@ -353,8 +350,6 @@ int b200_asysvd_create(b200_asysvd_t* out, int64_t n_users, int64_t n_items, int
 
 int b200_asysvd_destroy(b200_asysvd_t h) {
   if (!h) return B200_OK;
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
   delete h;
   return B200_OK;
 }
@@ -371,19 +366,17 @@ int b200_asysvd_epoch(b200_asysvd_t h, void* stream) {
     B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs.u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs.r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaEventRecord(h->ev0, st));
+    h->timer.begin(st);
     const size_t smem = (size_t)(WARPS + 2) * (size_t)p.fp * sizeof(float);
     // per launch: the attribute belongs to the function, and handles with other factor counts share it
     B200_CUDA(cudaFuncSetAttribute(asysvd_sequential_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1024)));
     asysvd_sequential_kernel<<<1, THREADS, smem, st>>>(p);
     B200_CUDA(cudaGetLastError());
     count_launch();
-    B200_CUDA(cudaEventRecord(h->ev1, st));
-    h->timed = true;
-    double pw[2];
-    B200_CUDA(cudaMemcpyAsync(pw, h->pow_out.get(), sizeof(pw), cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));  // the host sample buffers are reused by the next epoch
-    if (p.sgd_mode == ADAM) { p.b1_pow = pw[0]; p.b2_pow = pw[1]; }
+    h->timer.end(st);
+    // the host sample buffers are reused by the next epoch: both branches synchronise the stream
+    if (p.sgd_mode == B200_ADAM) read_powers(h->pow_out.get(), p.b1_pow, p.b2_pow, st);
+    else B200_CUDA(cudaStreamSynchronize(st));
     h->n_last = n;
   });
 }
@@ -412,9 +405,8 @@ int b200_asysvd_get_factors(b200_asysvd_t h, double* profile_factors, double* it
 
 int b200_asysvd_last_epoch_ms(b200_asysvd_t h, float* ms) {
   return guarded([&] {
-    B200_REQUIRE(h && ms && h->timed, "b200_asysvd_last_epoch_ms: no epoch run yet");
-    B200_CUDA(cudaEventSynchronize(h->ev1));
-    B200_CUDA(cudaEventElapsedTime(ms, h->ev0, h->ev1));
+    B200_REQUIRE(h && ms && h->timer.timed, "b200_asysvd_last_epoch_ms: no epoch run yet");
+    h->timer.elapsed(ms);
   });
 }
 

@@ -82,6 +82,31 @@ struct DevBuf {
   T* get() const { return p; }
 };
 
+// Device time of a handle's last call (an epoch, a kernel): events recorded around the work on the caller's stream
+struct EpochTimer {
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  bool timed = false;  // end() has run
+  EpochTimer() {
+    B200_CUDA(cudaEventCreate(&ev0));
+    B200_CUDA(cudaEventCreate(&ev1));
+  }
+  EpochTimer(const EpochTimer&) = delete;
+  EpochTimer& operator=(const EpochTimer&) = delete;
+  ~EpochTimer() {
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+  }
+  void begin(cudaStream_t st) { B200_CUDA(cudaEventRecord(ev0, st)); }
+  void end(cudaStream_t st) {
+    B200_CUDA(cudaEventRecord(ev1, st));
+    timed = true;
+  }
+  void elapsed(float* ms) const {  // waits for the end event
+    B200_CUDA(cudaEventSynchronize(ev1));
+    B200_CUDA(cudaEventElapsedTime(ms, ev0, ev1));
+  }
+};
+
 inline int sm_count() {
   int dev = 0, n = 0;
   B200_CUDA(cudaGetDevice(&dev));

@@ -31,6 +31,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "adaptive.cuh"
 #include "common.cuh"
 #include "sampler.cuh"
 
@@ -40,20 +41,18 @@ namespace b200 {
 namespace mf {
 
 enum Algo { MF_BPR = 0, FUNK_SVD = 1 };
-enum SgdMode { SGD = 0, ADAGRAD = 1, RMSPROP = 2, ADAM = 3 };
 
 struct Params {
-  int n_users, n_items, f, batch_size, algorithm, use_bias, sgd_mode, hogwild;
+  int n_users, n_items, f, batch_size, algorithm, use_bias, hogwild;
   float lr, user_reg, item_reg, bias_reg, positive_reg, negative_reg;
-  float gamma, beta1, beta2;
+  AdaptRule ad;  // mode and constants; the kernels set the bias corrections of each step
   double b1_pow, b2_pow;  // adam powers at the start of the epoch
   float *U, *V, *bu, *bi, *mu;
   // batch gradient sums are fp64 like pyx:305-354: a double atomic sum is order-independent to ~1e-16 relative, so the
   // mini-batch mode is run-to-run deterministic at the fp32 precision of the parameters (fp32 RED.ADD was not: the
   // summation order of a row's samples changed the rounded sum, and Adam's m/(sqrt(v)+eps) amplified it)
   double *accU, *accV, *accbu, *accbi, *accmu;
-  float *cU, *cV, *cbu, *cbi, *cmu;                                    // adagrad / rmsprop cache
-  float *m1U, *m2U, *m1V, *m2V, *m1bu, *m2bu, *m1bi, *m2bi, *m1mu, *m2mu;  // adam
+  AdaptState sU, sV, sbu, sbi, smu;  // adaptive state of U, V, bu, bi, mu
   int *flagI, *flagU, *listI, *listU, *cnt;  // cnt[4]: items/users counters, double-buffered by batch parity
   const int* su; const int* si; const int* sj; const float* sr;  // sample stream of the epoch
   long long n_batches;
@@ -65,31 +64,6 @@ struct Params {
   const int *slot_prev, *slot_expect;
   const float *inv1_b, *inv2_b;
 };
-
-struct AdaptCtx {
-  int mode;
-  float gamma, beta1, beta2, inv1, inv2;  // inv = 1 / (1 - beta^t)
-};
-
-// pyx:838-876 on one element; c / m1 / m2 point at this element's state
-__device__ __forceinline__ float adapt(const AdaptCtx& a, float g, float* c, float* m1, float* m2) {
-  if (a.mode == ADAGRAD) {
-    const float cc = *c + g * g;
-    *c = cc;
-    return g / (sqrtf(cc) + 1e-8f);
-  } else if (a.mode == RMSPROP) {
-    const float cc = *c * a.gamma + (1.f - a.gamma) * g * g;
-    *c = cc;
-    return g / (sqrtf(cc) + 1e-8f);
-  } else if (a.mode == ADAM) {
-    const float mm1 = *m1 * a.beta1 + (1.f - a.beta1) * g;
-    const float mm2 = *m2 * a.beta2 + (1.f - a.beta2) * g * g;
-    *m1 = mm1;
-    *m2 = mm2;
-    return (mm1 * a.inv1) / (sqrtf(mm2 * a.inv2) + 1e-8f);
-  }
-  return g;
-}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -169,22 +143,22 @@ __device__ __forceinline__ void mse_accumulate(const Params& p, int u, int i, fl
 }
 
 // ---- phase 2: one touched row takes its step (pyx:792-832)
-__device__ __forceinline__ void apply_row(const Params& p, const AdaptCtx& ad, float* P, double* acc, float* c, float* m1,
-                                          float* m2, size_t row, int lane, double inv_bs) {
+__device__ __forceinline__ void apply_row(const Params& p, const AdaptRule& ad, float* P, double* acc, const AdaptState& s,
+                                          size_t row, int lane, double inv_bs) {
   const int f = p.f;
   const size_t o = row * (size_t)f;
   for (int q = lane; q < f; q += 32) {
     float g = (float)(acc[o + q] * inv_bs);
-    g = adapt(ad, g, c ? c + o + q : nullptr, m1 ? m1 + o + q : nullptr, m2 ? m2 + o + q : nullptr);
+    g = adapt_at(ad, g, s, o + q);
     P[o + q] += p.lr * g;
     acc[o + q] = 0.0;
   }
 }
 
-__device__ __forceinline__ void apply_scalar(const Params& p, const AdaptCtx& ad, float* P, double* acc, float* c, float* m1,
-                                             float* m2, size_t k, double inv_bs) {
+__device__ __forceinline__ void apply_scalar(const Params& p, const AdaptRule& ad, float* P, double* acc, const AdaptState& s,
+                                             size_t k, double inv_bs) {
   float g = (float)(acc[k] * inv_bs);
-  g = adapt(ad, g, c ? c + k : nullptr, m1 ? m1 + k : nullptr, m2 ? m2 + k : nullptr);
+  g = adapt_at(ad, g, s, k);
   P[k] += p.lr * g;
   acc[k] = 0.0;
 }
@@ -197,8 +171,6 @@ __global__ void __launch_bounds__(256) mf_epoch_kernel(const Params p) {
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   const double inv_bs = 1.0 / (double)p.batch_size;
   double b1p = p.b1_pow, b2p = p.b2_pow;
-  AdaptCtx ad;
-  ad.mode = p.sgd_mode; ad.gamma = p.gamma; ad.beta1 = p.beta1; ad.beta2 = p.beta2;
   for (long long b = 0; b < p.n_batches; ++b) {
     int* cnt = p.cnt + 2 * (int)(b & 1);
     // ---------------- phase 1
@@ -216,25 +188,24 @@ __global__ void __launch_bounds__(256) mf_epoch_kernel(const Params p) {
     }
     grid.sync();
     // ---------------- phase 2
-    ad.inv1 = (float)(1.0 / (1.0 - b1p));
-    ad.inv2 = (float)(1.0 / (1.0 - b2p));
+    const AdaptRule ad{p.ad.mode, p.ad.gamma, p.ad.beta1, p.ad.beta2, adam_correction(b1p), adam_correction(b2p)};
     const int nI = cnt[0], nU = cnt[1];
-    if (p.use_bias && warp == 0 && lane == 0) apply_scalar(p, ad, p.mu, p.accmu, p.cmu, p.m1mu, p.m2mu, 0, inv_bs);
+    if (p.use_bias && warp == 0 && lane == 0) apply_scalar(p, ad, p.mu, p.accmu, p.smu, 0, inv_bs);
     for (long long t = warp; t < nI + nU; t += n_warps) {
       if (t < nI) {
         const int k = p.listI[t];
-        if (p.use_bias && lane == 0) apply_scalar(p, ad, p.bi, p.accbi, p.cbi, p.m1bi, p.m2bi, k, inv_bs);
-        apply_row(p, ad, p.V, p.accV, p.cV, p.m1V, p.m2V, k, lane, inv_bs);
+        if (p.use_bias && lane == 0) apply_scalar(p, ad, p.bi, p.accbi, p.sbi, k, inv_bs);
+        apply_row(p, ad, p.V, p.accV, p.sV, k, lane, inv_bs);
         if (lane == 0) p.flagI[k] = 0;
       } else {
         const int k = p.listU[t - nI];
-        if (p.use_bias && lane == 0) apply_scalar(p, ad, p.bu, p.accbu, p.cbu, p.m1bu, p.m2bu, k, inv_bs);
-        apply_row(p, ad, p.U, p.accU, p.cU, p.m1U, p.m2U, k, lane, inv_bs);
+        if (p.use_bias && lane == 0) apply_scalar(p, ad, p.bu, p.accbu, p.sbu, k, inv_bs);
+        apply_row(p, ad, p.U, p.accU, p.sU, k, lane, inv_bs);
         if (lane == 0) p.flagU[k] = 0;
       }
     }
     if (warp == 0 && lane == 0) { int* nxt = p.cnt + 2 * (int)((b + 1) & 1); nxt[0] = 0; nxt[1] = 0; }
-    if (p.sgd_mode == ADAM) { b1p *= (double)p.beta1; b2p *= (double)p.beta2; }  // once per batch, pyx:649-652
+    if (p.ad.mode == B200_ADAM) { b1p *= (double)p.ad.beta1; b2p *= (double)p.ad.beta2; }  // once per batch, pyx:649-652
     grid.sync();
   }
   if (warp == 0 && lane == 0) { p.pow_out[0] = b1p; p.pow_out[1] = b2p; p.cnt[0] = p.cnt[1] = p.cnt[2] = p.cnt[3] = 0; }
@@ -246,17 +217,16 @@ __global__ void __launch_bounds__(256) mf_hogwild_kernel(const Params p, long lo
   const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   const int f = p.f;
-  AdaptCtx ad;
-  ad.mode = p.sgd_mode; ad.gamma = p.gamma; ad.beta1 = p.beta1; ad.beta2 = p.beta2;
+  AdaptRule ad = p.ad;
   for (long long g = warp; g < n_samples; g += n_warps) {
-    if (p.sgd_mode == ADAM) {  // the reference advances the powers once per (size-1) batch
-      ad.inv1 = (float)(1.0 / (1.0 - p.b1_pow * pow((double)p.beta1, (double)g)));
-      ad.inv2 = (float)(1.0 / (1.0 - p.b2_pow * pow((double)p.beta2, (double)g)));
+    if (ad.mode == B200_ADAM) {  // the reference advances the powers once per (size-1) batch
+      ad.inv1 = adam_correction(p.b1_pow * pow((double)ad.beta1, (double)g));
+      ad.inv2 = adam_correction(p.b2_pow * pow((double)ad.beta2, (double)g));
     }
     const int u = p.su[g], i = p.si[g];
     float* Uu = p.U + (size_t)u * f;
     float* Vi = p.V + (size_t)i * f;
-    if (p.algorithm == MF_BPR && p.sgd_mode == SGD && (f & 3) == 0) {
+    if (p.algorithm == MF_BPR && ad.mode == B200_SGD && (f & 3) == 0) {
       // plain-SGD BPR, rows as float4: one 16-byte load and store per lane and row for f = 128
       const int j = p.sj[g];
       float* Vj = p.V + (size_t)j * f;
@@ -291,9 +261,9 @@ __global__ void __launch_bounds__(256) mf_hogwild_kernel(const Params p, long lo
         const float a = Uu[q], b = Vi[q], c = Vj[q];
         const size_t oi = (size_t)i * f + q, oj = (size_t)j * f + q, ou = (size_t)u * f + q;
         // items first, then the user, as pyx:792-832 orders the apply
-        atomicAdd(Vi + q, p.lr * adapt(ad, sig * a - p.positive_reg * b, p.cV ? p.cV + oi : nullptr, p.m1V ? p.m1V + oi : nullptr, p.m2V ? p.m2V + oi : nullptr));
-        atomicAdd(Vj + q, p.lr * adapt(ad, -sig * a - p.negative_reg * c, p.cV ? p.cV + oj : nullptr, p.m1V ? p.m1V + oj : nullptr, p.m2V ? p.m2V + oj : nullptr));
-        atomicAdd(Uu + q, p.lr * adapt(ad, sig * (b - c) - p.user_reg * a, p.cU ? p.cU + ou : nullptr, p.m1U ? p.m1U + ou : nullptr, p.m2U ? p.m2U + ou : nullptr));
+        atomicAdd(Vi + q, p.lr * adapt_at(ad, sig * a - p.positive_reg * b, p.sV, oi));
+        atomicAdd(Vj + q, p.lr * adapt_at(ad, -sig * a - p.negative_reg * c, p.sV, oj));
+        atomicAdd(Uu + q, p.lr * adapt_at(ad, sig * (b - c) - p.user_reg * a, p.sU, ou));
       }
     } else {
       float x = 0.f;
@@ -302,15 +272,15 @@ __global__ void __launch_bounds__(256) mf_hogwild_kernel(const Params p, long lo
       if (p.use_bias) x += p.mu[0] + p.bu[u] + p.bi[i];
       const float err = p.sr[g] - x;
       if (p.use_bias && lane == 0) {
-        p.mu[0] += p.lr * adapt(ad, err - p.bias_reg * p.mu[0], p.cmu, p.m1mu, p.m2mu);
-        p.bi[i] += p.lr * adapt(ad, err - p.bias_reg * p.bi[i], p.cbi ? p.cbi + i : nullptr, p.m1bi ? p.m1bi + i : nullptr, p.m2bi ? p.m2bi + i : nullptr);
-        p.bu[u] += p.lr * adapt(ad, err - p.bias_reg * p.bu[u], p.cbu ? p.cbu + u : nullptr, p.m1bu ? p.m1bu + u : nullptr, p.m2bu ? p.m2bu + u : nullptr);
+        p.mu[0] += p.lr * adapt_at(ad, err - p.bias_reg * p.mu[0], p.smu, 0);
+        p.bi[i] += p.lr * adapt_at(ad, err - p.bias_reg * p.bi[i], p.sbi, i);
+        p.bu[u] += p.lr * adapt_at(ad, err - p.bias_reg * p.bu[u], p.sbu, u);
       }
       for (int q = lane; q < f; q += 32) {
         const float a = Uu[q], b = Vi[q];
         const size_t oi = (size_t)i * f + q, ou = (size_t)u * f + q;
-        atomicAdd(Vi + q, p.lr * adapt(ad, err * a - p.positive_reg * b, p.cV ? p.cV + oi : nullptr, p.m1V ? p.m1V + oi : nullptr, p.m2V ? p.m2V + oi : nullptr));
-        atomicAdd(Uu + q, p.lr * adapt(ad, err * b - p.user_reg * a, p.cU ? p.cU + ou : nullptr, p.m1U ? p.m1U + ou : nullptr, p.m2U ? p.m2U + ou : nullptr));
+        atomicAdd(Vi + q, p.lr * adapt_at(ad, err * a - p.positive_reg * b, p.sV, oi));
+        atomicAdd(Uu + q, p.lr * adapt_at(ad, err * b - p.user_reg * a, p.sU, ou));
       }
     }
   }
@@ -337,54 +307,35 @@ __device__ __forceinline__ void st_relaxed(int* p, int v) { asm volatile("st.rel
 // it reads the rows; after its last write it executes ONE fence (release side) and then publishes with relaxed stores /
 // the arrival atomics.  fence + relaxed access is the PTX release / acquire pattern; one fence serves all three rows.
 
-// pyx:838-876 on one element with L2-only accesses to the state
-__device__ __forceinline__ float adapt_cg(const AdaptCtx& a, float g, float* c, float* m1, float* m2) {
-  if (a.mode == ADAGRAD) {
-    const float cc = __ldcg(c) + g * g;
-    __stcg(c, cc);
-    return g / (sqrtf(cc) + 1e-8f);
-  } else if (a.mode == RMSPROP) {
-    const float cc = __ldcg(c) * a.gamma + (1.f - a.gamma) * g * g;
-    __stcg(c, cc);
-    return g / (sqrtf(cc) + 1e-8f);
-  } else if (a.mode == ADAM) {
-    const float mm1 = __ldcg(m1) * a.beta1 + (1.f - a.beta1) * g;
-    const float mm2 = __ldcg(m2) * a.beta2 + (1.f - a.beta2) * g * g;
-    __stcg(m1, mm1);
-    __stcg(m2, mm2);
-    return (mm1 * a.inv1) / (sqrtf(mm2 * a.inv2) + 1e-8f);
-  }
-  return g;
-}
-
 // one row's share of a sample: either the row's whole step (it is hit once in this batch) or a contribution to its sum
 struct SlotCtx {
-  float* P; double* acc; float *c, *m1, *m2;  // row base pointers (state pointers may be null)
+  float* P; double* acc;  // row base pointers
+  AdaptState s; size_t o;  // the table's state, the row's first element in it
   bool direct;
 };
 // returns the element's new value when the slot steps directly (the caller stores it), `old` otherwise
-__device__ __forceinline__ float slot_element(const Params& p, const AdaptCtx& ad, const SlotCtx& s, int q, float old, double term,
+__device__ __forceinline__ float slot_element(const Params& p, const AdaptRule& ad, const SlotCtx& s, int q, float old, double term,
                                               double inv_bs) {
   if (s.direct) {
     float g = (float)(term * inv_bs);  // what apply_row computes from a one-term sum
-    g = adapt_cg(ad, g, s.c ? s.c + q : nullptr, s.m1 ? s.m1 + q : nullptr, s.m2 ? s.m2 + q : nullptr);
+    g = adapt_at<L2Access>(ad, g, s.s, s.o + q);
     return old + p.lr * g;
   }
   atomicAdd(s.acc + q, term);
   return old;
 }
 // the step of a row whose sum is complete (pyx:792-832), L2-only accesses
-__device__ __forceinline__ void apply_row_cg(const Params& p, const AdaptCtx& ad, const SlotCtx& s, int lane, double inv_bs) {
+__device__ __forceinline__ void apply_row_cg(const Params& p, const AdaptRule& ad, const SlotCtx& s, int lane, double inv_bs) {
   for (int q = lane; q < p.f; q += 32) {
     float g = (float)(__ldcg(s.acc + q) * inv_bs);
-    g = adapt_cg(ad, g, s.c ? s.c + q : nullptr, s.m1 ? s.m1 + q : nullptr, s.m2 ? s.m2 + q : nullptr);
+    g = adapt_at<L2Access>(ad, g, s.s, s.o + q);
     __stcg(s.P + q, __ldcg(s.P + q) + p.lr * g);
     __stcg(s.acc + q, 0.0);
   }
 }
 // after the release fence: publish a directly stepped row, or count the arrival at a shared row and, as the last sample
 // to arrive, take the row's step
-__device__ __forceinline__ void slot_publish(const Params& p, const AdaptCtx& ad, const SlotCtx& s, int row, int expect, int batch,
+__device__ __forceinline__ void slot_publish(const Params& p, const AdaptRule& ad, const SlotCtx& s, int row, int expect, int batch,
                                              int lane, double inv_bs) {
   if (s.direct) {
     if (lane == 0) st_relaxed(p.applied + row, batch);
@@ -414,8 +365,6 @@ __global__ void __launch_bounds__(256, 3) mf_dataflow_kernel(const Params p, lon
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   const int f = p.f, nU = p.n_users;
   const double inv_bs = 1.0 / (double)p.batch_size;
-  AdaptCtx ad;
-  ad.mode = p.sgd_mode; ad.gamma = p.gamma; ad.beta1 = p.beta1; ad.beta2 = p.beta2; ad.inv1 = ad.inv2 = 1.f;
   const double rp = (double)p.positive_reg, rn = (double)p.negative_reg, rgu = (double)p.user_reg;
   for (long long g = warp; g < n_samples; g += n_warps) {
     const int batch = (int)(g / p.batch_size);
@@ -424,7 +373,8 @@ __global__ void __launch_bounds__(256, 3) mf_dataflow_kernel(const Params p, lon
     const long long s0 = g * S;
     const int pu = p.slot_prev[s0], pi = p.slot_prev[s0 + 1], pj = BPR ? p.slot_prev[s0 + 2] : 0;
     const int eu = p.slot_expect[s0], ei = p.slot_expect[s0 + 1], ej = BPR ? p.slot_expect[s0 + 2] : 0;
-    if (p.sgd_mode == ADAM) { ad.inv1 = p.inv1_b[batch]; ad.inv2 = p.inv2_b[batch]; }
+    const bool adam = p.ad.mode == B200_ADAM;
+    const AdaptRule ad{p.ad.mode, p.ad.gamma, p.ad.beta1, p.ad.beta2, adam ? p.inv1_b[batch] : 1.f, adam ? p.inv2_b[batch] : 1.f};
     // ---- wait for the three rows' previous steps
     {
       unsigned ns = 20;
@@ -440,9 +390,9 @@ __global__ void __launch_bounds__(256, 3) mf_dataflow_kernel(const Params p, lon
     float* Vi = p.V + (size_t)i * f;
     float* Vj = p.V + (size_t)j * f;
     const size_t ou = (size_t)u * f, oi = (size_t)i * f, oj = (size_t)j * f;
-    SlotCtx su_{Uu, p.accU + ou, p.cU ? p.cU + ou : nullptr, p.m1U ? p.m1U + ou : nullptr, p.m2U ? p.m2U + ou : nullptr, eu == 1};
-    SlotCtx si_{Vi, p.accV + oi, p.cV ? p.cV + oi : nullptr, p.m1V ? p.m1V + oi : nullptr, p.m2V ? p.m2V + oi : nullptr, ei == 1};
-    SlotCtx sj_{Vj, p.accV + oj, p.cV ? p.cV + oj : nullptr, p.m1V ? p.m1V + oj : nullptr, p.m2V ? p.m2V + oj : nullptr, ej == 1};
+    SlotCtx su_{Uu, p.accU + ou, p.sU, ou, eu == 1};
+    SlotCtx si_{Vi, p.accV + oi, p.sV, oi, ei == 1};
+    SlotCtx sj_{Vj, p.accV + oj, p.sV, oj, ej == 1};
     if (ONE4) {
       const int q = lane * 4;
       const bool on = q < f;
@@ -689,8 +639,7 @@ struct b200_mf_s {
   size_t sort_tmp_bytes = 0;
   DevBuf<float> inv1_b, inv2_b;
   std::vector<float> h_inv1, h_inv2;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  bool timed = false;
+  EpochTimer timer;
   float* falloc(size_t n, const double* init) {
     fbufs.emplace_back(std::max<size_t>(n, 1));
     float* d = fbufs.back().get();
@@ -785,16 +734,16 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
     B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_mf_create: bad shape");
     B200_REQUIRE(n_factors >= 1 && batch_size >= 1, "b200_mf_create: n_factors and batch_size must be >= 1");
     B200_REQUIRE(algorithm == MF_BPR || algorithm == FUNK_SVD, "b200_mf_create: unknown algorithm %d", algorithm);
-    B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_mf_create: unknown sgd_mode %d", sgd_mode);
+    B200_REQUIRE(sgd_mode >= B200_SGD && sgd_mode <= B200_ADAM, "b200_mf_create: unknown sgd_mode %d", sgd_mode);
     B200_REQUIRE(sampler == 0 || has_sampleable_user(h_indptr, 0, n_users, n_items),
                  "b200_mf_create: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
     h = new b200_mf_s();
     Params& p = h->p;
     p.n_users = (int)n_users; p.n_items = (int)n_items; p.f = n_factors; p.batch_size = batch_size;
-    p.algorithm = algorithm; p.use_bias = use_bias != 0; p.sgd_mode = sgd_mode; p.hogwild = hogwild != 0;
+    p.algorithm = algorithm; p.use_bias = use_bias != 0; p.hogwild = hogwild != 0;
     p.lr = learning_rate; p.user_reg = user_reg; p.item_reg = item_reg; p.bias_reg = bias_reg;
     p.positive_reg = positive_reg; p.negative_reg = negative_reg;
-    p.gamma = gamma; p.beta1 = beta_1; p.beta2 = beta_2;
+    p.ad = {sgd_mode, gamma, beta_1, beta_2, 1.f, 1.f};
     p.b1_pow = beta_1; p.b2_pow = beta_2;  // pyx:220-221
     h->nnz = nnz;
     h->quota = negative_interactions_quota;
@@ -823,17 +772,12 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
       p.bu = h->falloc((size_t)n_users, nullptr); p.bi = h->falloc((size_t)n_items, nullptr); p.mu = h->falloc(1, nullptr);
       p.accbu = h->dalloc((size_t)n_users); p.accbi = h->dalloc((size_t)n_items); p.accmu = h->dalloc(1);
     }
-    if (sgd_mode == ADAGRAD || sgd_mode == RMSPROP) {
-      p.cU = h->falloc(nUf, nullptr); p.cV = h->falloc(nIf, nullptr);
-      if (p.use_bias) { p.cbu = h->falloc((size_t)n_users, nullptr); p.cbi = h->falloc((size_t)n_items, nullptr); p.cmu = h->falloc(1, nullptr); }
-    } else if (sgd_mode == ADAM) {
-      p.m1U = h->falloc(nUf, nullptr); p.m2U = h->falloc(nUf, nullptr); p.m1V = h->falloc(nIf, nullptr); p.m2V = h->falloc(nIf, nullptr);
-      if (p.use_bias) {
-        p.m1bu = h->falloc((size_t)n_users, nullptr); p.m2bu = h->falloc((size_t)n_users, nullptr);
-        p.m1bi = h->falloc((size_t)n_items, nullptr); p.m2bi = h->falloc((size_t)n_items, nullptr);
-        p.m1mu = h->falloc(1, nullptr); p.m2mu = h->falloc(1, nullptr);
-      }
-    }
+    // adaptive state: s1 in every adaptive mode, s2 in Adam only
+    auto state = [&](size_t n) {
+      return AdaptState{sgd_mode != B200_SGD ? h->falloc(n, nullptr) : nullptr, sgd_mode == B200_ADAM ? h->falloc(n, nullptr) : nullptr};
+    };
+    p.sU = state(nUf); p.sV = state(nIf);
+    if (p.use_bias) { p.sbu = state((size_t)n_users); p.sbi = state((size_t)n_items); p.smu = state(1); }
     h->flagI.alloc((size_t)n_items); h->flagU.alloc((size_t)n_users);
     h->listI.alloc((size_t)2 * batch_size); h->listU.alloc((size_t)batch_size); h->cnt.alloc(4);
     B200_CUDA(cudaMemset(h->flagI.get(), 0, sizeof(int) * (size_t)n_items));
@@ -875,7 +819,7 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
       cub::DoubleBuffer<int> dv(h->vals_a.get(), h->vals_b.get());
       B200_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, h->sort_tmp_bytes, dk, dv, (int)slots, 0, h->bbits + h->rbits));
       h->sort_tmp.alloc(h->sort_tmp_bytes + 16);
-      if (sgd_mode == ADAM) { h->inv1_b.alloc((size_t)nb); h->inv2_b.alloc((size_t)nb); }
+      if (sgd_mode == B200_ADAM) { h->inv1_b.alloc((size_t)nb); h->inv2_b.alloc((size_t)nb); }
       p.applied = h->applied.get(); p.arrived = h->arrived.get();
       p.slot_prev = h->slot_prev.get(); p.slot_expect = h->slot_expect.get();
       p.inv1_b = h->inv1_b.get(); p.inv2_b = h->inv2_b.get();
@@ -884,8 +828,6 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
       B200_REQUIRE(per_sm_df >= 1, "b200_mf_create: dataflow kernel does not fit on an SM");
       h->df_grid = sm_count() * std::min(per_sm_df, 8);
     }
-    B200_CUDA(cudaEventCreate(&h->ev0));
-    B200_CUDA(cudaEventCreate(&h->ev1));
     *out = h;
   });
   if (rc != B200_OK && h) delete h;
@@ -894,8 +836,6 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
 
 int b200_mf_destroy(b200_mf_t h) {
   if (!h) return B200_OK;
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->h_raw) cudaFreeHost(h->h_raw);
   delete h;
   return B200_OK;
@@ -918,7 +858,7 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
       if (p.algorithm == MF_BPR) B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs.j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
       else B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs.r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
     }
-    B200_CUDA(cudaEventRecord(h->ev0, st));
+    h->timer.begin(st);
     if (h->sampler != 0) {
       mf_sample_kernel<<<div_up(n, 256), 256, 0, st>>>(h->d_indptr.get(), h->d_indices.get(), h->d_data.get(), h->shard_lo,
                                                       (h->shard_hi > h->shard_lo ? h->shard_hi - h->shard_lo : p.n_users), p.n_items,
@@ -929,10 +869,7 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
     if (p.hogwild) {
       mf_hogwild_kernel<<<sm_count() * h->hog_blocks, 256, 0, st>>>(p, n);
       B200_CUDA(cudaGetLastError());
-      if (p.sgd_mode == ADAM) {  // powers advance once per size-1 batch
-        p.b1_pow *= pow((double)p.beta1, (double)n);
-        p.b2_pow *= pow((double)p.beta2, (double)n);
-      }
+      if (p.ad.mode == B200_ADAM) advance_powers(p.ad.beta1, p.ad.beta2, p.b1_pow, p.b2_pow, (double)n);  // once per size-1 batch
     } else if (h->dataflow) {
       // dependency tables of this epoch's stream: (row, batch) keys sorted, run heads give hit counts and previous batches
       const bool bpr = p.algorithm == MF_BPR;
@@ -949,13 +886,13 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
       mf_deps_kernel<<<div_up(m, 256), 256, 0, st>>>(dk.Current(), dv.Current(), m, h->bbits, h->slot_prev.get(), h->slot_expect.get());
       count_launch();
       B200_CUDA(cudaMemsetAsync(h->applied.get(), 0xFF, sizeof(int) * ((size_t)p.n_users + (size_t)p.n_items), st));  // -1
-      if (p.sgd_mode == ADAM) {  // the powers advance once per batch (pyx:649-652), the same repeated product as the other kernel
+      if (p.ad.mode == B200_ADAM) {  // the powers advance once per batch (pyx:649-652), the same repeated product as the other kernel
         h->h_inv1.resize((size_t)p.n_batches); h->h_inv2.resize((size_t)p.n_batches);
         double b1p = p.b1_pow, b2p = p.b2_pow;
         for (long long b = 0; b < p.n_batches; ++b) {
-          h->h_inv1[(size_t)b] = (float)(1.0 / (1.0 - b1p));
-          h->h_inv2[(size_t)b] = (float)(1.0 / (1.0 - b2p));
-          b1p *= (double)p.beta1; b2p *= (double)p.beta2;
+          h->h_inv1[(size_t)b] = adam_correction(b1p);
+          h->h_inv2[(size_t)b] = adam_correction(b2p);
+          b1p *= (double)p.ad.beta1; b2p *= (double)p.ad.beta2;
         }
         B200_CUDA(cudaMemcpyAsync(h->inv1_b.get(), h->h_inv1.data(), sizeof(float) * (size_t)p.n_batches, cudaMemcpyHostToDevice, st));
         B200_CUDA(cudaMemcpyAsync(h->inv2_b.get(), h->h_inv2.data(), sizeof(float) * (size_t)p.n_batches, cudaMemcpyHostToDevice, st));
@@ -971,16 +908,11 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
       else B200_CUDA(cudaLaunchCooperativeKernel((void*)mf_epoch_kernel<false>, dim3(h->grid), dim3(256), args, 0, st));
     }
     count_launch();
-    B200_CUDA(cudaEventRecord(h->ev1, st));
-    h->timed = true;
-    if (h->dataflow && p.sgd_mode == ADAM) {
+    h->timer.end(st);
+    if (h->dataflow && p.ad.mode == B200_ADAM) {
       B200_CUDA(cudaStreamSynchronize(st));  // the host-side inv tables are reused by the next epoch
-    } else if (!p.hogwild && p.sgd_mode == ADAM) {
-      double pw[2];
-      B200_CUDA(cudaMemcpyAsync(pw, h->pow_out.get(), sizeof(pw), cudaMemcpyDeviceToHost, st));
-      B200_CUDA(cudaStreamSynchronize(st));
-      p.b1_pow = pw[0];
-      p.b2_pow = pw[1];
+    } else if (!p.hogwild && p.ad.mode == B200_ADAM) {
+      read_powers(h->pow_out.get(), p.b1_pow, p.b2_pow, st);
     } else if (h->sampler == 0 && !(h->glibc_device && n * 4 + 65536 < (1ll << 30))) {
       B200_CUDA(cudaStreamSynchronize(st));  // the host sample vectors are reused by the next epoch
     }
@@ -1075,9 +1007,8 @@ int b200_mf_delta_apply_device(float* d_V, float* d_B, const float* d_sum, const
 
 int b200_mf_last_epoch_ms(b200_mf_t h, float* ms) {
   return guarded([&] {
-    B200_REQUIRE(h && ms && h->timed, "b200_mf_last_epoch_ms: no epoch run yet");
-    B200_CUDA(cudaEventSynchronize(h->ev1));
-    B200_CUDA(cudaEventElapsedTime(ms, h->ev0, h->ev1));
+    B200_REQUIRE(h && ms && h->timer.timed, "b200_mf_last_epoch_ms: no epoch run yet");
+    h->timer.elapsed(ms);
   });
 }
 

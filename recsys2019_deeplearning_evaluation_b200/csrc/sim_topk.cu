@@ -1152,8 +1152,7 @@ struct b200_sim_s {
   bool order_k1c = false;
   DevBuf<unsigned long long> prof;
   bool prof_on = false;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  bool timed = false;
+  EpochTimer timer;
 };
 
 namespace {
@@ -1173,8 +1172,6 @@ void build(b200_sim_s* h, const int32_t* h_indptr, const int32_t* h_indices, con
   const long long nnz = h->nnz;
   const size_t nnz1 = (size_t)std::max<long long>(nnz, 1);
   h->n_sm = sm_count();
-  B200_CUDA(cudaEventCreate(&h->ev0));
-  B200_CUDA(cudaEventCreate(&h->ev1));
 
   h->csr_ptr.alloc((size_t)n_rows + 1);
   DevBuf<int> idx_old(nnz1);
@@ -1532,8 +1529,6 @@ int b200_sim_create_euclidean(b200_sim_t* out, int64_t n_rows, int64_t n_cols, i
 
 int b200_sim_destroy(b200_sim_t h) {
   if (!h) return B200_OK;
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
   delete h;
   return B200_OK;
 }
@@ -1601,7 +1596,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
   p.dense_out = d_dense;
   p.prof = h->prof_on ? h->prof.get() : nullptr;
   p.n_range_dev = nullptr;
-  B200_CUDA(cudaEventRecord(h->ev0, st));
+  h->timer.begin(st);
   if (n_sparse > 0) k1d_launch(h, p, n_sparse, pair_path, st);  // the pair path implies n_sparse > 0
   if (n_dense > 0 || n_sparse > 0) {
     const int grid = n_sparse > 0 ? h->n_sm : std::min(n_dense, h->n_sm);
@@ -1609,8 +1604,7 @@ static void launch_topk(b200_sim_t h, int start_col, int end_col, int32_t* d_idx
     B200_CUDA(cudaGetLastError());
     count_launch();
   }
-  B200_CUDA(cudaEventRecord(h->ev1, st));
-  h->timed = true;
+  h->timer.end(st);
 }
 
 int b200_sim_compute_device(b200_sim_t h, int start_col, int end_col, int32_t* d_idx, float* d_val, int32_t* d_cnt,
@@ -1739,9 +1733,8 @@ int b200_sim_debug_pair_lists(b200_sim_t h, int set_tile_log2, int* tile_log2, i
 int b200_sim_last_kernel_ms(b200_sim_t h, float* ms) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr && ms != nullptr, "b200_sim_last_kernel_ms: NULL argument");
-    B200_REQUIRE(h->timed, "b200_sim_last_kernel_ms: no kernel launched yet");
-    B200_CUDA(cudaEventSynchronize(h->ev1));
-    B200_CUDA(cudaEventElapsedTime(ms, h->ev0, h->ev1));
+    B200_REQUIRE(h->timer.timed, "b200_sim_last_kernel_ms: no kernel launched yet");
+    h->timer.elapsed(ms);
   });
 }
 

@@ -24,14 +24,13 @@
 #include <algorithm>
 #include <vector>
 
+#include "adaptive.cuh"
 #include "common.cuh"
 #include "sampler.cuh"
 #include "select.cuh"
 
 namespace b200 {
 namespace slim {
-
-enum SgdMode { SGD = 0, ADAGRAD = 1, RMSPROP = 2, ADAM = 3 };
 
 struct Params {
   int n_users, n_items, symmetric, sgd_mode;
@@ -58,15 +57,15 @@ __device__ __forceinline__ size_t cell(const Params& p, int a, int b) {
 }
 
 __device__ __forceinline__ float adapt_item(const Params& p, float g, int item, float inv1, float inv2) {  // pyx:395-433
-  if (p.sgd_mode == ADAGRAD) {
+  if (p.sgd_mode == B200_ADAGRAD) {
     const float cc = p.c[item] + g * g;
     p.c[item] = cc;
     return g / (sqrtf(cc) + 1e-8f);
-  } else if (p.sgd_mode == RMSPROP) {
+  } else if (p.sgd_mode == B200_RMSPROP) {
     const float cc = p.c[item] * p.gamma + (1.f - p.gamma) * g * g;
     p.c[item] = cc;
     return g / (sqrtf(cc) + 1e-8f);
-  } else if (p.sgd_mode == ADAM) {
+  } else if (p.sgd_mode == B200_ADAM) {
     const float a = p.m1[item] * p.beta1 + (1.f - p.beta1) * g;
     const float b = p.m2[item] * p.beta2 + (1.f - p.beta2) * g * g;
     p.m1[item] = a;
@@ -120,8 +119,8 @@ __global__ void __launch_bounds__(SEQ_THREADS) slim_sequential_kernel(const Para
     // thread 0: the adaptive state of i and j, in flight during the gather (pyx:395-433 reads it after the gradient)
     float st_i0 = 0.f, st_i1 = 0.f, st_j0 = 0.f, st_j1 = 0.f;
     if (tid == 0) {
-      if (p.sgd_mode == ADAGRAD || p.sgd_mode == RMSPROP) { st_i0 = p.c[i]; st_j0 = p.c[j]; }
-      else if (p.sgd_mode == ADAM) { st_i0 = p.m1[i]; st_i1 = p.m2[i]; st_j0 = p.m1[j]; st_j1 = p.m2[j]; }
+      if (p.sgd_mode == B200_ADAGRAD || p.sgd_mode == B200_RMSPROP) { st_i0 = p.c[i]; st_j0 = p.c[j]; }
+      else if (p.sgd_mode == B200_ADAM) { st_i0 = p.m1[i]; st_i1 = p.m2[i]; st_j0 = p.m1[j]; st_j1 = p.m2[j]; }
     }
     float x = 0.f;
     int nsn0 = -1;
@@ -154,15 +153,15 @@ __global__ void __launch_bounds__(SEQ_THREADS) slim_sequential_kernel(const Para
       for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
       if (lane == 0) {
         const float g = 1.f / (1.f + expf(t));  // pyx:258
-        const float inv1 = (float)(1.0 / (1.0 - b1p)), inv2 = (float)(1.0 / (1.0 - b2p));
+        const float inv1 = adam_correction(b1p), inv2 = adam_correction(b2p);
         float gi = g, gj = g;  // i first, then j (pyx:262-263); i != j always (j is not in the profile, i is)
-        if (p.sgd_mode == ADAGRAD) {
+        if (p.sgd_mode == B200_ADAGRAD) {
           st_i0 += g * g; gi = g / (sqrtf(st_i0) + 1e-8f); p.c[i] = st_i0;
           st_j0 += g * g; gj = g / (sqrtf(st_j0) + 1e-8f); p.c[j] = st_j0;
-        } else if (p.sgd_mode == RMSPROP) {
+        } else if (p.sgd_mode == B200_RMSPROP) {
           st_i0 = st_i0 * p.gamma + (1.f - p.gamma) * g * g; gi = g / (sqrtf(st_i0) + 1e-8f); p.c[i] = st_i0;
           st_j0 = st_j0 * p.gamma + (1.f - p.gamma) * g * g; gj = g / (sqrtf(st_j0) + 1e-8f); p.c[j] = st_j0;
-        } else if (p.sgd_mode == ADAM) {
+        } else if (p.sgd_mode == B200_ADAM) {
           st_i0 = st_i0 * p.beta1 + (1.f - p.beta1) * g; st_i1 = st_i1 * p.beta2 + (1.f - p.beta2) * g * g;
           gi = (st_i0 * inv1) / (sqrtf(st_i1 * inv2) + 1e-8f); p.m1[i] = st_i0; p.m2[i] = st_i1;
           st_j0 = st_j0 * p.beta1 + (1.f - p.beta1) * g; st_j1 = st_j1 * p.beta2 + (1.f - p.beta2) * g * g;
@@ -192,7 +191,7 @@ __global__ void __launch_bounds__(SEQ_THREADS) slim_sequential_kernel(const Para
         { const float v = p.val[b]; p.val[b] = v - p.lr * (gj - p.lj_reg * v); }  // s != j: j is not in the profile
       }
     }
-    if (p.sgd_mode == ADAM) { b1p *= (double)p.beta1; b2p *= (double)p.beta2; }  // per sample, pyx:309-312
+    if (p.sgd_mode == B200_ADAM) { b1p *= (double)p.beta1; b2p *= (double)p.beta2; }  // per sample, pyx:309-312
     u = nu; i = ni; j = nj; s = ns; e = ne; sn0 = nsn0;
     base = nbase; ci0 = nci0; cj0 = ncj0;
     nu = nnu; ni = nni; nj = nnj;
@@ -226,11 +225,11 @@ __global__ void __launch_bounds__(256) slim_hogwild_kernel(const Params p) {
     for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
     const float g = 1.f / (1.f + expf(x));
     float gi = g, gj = g;
-    if (p.sgd_mode != SGD) {
+    if (p.sgd_mode != B200_SGD) {
       float inv1 = 1.f, inv2 = 1.f;
-      if (p.sgd_mode == ADAM) {
-        inv1 = (float)(1.0 / (1.0 - p.b1_pow * pow((double)p.beta1, (double)n)));
-        inv2 = (float)(1.0 / (1.0 - p.b2_pow * pow((double)p.beta2, (double)n)));
+      if (p.sgd_mode == B200_ADAM) {
+        inv1 = adam_correction(p.b1_pow * pow((double)p.beta1, (double)n));
+        inv2 = adam_correction(p.b2_pow * pow((double)p.beta2, (double)n));
       }
       if (lane == 0) { gi = adapt_item(p, g, i, inv1, inv2); gj = adapt_item(p, g, j, inv1, inv2); }
       gi = __shfl_sync(0xffffffffu, gi, 0);
@@ -281,9 +280,9 @@ __global__ void __launch_bounds__(256) slim_shard_partial_kernel(const ShardPara
 // the adaptive scale of one gradient from the item's state AS OF THE START OF THE BATCH plus this sample's own contribution
 // (pyx:395-433 without the store); with one sample per batch this is the reference's value exactly
 __device__ __forceinline__ float adapt_item_frozen(const Params& p, float g, int item, float inv1, float inv2) {
-  if (p.sgd_mode == ADAGRAD) return g / (sqrtf(p.c[item] + g * g) + 1e-8f);
-  if (p.sgd_mode == RMSPROP) return g / (sqrtf(p.c[item] * p.gamma + (1.f - p.gamma) * g * g) + 1e-8f);
-  if (p.sgd_mode == ADAM) {
+  if (p.sgd_mode == B200_ADAGRAD) return g / (sqrtf(p.c[item] + g * g) + 1e-8f);
+  if (p.sgd_mode == B200_RMSPROP) return g / (sqrtf(p.c[item] * p.gamma + (1.f - p.gamma) * g * g) + 1e-8f);
+  if (p.sgd_mode == B200_ADAM) {
     const float a = p.m1[item] * p.beta1 + (1.f - p.beta1) * g;
     const float b = p.m2[item] * p.beta2 + (1.f - p.beta2) * g * g;
     return (a * inv1) / (sqrtf(b * inv2) + 1e-8f);
@@ -310,11 +309,11 @@ __global__ void __launch_bounds__(256) slim_shard_apply_kernel(const ShardParams
     const int s = p.indptr[u], e = p.indptr[u + 1];
     const float gr = 1.f / (1.f + expf(x_sum[n]));  // pyx:258
     float gi = gr, gj = gr;
-    if (p.sgd_mode != SGD) {
+    if (p.sgd_mode != B200_SGD) {
       float inv1 = 1.f, inv2 = 1.f;
-      if (p.sgd_mode == ADAM) {  // the powers advance once per sample (pyx:309-312)
-        inv1 = (float)(1.0 / (1.0 - p.b1_pow * pow((double)p.beta1, (double)g)));
-        inv2 = (float)(1.0 / (1.0 - p.b2_pow * pow((double)p.beta2, (double)g)));
+      if (p.sgd_mode == B200_ADAM) {  // the powers advance once per sample (pyx:309-312)
+        inv1 = adam_correction(p.b1_pow * pow((double)p.beta1, (double)g));
+        inv2 = adam_correction(p.b2_pow * pow((double)p.beta2, (double)g));
       }
       // the per-item state is replicated and frozen while a batch is applied: every rank derives the same scales
       if (lane == 0) { gi = adapt_item_frozen(p, gr, i, inv1, inv2); gj = adapt_item_frozen(p, gr, j, inv1, inv2); }
@@ -344,9 +343,9 @@ __global__ void slim_shard_state_kernel(const ShardParams sp, const float* __res
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
     const int it = items[t];
-    if (p.sgd_mode == ADAGRAD) atomicAdd(p.c + it, gr * gr);
-    else if (p.sgd_mode == RMSPROP) ema_atomic(p.c + it, p.gamma, (1.f - p.gamma) * gr * gr);
-    else if (p.sgd_mode == ADAM) { ema_atomic(p.m1 + it, p.beta1, (1.f - p.beta1) * gr); ema_atomic(p.m2 + it, p.beta2, (1.f - p.beta2) * gr * gr); }
+    if (p.sgd_mode == B200_ADAGRAD) atomicAdd(p.c + it, gr * gr);
+    else if (p.sgd_mode == B200_RMSPROP) ema_atomic(p.c + it, p.gamma, (1.f - p.gamma) * gr * gr);
+    else if (p.sgd_mode == B200_ADAM) { ema_atomic(p.m1 + it, p.beta1, (1.f - p.beta1) * gr); ema_atomic(p.m2 + it, p.beta2, (1.f - p.beta2) * gr * gr); }
   }
 }
 
@@ -650,8 +649,7 @@ struct b200_slim_s {
   DevBuf<int> d_indptr, d_indices, su, si, sj;
   DevBuf<float> S, c, m1, m2;
   DevBuf<double> pow_out;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  bool timed = false;
+  EpochTimer timer;
   int shard_lo = 0, shard_hi = 0;  // column-sharded handle (b200_slim_create_sharded): S is [n_items, shard_hi - shard_lo]
   long long drawn_epoch = -1;      // the epoch whose sample stream is in su / si / sj
   TreeStore ts;                    // tree mode (b200_slim_enable_tree)
@@ -731,7 +729,7 @@ int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t
   int rc = guarded([&] {
     B200_REQUIRE(out && h_indptr && (nnz == 0 || h_indices), "b200_slim_create: NULL argument");
     B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_slim_create: bad shape");
-    B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_slim_create: unknown sgd_mode %d", sgd_mode);
+    B200_REQUIRE(sgd_mode >= B200_SGD && sgd_mode <= B200_ADAM, "b200_slim_create: unknown sgd_mode %d", sgd_mode);
     B200_REQUIRE(sampler == 0 || has_sampleable_user(h_indptr, 0, n_users, n_items),
                  "b200_slim_create: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
     h = new b200_slim_s();
@@ -751,9 +749,9 @@ int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t
     p.indptr = h->d_indptr.get(); p.indices = h->d_indices.get();
     // S starts at zero (pyx:122-125): a dense S is allocated by the first call that needs it (ensure_dense_S), so a handle
     // that becomes a tree handle (b200_slim_enable_tree) never holds one
-    if (sgd_mode == ADAGRAD || sgd_mode == RMSPROP) {
+    if (sgd_mode == B200_ADAGRAD || sgd_mode == B200_RMSPROP) {
       h->c.alloc((size_t)n_items); B200_CUDA(cudaMemset(h->c.get(), 0, sizeof(float) * (size_t)n_items)); p.c = h->c.get();
-    } else if (sgd_mode == ADAM) {
+    } else if (sgd_mode == B200_ADAM) {
       h->m1.alloc((size_t)n_items); h->m2.alloc((size_t)n_items);
       B200_CUDA(cudaMemset(h->m1.get(), 0, sizeof(float) * (size_t)n_items));
       B200_CUDA(cudaMemset(h->m2.get(), 0, sizeof(float) * (size_t)n_items));
@@ -763,8 +761,6 @@ int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t
     p.su = h->su.get(); p.si = h->si.get(); p.sj = h->sj.get();
     h->pow_out.alloc(2);
     p.pow_out = h->pow_out.get();
-    B200_CUDA(cudaEventCreate(&h->ev0));
-    B200_CUDA(cudaEventCreate(&h->ev1));
     *out = h;
   });
   if (rc != B200_OK && h) delete h;
@@ -779,7 +775,7 @@ int b200_slim_create_sharded(b200_slim_t* out, int64_t n_users, int64_t n_items,
   int rc = guarded([&] {
     B200_REQUIRE(out && h_indptr && (nnz == 0 || h_indices), "b200_slim_create_sharded: NULL argument");
     B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_slim_create_sharded: bad shape");
-    B200_REQUIRE(sgd_mode >= SGD && sgd_mode <= ADAM, "b200_slim_create_sharded: unknown sgd_mode %d", sgd_mode);
+    B200_REQUIRE(sgd_mode >= B200_SGD && sgd_mode <= B200_ADAM, "b200_slim_create_sharded: unknown sgd_mode %d", sgd_mode);
     B200_REQUIRE(0 <= col_lo && col_lo < col_hi && col_hi <= n_items, "b200_slim_create_sharded: bad column range [%d,%d)", col_lo, col_hi);
     B200_REQUIRE(has_sampleable_user(h_indptr, 0, n_users, n_items),
                  "b200_slim_create_sharded: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
@@ -800,9 +796,9 @@ int b200_slim_create_sharded(b200_slim_t* out, int64_t n_users, int64_t n_items,
     h->S.alloc(cells);
     B200_CUDA(cudaMemset(h->S.get(), 0, cells * sizeof(float)));
     p.S = h->S.get();
-    if (sgd_mode == ADAGRAD || sgd_mode == RMSPROP) {
+    if (sgd_mode == B200_ADAGRAD || sgd_mode == B200_RMSPROP) {
       h->c.alloc((size_t)n_items); B200_CUDA(cudaMemset(h->c.get(), 0, sizeof(float) * (size_t)n_items)); p.c = h->c.get();
-    } else if (sgd_mode == ADAM) {
+    } else if (sgd_mode == B200_ADAM) {
       h->m1.alloc((size_t)n_items); h->m2.alloc((size_t)n_items);
       B200_CUDA(cudaMemset(h->m1.get(), 0, sizeof(float) * (size_t)n_items));
       B200_CUDA(cudaMemset(h->m2.get(), 0, sizeof(float) * (size_t)n_items));
@@ -812,8 +808,6 @@ int b200_slim_create_sharded(b200_slim_t* out, int64_t n_users, int64_t n_items,
     p.su = h->su.get(); p.si = h->si.get(); p.sj = h->sj.get();
     h->pow_out.alloc(2);
     p.pow_out = h->pow_out.get();
-    B200_CUDA(cudaEventCreate(&h->ev0));
-    B200_CUDA(cudaEventCreate(&h->ev1));
     *out = h;
   });
   if (rc != B200_OK && h) delete h;
@@ -848,16 +842,13 @@ int b200_slim_shard_apply_device(b200_slim_t h, int64_t first, int n_batch, cons
     slim_shard_apply_kernel<<<std::min<int>(div_up(n_batch, 8), sm_count() * 8), 256, 0, (cudaStream_t)stream>>>(sp, d_x_sum);
     B200_CUDA(cudaGetLastError());
     count_launch();
-    if (h->p.sgd_mode != SGD) {
+    if (h->p.sgd_mode != B200_SGD) {
       slim_shard_state_kernel<<<div_up(n_batch, 256), 256, 0, (cudaStream_t)stream>>>(sp, d_x_sum);
       B200_CUDA(cudaGetLastError());
       count_launch();
     }
     if (first + n_batch == h->p.n_users) {  // the epoch is complete
-      if (h->p.sgd_mode == ADAM) {
-        h->p.b1_pow *= pow((double)h->p.beta1, (double)h->p.n_users);
-        h->p.b2_pow *= pow((double)h->p.beta2, (double)h->p.n_users);
-      }
+      if (h->p.sgd_mode == B200_ADAM) advance_powers(h->p.beta1, h->p.beta2, h->p.b1_pow, h->p.b2_pow, (double)h->p.n_users);
       h->epoch += 1;
     }
   });
@@ -874,8 +865,6 @@ int b200_slim_shard_device(b200_slim_t h, float** d_S, int* col_lo, int* col_hi)
 
 int b200_slim_destroy(b200_slim_t h) {
   if (!h) return B200_OK;
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
   delete h;
   return B200_OK;
 }
@@ -895,7 +884,7 @@ int b200_slim_epoch(b200_slim_t h, void* stream) {
       B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
       B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs.j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
     }
-    B200_CUDA(cudaEventRecord(h->ev0, st));
+    h->timer.begin(st);
     if (h->sampler != 0) {
       slim_sample_kernel<<<div_up(n, 256), 256, 0, st>>>(p.indptr, p.indices, p.n_users, p.n_items, n, h->seed, h->epoch,
                                                         h->su.get(), h->si.get(), h->sj.get());
@@ -904,7 +893,7 @@ int b200_slim_epoch(b200_slim_t h, void* stream) {
     if (!h->tree) ensure_dense_S(h, st);
     if (h->hogwild) {
       slim_hogwild_kernel<<<sm_count() * 8, 256, 0, st>>>(p);
-      if (p.sgd_mode == ADAM) { p.b1_pow *= pow((double)p.beta1, (double)n); p.b2_pow *= pow((double)p.beta2, (double)n); }
+      if (p.sgd_mode == B200_ADAM) advance_powers(p.beta1, p.beta2, p.b1_pow, p.b2_pow, (double)n);
     } else if (h->tree) {
       tree_epoch(h, st);
     } else {
@@ -912,13 +901,9 @@ int b200_slim_epoch(b200_slim_t h, void* stream) {
     }
     B200_CUDA(cudaGetLastError());
     count_launch();
-    B200_CUDA(cudaEventRecord(h->ev1, st));
-    h->timed = true;
-    if (!h->hogwild && p.sgd_mode == ADAM) {
-      double pw[2];
-      B200_CUDA(cudaMemcpyAsync(pw, h->pow_out.get(), sizeof(pw), cudaMemcpyDeviceToHost, st));
-      B200_CUDA(cudaStreamSynchronize(st));
-      p.b1_pow = pw[0]; p.b2_pow = pw[1];
+    h->timer.end(st);
+    if (!h->hogwild && p.sgd_mode == B200_ADAM) {
+      read_powers(h->pow_out.get(), p.b1_pow, p.b2_pow, st);
     } else if (h->sampler == 0) {
       B200_CUDA(cudaStreamSynchronize(st));
     }
@@ -1047,9 +1032,8 @@ int b200_slim_get_S_dense(b200_slim_t h, float* h_out, float* d_out) {
 
 int b200_slim_last_epoch_ms(b200_slim_t h, float* ms) {
   return guarded([&] {
-    B200_REQUIRE(h && ms && h->timed, "b200_slim_last_epoch_ms: no epoch run yet");
-    B200_CUDA(cudaEventSynchronize(h->ev1));
-    B200_CUDA(cudaEventElapsedTime(ms, h->ev0, h->ev1));
+    B200_REQUIRE(h && ms && h->timer.timed, "b200_slim_last_epoch_ms: no epoch run yet");
+    h->timer.elapsed(ms);
   });
 }
 
