@@ -50,6 +50,16 @@ struct AdaptState {
   float *s1, *s2;
 };
 
+// Owns the zeroed state arrays of one parameter table of n elements
+struct AdaptBuffers {
+  DevBuf<float> s1, s2;
+  AdaptState alloc(int mode, size_t n) {
+    if (mode != B200_SGD) s1.alloc_zeroed(n);
+    if (mode == B200_ADAM) s2.alloc_zeroed(n);
+    return {s1.get(), s2.get()};
+  }
+};
+
 // pyx:838-876 on element o of a table whose state is in memory: loads what the mode reads, stores it back.  An array is
 // indexed only in the modes that have it.
 template <class Access = PlainAccess>

@@ -251,45 +251,12 @@ using namespace b200::asy;
 
 struct b200_asysvd_s {
   Params p{};
-  double quota = 0.0;
-  GlibcRandHost rng;
-  std::vector<int> h_indptr, h_indices;
-  std::vector<float> h_data;
-  HostSamples hs;
-  DevBuf<int> d_indptr, d_indices, su, si;
-  DevBuf<float> sr, Y, X, bu, bi, mu, cY, cX, cbu, cbi, cmu, m2Y, m2X, m2bu, m2bi, m2mu;
+  SampleStream ss;
+  DevBuf<float> Y, X, bu, bi, mu;
+  AdaptBuffers sY, sX, sbu, sbi, smu;  // their optimiser state
   DevBuf<double> pow_out;
   EpochTimer timer;
-  long long n_last = 0;
 };
-
-namespace {
-// rows of f doubles -> rows of fp floats (zero padding)
-void upload_rows(DevBuf<float>& dst, const double* src, size_t rows, size_t f, size_t fp) {
-  std::vector<float> tmp(rows * fp, 0.f);
-  for (size_t r = 0; r < rows; ++r)
-    for (size_t k = 0; k < f; ++k) tmp[r * fp + k] = (float)src[r * f + k];
-  dst.alloc(rows * fp);
-  B200_CUDA(cudaMemcpy(dst.get(), tmp.data(), rows * fp * sizeof(float), cudaMemcpyHostToDevice));
-}
-void download_rows(double* dst, const float* src, size_t rows, size_t f, size_t fp) {
-  if (!dst) return;
-  std::vector<float> tmp(rows * fp);
-  B200_CUDA(cudaMemcpy(tmp.data(), src, rows * fp * sizeof(float), cudaMemcpyDeviceToHost));
-  for (size_t r = 0; r < rows; ++r)
-    for (size_t k = 0; k < f; ++k) dst[r * f + k] = (double)tmp[r * fp + k];
-}
-void zeros(DevBuf<float>& dst, size_t n) {
-  dst.alloc(n);
-  B200_CUDA(cudaMemset(dst.get(), 0, n * sizeof(float)));
-}
-void download_doubles(double* dst, const float* src, size_t n) {
-  if (!dst) return;
-  std::vector<float> tmp(n);
-  B200_CUDA(cudaMemcpy(tmp.data(), src, n * sizeof(float), cudaMemcpyDeviceToHost));
-  for (size_t k = 0; k < n; ++k) dst[k] = (double)tmp[k];
-}
-}  // namespace
 
 extern "C" {
 
@@ -315,31 +282,21 @@ int b200_asysvd_create(b200_asysvd_t* out, int64_t n_users, int64_t n_items, int
     p.lr = learning_rate; p.user_reg = user_reg; p.item_reg = item_reg; p.bias_reg = bias_reg;
     p.gamma = gamma; p.beta1 = beta_1; p.beta2 = beta_2;
     p.b1_pow = beta_1; p.b2_pow = beta_2;  // pyx:220-221
-    h->quota = negative_interactions_quota;
-    h->rng.seed(has_seed ? random_seed : 1u);
-    h->h_indptr.assign(h_indptr, h_indptr + n_users + 1);
-    h->h_indices.assign(h_indices, h_indices + nnz);
-    h->h_data.assign(h_data, h_data + nnz);
-    h->d_indptr.alloc((size_t)n_users + 1);
-    h->d_indices.alloc((size_t)nnz);
-    B200_CUDA(cudaMemcpy(h->d_indptr.get(), h_indptr, sizeof(int) * ((size_t)n_users + 1), cudaMemcpyHostToDevice));
-    B200_CUDA(cudaMemcpy(h->d_indices.get(), h_indices, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice));
-    p.indptr = h->d_indptr.get(); p.indices = h->d_indices.get();
-    upload_rows(h->Y, h_profile_factors, (size_t)n_items, f, fp); p.Y = h->Y.get();
-    upload_rows(h->X, h_item_factors, (size_t)n_items, f, fp); p.X = h->X.get();
-    zeros(h->bu, (size_t)n_users); zeros(h->bi, (size_t)n_items); zeros(h->mu, 1);  // pyx:184-186
-    p.bu = h->bu.get(); p.bi = h->bi.get(); p.mu = h->mu.get();
-    if (sgd_mode != B200_SGD) {  // pyx:248-270
-      zeros(h->cY, nf); zeros(h->cX, nf); zeros(h->cbu, (size_t)n_users); zeros(h->cbi, (size_t)n_items); zeros(h->cmu, 1);
-      p.cY = h->cY.get(); p.cX = h->cX.get(); p.cbu = h->cbu.get(); p.cbi = h->cbi.get(); p.cmu = h->cmu.get();
-    }
-    if (sgd_mode == B200_ADAM) {
-      zeros(h->m2Y, nf); zeros(h->m2X, nf); zeros(h->m2bu, (size_t)n_users); zeros(h->m2bi, (size_t)n_items); zeros(h->m2mu, 1);
-      p.m2Y = h->m2Y.get(); p.m2X = h->m2X.get(); p.m2bu = h->m2bu.get(); p.m2bi = h->m2bi.get(); p.m2mu = h->m2mu.get();
-    }
     const size_t n_epoch = (size_t)nnz + 1;  // pyx:402: int(len(data) / batch_size) + 1 with batch_size == 1
-    h->su.alloc(n_epoch); h->si.alloc(n_epoch); h->sr.alloc(n_epoch);
-    p.su = h->su.get(); p.si = h->si.get(); p.sr = h->sr.get();
+    h->ss.init(n_users, n_items, nnz, h_indptr, h_indices, h_data, false, negative_interactions_quota, n_epoch, false, 0,
+               has_seed ? random_seed : 1u, false);
+    p.indptr = h->ss.indptr.get(); p.indices = h->ss.indices.get();
+    p.su = h->ss.su.get(); p.si = h->ss.si.get(); p.sr = h->ss.sr.get();
+    upload_f32(h->Y, h_profile_factors, (size_t)n_items, f, fp); p.Y = h->Y.get();
+    upload_f32(h->X, h_item_factors, (size_t)n_items, f, fp); p.X = h->X.get();
+    h->bu.alloc_zeroed((size_t)n_users); h->bi.alloc_zeroed((size_t)n_items); h->mu.alloc_zeroed(1);  // pyx:184-186
+    p.bu = h->bu.get(); p.bi = h->bi.get(); p.mu = h->mu.get();
+    AdaptState a;  // pyx:248-270
+    a = h->sY.alloc(sgd_mode, nf); p.cY = a.s1; p.m2Y = a.s2;
+    a = h->sX.alloc(sgd_mode, nf); p.cX = a.s1; p.m2X = a.s2;
+    a = h->sbu.alloc(sgd_mode, (size_t)n_users); p.cbu = a.s1; p.m2bu = a.s2;
+    a = h->sbi.alloc(sgd_mode, (size_t)n_items); p.cbi = a.s1; p.m2bi = a.s2;
+    a = h->smu.alloc(sgd_mode, 1); p.cmu = a.s1; p.m2mu = a.s2;
     h->pow_out.alloc(2);
     p.pow_out = h->pow_out.get();
     *out = h;
@@ -359,13 +316,10 @@ int b200_asysvd_epoch(b200_asysvd_t h, void* stream) {
     B200_REQUIRE(h != nullptr, "b200_asysvd_epoch: NULL handle");
     cudaStream_t st = (cudaStream_t)stream;
     Params& p = h->p;
-    const long long n = (long long)h->h_indices.size() + 1;
+    const long long n = (long long)h->ss.h_indices.size() + 1;
     p.n_samples = n;
     p.prof = getenv("B200REC_ASY_PROF") != nullptr;
-    h->hs.draw(h->rng, h->h_indptr.data(), h->h_indices.data(), h->h_data.data(), p.n_users, p.n_items, false, h->quota, n);
-    B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs.u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs.r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
+    h->ss.draw_glibc(n, st);
     h->timer.begin(st);
     const size_t smem = (size_t)(WARPS + 2) * (size_t)p.fp * sizeof(float);
     // per launch: the attribute belongs to the function, and handles with other factor counts share it
@@ -374,19 +328,15 @@ int b200_asysvd_epoch(b200_asysvd_t h, void* stream) {
     B200_CUDA(cudaGetLastError());
     count_launch();
     h->timer.end(st);
-    // the host sample buffers are reused by the next epoch: both branches synchronise the stream
     if (p.sgd_mode == B200_ADAM) read_powers(h->pow_out.get(), p.b1_pow, p.b2_pow, st);
-    else B200_CUDA(cudaStreamSynchronize(st));
-    h->n_last = n;
+    else if (h->ss.host_vectors_in_flight()) B200_CUDA(cudaStreamSynchronize(st));
   });
 }
 
 int b200_asysvd_get_samples(b200_asysvd_t h, int32_t* u, int32_t* i, float* r) {
   return guarded([&] {
-    B200_REQUIRE(h && u && i && r && h->n_last > 0, "b200_asysvd_get_samples: NULL argument or no epoch run yet");
-    std::copy(h->hs.u.begin(), h->hs.u.end(), u);
-    std::copy(h->hs.i.begin(), h->hs.i.end(), i);
-    std::copy(h->hs.r.begin(), h->hs.r.end(), r);
+    B200_REQUIRE(h && u && i && r && h->ss.drawn > 0, "b200_asysvd_get_samples: NULL argument or no epoch run yet");
+    h->ss.copy_out(u, i, nullptr, r);
   });
 }
 
@@ -395,11 +345,11 @@ int b200_asysvd_get_factors(b200_asysvd_t h, double* profile_factors, double* it
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_asysvd_get_factors: NULL handle");
     B200_CUDA(cudaDeviceSynchronize());
-    download_rows(profile_factors, h->Y.get(), (size_t)h->p.n_items, (size_t)h->p.f, (size_t)h->p.fp);
-    download_rows(item_factors, h->X.get(), (size_t)h->p.n_items, (size_t)h->p.f, (size_t)h->p.fp);
-    download_doubles(user_bias, h->bu.get(), (size_t)h->p.n_users);
-    download_doubles(item_bias, h->bi.get(), (size_t)h->p.n_items);
-    download_doubles(global_bias, h->mu.get(), 1);
+    download_f64(profile_factors, h->Y.get(), (size_t)h->p.n_items, (size_t)h->p.f, (size_t)h->p.fp);
+    download_f64(item_factors, h->X.get(), (size_t)h->p.n_items, (size_t)h->p.f, (size_t)h->p.fp);
+    download_f64(user_bias, h->bu.get(), (size_t)h->p.n_users, 1, 1);
+    download_f64(item_bias, h->bi.get(), (size_t)h->p.n_items, 1, 1);
+    download_f64(global_bias, h->mu.get(), 1, 1, 1);
   });
 }
 

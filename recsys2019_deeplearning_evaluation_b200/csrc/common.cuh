@@ -6,6 +6,7 @@
 #include <stdarg.h>
 #include <atomic>
 #include <new>
+#include <vector>
 
 #include "b200rec.h"
 
@@ -74,6 +75,10 @@ struct DevBuf {
     n = count;
     if (count) B200_CUDA(cudaMalloc(reinterpret_cast<void**>(&p), count * sizeof(T)));
   }
+  void alloc_zeroed(size_t count) {
+    alloc(count);
+    if (count) B200_CUDA(cudaMemset(p, 0, count * sizeof(T)));
+  }
   void release() {
     if (p) cudaFree(p);
     p = nullptr;
@@ -81,6 +86,24 @@ struct DevBuf {
   }
   T* get() const { return p; }
 };
+
+// Host fp64 rows of f values -> device fp32 rows of ld >= f values; columns f..ld are zero
+inline void upload_f32(DevBuf<float>& dst, const double* src, size_t rows, size_t f, size_t ld) {
+  std::vector<float> tmp(rows * ld, 0.f);
+  for (size_t r = 0; r < rows; ++r)
+    for (size_t k = 0; k < f; ++k) tmp[r * ld + k] = (float)src[r * f + k];
+  dst.alloc(rows * ld);
+  B200_CUDA(cudaMemcpy(dst.get(), tmp.data(), rows * ld * sizeof(float), cudaMemcpyHostToDevice));
+}
+
+// Device fp32 rows of ld values -> host fp64 rows of their first f values; nothing when either side is null
+inline void download_f64(double* dst, const float* src, size_t rows, size_t f, size_t ld) {
+  if (!dst || !src) return;
+  std::vector<float> tmp(rows * ld);
+  B200_CUDA(cudaMemcpy(tmp.data(), src, rows * ld * sizeof(float), cudaMemcpyDeviceToHost));
+  for (size_t r = 0; r < rows; ++r)
+    for (size_t k = 0; k < f; ++k) dst[r * f + k] = (double)tmp[r * ld + k];
+}
 
 // Device time of a handle's last call (an epoch, a kernel): events recorded around the work on the caller's stream
 struct EpochTimer {

@@ -26,8 +26,6 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <stdlib.h>
 
-#include <string.h>
-
 #include <algorithm>
 #include <vector>
 
@@ -520,74 +518,6 @@ __global__ void mf_deps_kernel(const unsigned long long* __restrict__ keys, cons
   }
 }
 
-// Philox stream of the user shard [user_lo, user_lo + n_users) (sampler.cuh)
-__global__ void mf_sample_kernel(const int* __restrict__ indptr, const int* __restrict__ indices, const float* __restrict__ data,
-                                 int user_lo, int n_users, int n_items, int algorithm, float quota, long long n_samples, unsigned seed,
-                                 unsigned epoch, int* su, int* si, int* sj, float* sr) {
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= n_samples) return;
-  PhiloxDraws d{(unsigned long long)g, seed, epoch, 0x9E3779B9u};
-  Sample s;
-  draw_sample(d, indptr, indices, data, user_lo, n_users, n_items, algorithm == MF_BPR, quota, s);
-  su[g] = s.u;
-  si[g] = s.i;
-  if (algorithm == MF_BPR) sj[g] = s.j; else sr[g] = s.r;
-}
-
-
-// =====================================================================================================================
-// glibc stream on the device.  The reference draws its samples with libc rand() (sampleBPR_Cython pyx:943-987,
-// sampleMSE_Cython :881-938): a sequential recurrence feeding rejection loops, so sample g's first draw depends on how many
-// draws every earlier sample consumed.  The raw stream itself is cheap to produce in order (1 ns per draw on the host);
-// what made the host replay slow (160 ms per C5 epoch) are the dependent memory lookups of the acceptance rules.  Here:
-//   1. the host appends raw draws to a pinned buffer and uploads them;
-//   2. glibc_len_kernel: for EVERY position p of the buffer, how many draws a sample STARTING at p would consume;
-//   3. pointer doubling: J_0[p] = p + len[p], J_{k+1} = J_k o J_k, so that any number of samples can be skipped at once;
-//   4. glibc_emit_kernel: sample g starts where the binary expansion of g leads from position 0; it is re-evaluated there
-//      and written out.  The number of draws the epoch consumed tells the host where the next epoch's stream begins.
-// Bit-identical to the host replay (same draws, same rules); tests compare the two.
-struct GlibcView {
-  const int* __restrict__ raw; int R;  // draws raw[0 .. R)
-  const int* __restrict__ indptr; const int* __restrict__ indices; const float* __restrict__ data;
-  int n_users, n_items, algorithm; float quota;
-};
-
-// the sample starting at raw position p: returns the position after its last draw (> R when the buffer ran out)
-__device__ __forceinline__ int glibc_sample_at(const GlibcView& v, int p, Sample* out) {
-  GlibcReplay d{v.raw, p, v.R};
-  Sample s{};
-  if (!draw_sample(d, v.indptr, v.indices, v.data, 0, v.n_users, v.n_items, v.algorithm == MF_BPR, v.quota, s)) return v.R + 1;
-  if (out) *out = s;
-  return d.q;
-}
-
-__global__ void glibc_len_kernel(const GlibcView v, int* __restrict__ nxt) {  // nxt[p] = start of the following sample; nxt[R] = R
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p > v.R) return;
-  nxt[p] = p == v.R ? v.R : min(glibc_sample_at(v, p, nullptr), v.R);
-}
-
-__global__ void glibc_double_kernel(const int* __restrict__ jk, int R, int* __restrict__ jk1) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p <= R) jk1[p] = jk[jk[p]];
-}
-
-// sample g: follow the binary expansion of g through the jump tables (tables[k] = J_k, (R + 1) ints each), evaluate, store
-__global__ void glibc_emit_kernel(const GlibcView v, const int* __restrict__ tables, int levels, long long n_samples, int* su, int* si,
-                                  int* sj, float* sr, int* consumed) {
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= n_samples) return;
-  int p = 0;
-  for (int k = 0; k < levels; ++k)
-    if ((g >> k) & 1) p = tables[(size_t)k * (v.R + 1) + p];
-  Sample s{};
-  const int q = p < v.R ? glibc_sample_at(v, p, &s) : v.R + 1;
-  su[g] = s.u; si[g] = s.i;
-  if (v.algorithm == MF_BPR) sj[g] = s.j; else sr[g] = s.r;
-  if (q > v.R) atomicMax(consumed, 0x7FFFFFFF);  // the buffer ran out somewhere: the host extends it and repeats
-  else if (g == n_samples - 1) atomicMax(consumed, q);
-}
-
 }  // namespace mf
 }  // namespace b200
 
@@ -596,18 +526,13 @@ using namespace b200::mf;
 
 struct b200_mf_s {
   Params p{};
-  int sampler = 0;  // 0 glibc replay on the host, 1 Philox on the device
+  SampleStream ss;
   unsigned seed = 1;       // the Philox key of the draws
   unsigned base_seed = 1;  // random_seed as created: b200_mf_set_user_shard derives `seed` from it
   unsigned epoch = 0;
   long long nnz = 0;
-  float quota = 0.5f;
-  GlibcRandHost rng;
-  std::vector<int> h_indptr, h_indices;
-  std::vector<float> h_data;
-  DevBuf<int> d_indptr, d_indices;
-  DevBuf<float> d_data;
-  std::vector<DevBuf<float>> fbufs;  // owns every float device array referenced by p
+  DevBuf<float> U, V, bu, bi, mu;
+  AdaptBuffers sU, sV, sbu, sbi, smu;  // their optimiser state
   std::vector<DevBuf<double>> dbufs;  // the fp64 gradient accumulators of the mini-batch mode
   double* dalloc(size_t n) {
     dbufs.emplace_back(std::max<size_t>(n, 1));
@@ -615,20 +540,11 @@ struct b200_mf_s {
     B200_CUDA(cudaMemset(d, 0, std::max<size_t>(n, 1) * sizeof(double)));
     return d;
   }
-  DevBuf<int> flagI, flagU, listI, listU, cnt, su, si, sj;
-  DevBuf<float> sr;
+  DevBuf<int> flagI, flagU, listI, listU, cnt;
   DevBuf<double> pow_out;
-  HostSamples hs;  // the host replay's samples (B200REC_GLIBC_HOST=1, or a stream too long for the device replay)
-  long long samples_last = 0, cap_samples = 0, epoch_samples_override = 0;
+  long long cap_samples = 0, epoch_samples_override = 0;
   int shard_lo = 0, shard_hi = 0;  // device sampler draws users from [shard_lo, shard_hi) when set (multi-GPU user sharding)
   int grid = 0;
-  // device-side replay of the glibc stream (glibc_*_kernel): pinned raw draws with the unread tail of the previous epoch in
-  // front, their device copy, the jump tables, the consumed-draw counter
-  bool glibc_device = true;
-  int* h_raw = nullptr;            // pinned
-  long long raw_cap = 0, raw_have = 0;  // capacity / draws currently in h_raw (all unread)
-  DevBuf<int> d_raw, d_tables, d_consumed;
-  long long tables_cap = 0;
   int hog_blocks = 8;  // hogwild CTAs per SM; a sharded (multi-GPU) run leaves room for the collective's CTAs
   // dataflow mode (mf_dataflow_kernel): dependency tables rebuilt from every epoch's sample stream
   bool dataflow = false;
@@ -640,18 +556,6 @@ struct b200_mf_s {
   DevBuf<float> inv1_b, inv2_b;
   std::vector<float> h_inv1, h_inv2;
   EpochTimer timer;
-  float* falloc(size_t n, const double* init) {
-    fbufs.emplace_back(std::max<size_t>(n, 1));
-    float* d = fbufs.back().get();
-    if (init) {
-      std::vector<float> tmp(n);
-      for (size_t i = 0; i < n; ++i) tmp[i] = (float)init[i];
-      B200_CUDA(cudaMemcpy(d, tmp.data(), n * sizeof(float), cudaMemcpyHostToDevice));
-    } else {
-      B200_CUDA(cudaMemset(d, 0, std::max<size_t>(n, 1) * sizeof(float)));
-    }
-    return d;
-  }
 };
 
 namespace {
@@ -665,56 +569,6 @@ const void* dataflow_kernel_for(bool bpr, int f) {
 long long epoch_batches(const b200_mf_s* h) {
   // pyx:586 (BPR: n_users / batch_size + 1) and pyx:292 (FunkSVD: nnz / batch_size + 1)
   return (h->p.algorithm == MF_BPR ? (long long)h->p.n_users : h->nnz) / h->p.batch_size + 1;
-}
-
-// The epoch's n samples from the glibc stream, resolved on the device (see glibc_len_kernel).  Synchronises the stream once
-// (the host must know how many draws were consumed before it can continue the stream).
-void glibc_device_samples(b200_mf_s* h, long long n, cudaStream_t st) {
-  const Params& p = h->p;
-  const int per = 3;  // draws of a sample without rejections (user, positive | quota, negative | item)
-  int levels = 1;
-  while ((1ll << levels) < n) ++levels;
-  long long want = n * per + n / 16 + 4096;
-  for (int attempt = 0;; ++attempt) {
-    B200_REQUIRE(attempt < 8 && want < (1ll << 30), "b200_mf_epoch: the glibc replay buffer does not converge (degenerate URM?)");
-    if (want > h->raw_cap) {
-      int* fresh = nullptr;
-      B200_CUDA(cudaMallocHost(reinterpret_cast<void**>(&fresh), sizeof(int) * (size_t)want));
-      if (h->raw_have) memcpy(fresh, h->h_raw, sizeof(int) * (size_t)h->raw_have);
-      if (h->h_raw) cudaFreeHost(h->h_raw);
-      h->h_raw = fresh;
-      h->raw_cap = want;
-      h->d_raw.alloc((size_t)want);
-    }
-    for (long long q = h->raw_have; q < want; ++q) h->h_raw[q] = h->rng.next();
-    h->raw_have = want;
-    const int R = (int)want;
-    if ((long long)levels * (R + 1) > h->tables_cap) {
-      h->tables_cap = (long long)levels * (R + 1);
-      h->d_tables.alloc((size_t)h->tables_cap);
-    }
-    if (h->d_consumed.n == 0) h->d_consumed.alloc(1);
-    B200_CUDA(cudaMemcpyAsync(h->d_raw.get(), h->h_raw, sizeof(int) * (size_t)R, cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemsetAsync(h->d_consumed.get(), 0, sizeof(int), st));
-    GlibcView v{h->d_raw.get(), R, h->d_indptr.get(), h->d_indices.get(), h->d_data.get(), p.n_users, p.n_items, p.algorithm, h->quota};
-    int* T = h->d_tables.get();
-    glibc_len_kernel<<<div_up(R + 1, 256), 256, 0, st>>>(v, T);
-    for (int k = 0; k + 1 < levels; ++k)
-      glibc_double_kernel<<<div_up(R + 1, 256), 256, 0, st>>>(T + (size_t)k * (R + 1), R, T + (size_t)(k + 1) * (R + 1));
-    glibc_emit_kernel<<<div_up(n, 256), 256, 0, st>>>(v, T, levels, n, h->su.get(), h->si.get(), h->sj.get(), h->sr.get(), h->d_consumed.get());
-    B200_CUDA(cudaGetLastError());
-    count_launch(levels + 1);
-    int consumed = 0;
-    B200_CUDA(cudaMemcpyAsync(&consumed, h->d_consumed.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    if (consumed != 0x7FFFFFFF && consumed <= R) {
-      // the unread tail opens the next epoch's stream
-      h->raw_have = R - consumed;
-      if (h->raw_have) memmove(h->h_raw, h->h_raw + consumed, sizeof(int) * (size_t)h->raw_have);
-      return;
-    }
-    want = want + want / 2;  // many rejections (dense profiles): a longer buffer, same draws in front
-  }
 }
 
 }  // namespace
@@ -746,38 +600,23 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
     p.ad = {sgd_mode, gamma, beta_1, beta_2, 1.f, 1.f};
     p.b1_pow = beta_1; p.b2_pow = beta_2;  // pyx:220-221
     h->nnz = nnz;
-    h->quota = negative_interactions_quota;
-    h->sampler = sampler;
     h->seed = h->base_seed = has_seed ? random_seed : 1u;
-    h->rng.seed(h->seed);
-    if (const char* e = getenv("B200REC_GLIBC_HOST")) h->glibc_device = atoi(e) == 0;  // 1: the sequential host replay (A/B, tests)
-    h->h_indptr.assign(h_indptr, h_indptr + n_users + 1);
-    h->h_indices.assign(h_indices, h_indices + nnz);
-    if (algorithm == FUNK_SVD) h->h_data.assign(h_data, h_data + nnz);
-    h->d_indptr.alloc((size_t)n_users + 1);
-    h->d_indices.alloc((size_t)std::max<int64_t>(nnz, 1));
-    h->d_data.alloc((size_t)std::max<int64_t>(nnz, 1));
-    B200_CUDA(cudaMemcpy(h->d_indptr.get(), h_indptr, sizeof(int) * ((size_t)n_users + 1), cudaMemcpyHostToDevice));
-    if (nnz) {
-      B200_CUDA(cudaMemcpy(h->d_indices.get(), h_indices, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice));
-      B200_CUDA(cudaMemcpy(h->d_data.get(), h_data, sizeof(float) * (size_t)nnz, cudaMemcpyHostToDevice));
-    }
-    const size_t nUf = (size_t)n_users * n_factors, nIf = (size_t)n_items * n_factors;
-    h->fbufs.reserve(40);
-    p.U = h->falloc(nUf, h_user_factors);
-    p.V = h->falloc(nIf, h_item_factors);
+    h->cap_samples = epoch_batches(h) * batch_size;
+    h->ss.init(n_users, n_items, nnz, h_indptr, h_indices, h_data, algorithm == MF_BPR, negative_interactions_quota,
+               (size_t)h->cap_samples, sampler != 0, 0x9E3779B9u, h->seed, true);
+    p.su = h->ss.su.get(); p.si = h->ss.si.get(); p.sj = h->ss.sj.get(); p.sr = h->ss.sr.get();
+    const size_t f = (size_t)n_factors, nUf = (size_t)n_users * f, nIf = (size_t)n_items * f;
+    upload_f32(h->U, h_user_factors, (size_t)n_users, f, f); p.U = h->U.get();
+    upload_f32(h->V, h_item_factors, (size_t)n_items, f, f); p.V = h->V.get();
     h->dbufs.reserve(8);
     if (!p.hogwild) { p.accU = h->dalloc(nUf); p.accV = h->dalloc(nIf); }
+    p.sU = h->sU.alloc(sgd_mode, nUf); p.sV = h->sV.alloc(sgd_mode, nIf);
     if (p.use_bias) {
-      p.bu = h->falloc((size_t)n_users, nullptr); p.bi = h->falloc((size_t)n_items, nullptr); p.mu = h->falloc(1, nullptr);
+      h->bu.alloc_zeroed((size_t)n_users); h->bi.alloc_zeroed((size_t)n_items); h->mu.alloc_zeroed(1);
+      p.bu = h->bu.get(); p.bi = h->bi.get(); p.mu = h->mu.get();
       p.accbu = h->dalloc((size_t)n_users); p.accbi = h->dalloc((size_t)n_items); p.accmu = h->dalloc(1);
+      p.sbu = h->sbu.alloc(sgd_mode, (size_t)n_users); p.sbi = h->sbi.alloc(sgd_mode, (size_t)n_items); p.smu = h->smu.alloc(sgd_mode, 1);
     }
-    // adaptive state: s1 in every adaptive mode, s2 in Adam only
-    auto state = [&](size_t n) {
-      return AdaptState{sgd_mode != B200_SGD ? h->falloc(n, nullptr) : nullptr, sgd_mode == B200_ADAM ? h->falloc(n, nullptr) : nullptr};
-    };
-    p.sU = state(nUf); p.sV = state(nIf);
-    if (p.use_bias) { p.sbu = state((size_t)n_users); p.sbi = state((size_t)n_items); p.smu = state(1); }
     h->flagI.alloc((size_t)n_items); h->flagU.alloc((size_t)n_users);
     h->listI.alloc((size_t)2 * batch_size); h->listU.alloc((size_t)batch_size); h->cnt.alloc(4);
     B200_CUDA(cudaMemset(h->flagI.get(), 0, sizeof(int) * (size_t)n_items));
@@ -786,10 +625,6 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
     p.flagI = h->flagI.get(); p.flagU = h->flagU.get(); p.listI = h->listI.get(); p.listU = h->listU.get(); p.cnt = h->cnt.get();
     h->pow_out.alloc(2);
     p.pow_out = h->pow_out.get();
-    h->cap_samples = epoch_batches(h) * batch_size;
-    h->su.alloc((size_t)h->cap_samples); h->si.alloc((size_t)h->cap_samples);
-    if (algorithm == MF_BPR) h->sj.alloc((size_t)h->cap_samples); else h->sr.alloc((size_t)h->cap_samples);
-    p.su = h->su.get(); p.si = h->si.get(); p.sj = h->sj.get(); p.sr = h->sr.get();
     // cooperative grid: every block resident
     int per_sm = 0;
     const bool vec4 = (n_factors % 4) == 0;
@@ -836,7 +671,6 @@ int b200_mf_create(b200_mf_t* out, int64_t n_users, int64_t n_items, int64_t nnz
 
 int b200_mf_destroy(b200_mf_t h) {
   if (!h) return B200_OK;
-  if (h->h_raw) cudaFreeHost(h->h_raw);
   delete h;
   return B200_OK;
 }
@@ -849,23 +683,9 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
     p.n_batches = epoch_batches(h);
     if (h->epoch_samples_override > 0) p.n_batches = std::max<long long>(1, h->epoch_samples_override / p.batch_size);
     const long long n = p.n_batches * p.batch_size;
-    if (h->sampler == 0 && h->glibc_device && n * 4 + 65536 < (1ll << 30)) {
-      glibc_device_samples(h, n, st);
-    } else if (h->sampler == 0) {
-      h->hs.draw(h->rng, h->h_indptr.data(), h->h_indices.data(), h->h_data.data(), p.n_users, p.n_items, p.algorithm == MF_BPR, h->quota, n);
-      B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs.u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      if (p.algorithm == MF_BPR) B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs.j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      else B200_CUDA(cudaMemcpyAsync(h->sr.get(), h->hs.r.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, st));
-    }
+    h->ss.draw_glibc(n, st);
     h->timer.begin(st);
-    if (h->sampler != 0) {
-      mf_sample_kernel<<<div_up(n, 256), 256, 0, st>>>(h->d_indptr.get(), h->d_indices.get(), h->d_data.get(), h->shard_lo,
-                                                      (h->shard_hi > h->shard_lo ? h->shard_hi - h->shard_lo : p.n_users), p.n_items,
-                                                      p.algorithm, h->quota, n, h->seed, h->epoch, h->su.get(), h->si.get(),
-                                                      h->sj.get(), h->sr.get());
-      count_launch();
-    }
+    h->ss.draw_philox(n, h->seed, h->epoch, h->shard_lo, h->shard_hi > h->shard_lo ? h->shard_hi - h->shard_lo : p.n_users, st);
     if (p.hogwild) {
       mf_hogwild_kernel<<<sm_count() * h->hog_blocks, 256, 0, st>>>(p, n);
       B200_CUDA(cudaGetLastError());
@@ -913,10 +733,9 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
       B200_CUDA(cudaStreamSynchronize(st));  // the host-side inv tables are reused by the next epoch
     } else if (!p.hogwild && p.ad.mode == B200_ADAM) {
       read_powers(h->pow_out.get(), p.b1_pow, p.b2_pow, st);
-    } else if (h->sampler == 0 && !(h->glibc_device && n * 4 + 65536 < (1ll << 30))) {
-      B200_CUDA(cudaStreamSynchronize(st));  // the host sample vectors are reused by the next epoch
+    } else if (h->ss.host_vectors_in_flight()) {
+      B200_CUDA(cudaStreamSynchronize(st));
     }
-    h->samples_last = n;
     h->epoch += 1;
   });
 }
@@ -924,10 +743,10 @@ int b200_mf_epoch(b200_mf_t h, void* stream) {
 int b200_mf_set_user_shard(b200_mf_t h, int user_lo, int user_hi, int64_t samples_per_epoch, uint32_t stream_id) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_mf_set_user_shard: NULL handle");
-    B200_REQUIRE(h->sampler != 0, "b200_mf_set_user_shard: only the device (Philox) sampler can be sharded");
+    B200_REQUIRE(h->ss.philox, "b200_mf_set_user_shard: only the device (Philox) sampler can be sharded");
     B200_REQUIRE(0 <= user_lo && user_lo < user_hi && user_hi <= h->p.n_users, "b200_mf_set_user_shard: bad range [%d,%d)", user_lo, user_hi);
     B200_REQUIRE(samples_per_epoch >= 0 && samples_per_epoch <= h->cap_samples, "b200_mf_set_user_shard: samples_per_epoch out of range");
-    B200_REQUIRE(has_sampleable_user(h->h_indptr.data(), user_lo, user_hi, h->p.n_items),
+    B200_REQUIRE(has_sampleable_user(h->ss.h_indptr.data(), user_lo, user_hi, h->p.n_items),
                  "b200_mf_set_user_shard: no user of [%d,%d) has 0 < profile length < n_items", user_lo, user_hi);
     h->shard_lo = user_lo;
     h->shard_hi = user_hi;
@@ -940,19 +759,14 @@ int b200_mf_set_user_shard(b200_mf_t h, int user_lo, int user_hi, int64_t sample
 int b200_mf_samples_last_epoch(b200_mf_t h, int64_t* n) {
   return guarded([&] {
     B200_REQUIRE(h && n, "b200_mf_samples_last_epoch: NULL argument");
-    *n = h->samples_last;
+    *n = h->ss.drawn;
   });
 }
 
 int b200_mf_get_samples(b200_mf_t h, int32_t* u, int32_t* i, int32_t* j, float* r) {
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_mf_get_samples: NULL handle");
-    B200_CUDA(cudaDeviceSynchronize());
-    const size_t n = (size_t)h->samples_last;
-    if (u) B200_CUDA(cudaMemcpy(u, h->su.get(), sizeof(int) * n, cudaMemcpyDeviceToHost));
-    if (i) B200_CUDA(cudaMemcpy(i, h->si.get(), sizeof(int) * n, cudaMemcpyDeviceToHost));
-    if (j && h->p.algorithm == MF_BPR) B200_CUDA(cudaMemcpy(j, h->sj.get(), sizeof(int) * n, cudaMemcpyDeviceToHost));
-    if (r && h->p.algorithm == FUNK_SVD) B200_CUDA(cudaMemcpy(r, h->sr.get(), sizeof(float) * n, cudaMemcpyDeviceToHost));
+    h->ss.copy_out(u, i, j, r);
   });
 }
 
@@ -961,17 +775,12 @@ int b200_mf_get_factors(b200_mf_t h, double* user_factors, double* item_factors,
   return guarded([&] {
     B200_REQUIRE(h != nullptr, "b200_mf_get_factors: NULL handle");
     B200_CUDA(cudaDeviceSynchronize());
-    auto fetch = [&](const float* d, double* out, size_t n) {
-      if (!out || !d) return;
-      std::vector<float> tmp(n);
-      B200_CUDA(cudaMemcpy(tmp.data(), d, n * sizeof(float), cudaMemcpyDeviceToHost));
-      for (size_t k = 0; k < n; ++k) out[k] = (double)tmp[k];
-    };
-    fetch(h->p.U, user_factors, (size_t)h->p.n_users * h->p.f);
-    fetch(h->p.V, item_factors, (size_t)h->p.n_items * h->p.f);
-    fetch(h->p.bu, user_bias, (size_t)h->p.n_users);
-    fetch(h->p.bi, item_bias, (size_t)h->p.n_items);
-    fetch(h->p.mu, global_bias, 1);
+    const size_t f = (size_t)h->p.f;
+    download_f64(user_factors, h->p.U, (size_t)h->p.n_users, f, f);
+    download_f64(item_factors, h->p.V, (size_t)h->p.n_items, f, f);
+    download_f64(user_bias, h->p.bu, (size_t)h->p.n_users, 1, 1);
+    download_f64(item_bias, h->p.bi, (size_t)h->p.n_items, 1, 1);
+    download_f64(global_bias, h->p.mu, 1, 1, 1);
   });
 }
 

@@ -3,8 +3,8 @@
 //   MatrixFactorization_Cython_Epoch.pyx: sampleMSE_Cython :881-938, sampleBPR_Cython :943-987
 //   SLIM_BPR_Cython_Epoch.pyx: sampleBPR_Cython :436-480
 // Streams: glibc's rand() replayed on the host (GlibcRandHost) or resolved on the device from uploaded draws (GlibcReplay),
-// both draw for draw the reference's; Philox4x32-10 on the device (PhiloxDraws).  tests/test_sample_streams_gpu.py pins
-// every stream value for value.
+// both draw for draw the reference's; Philox4x32-10 on the device (PhiloxDraws).  SampleStream turns them into an epoch's
+// device samples.  tests/test_sample_streams_gpu.py pins every stream value for value.
 #pragma once
 #include <vector>
 
@@ -156,6 +156,49 @@ struct PhiloxDraws {
     return v;
   }
   __device__ static bool uniform_le(unsigned x, double quota) { return (float)(x >> 8) * (1.f / 16777216.f) <= (float)quota; }
+};
+
+// ---- One trainer's sample stream (sample_stream.cu): the URM it draws from, the epoch's sample buffers and the source that
+// fills them.  A glibc stream is drawn before the epoch's timed window (draw_glibc): replayed on the host and uploaded, or
+// resolved on the device from uploaded raw draws (glibc_len_kernel).  A Philox stream is drawn inside it (draw_philox).
+struct SampleStream {
+  bool bpr = true, philox = false;
+  double quota = 0.0;                    // MSE: the probability of a positive
+  unsigned c3 = 0;                       // Philox: the fourth counter word (PhiloxDraws)
+  std::vector<int> h_indptr, h_indices;  // host copy: the host replay and has_sampleable_user read it
+  std::vector<float> h_data;             // MSE only
+  DevBuf<int> indptr, indices;
+  DevBuf<float> data;                    // MSE streams that can draw on the device only
+  DevBuf<int> su, si, sj;                // the drawn samples: (u, i, j) for BPR, (u, i, r) for MSE
+  DevBuf<float> sr;
+  long long drawn = 0;                   // samples of the last draw
+
+  SampleStream() = default;
+  SampleStream(const SampleStream&) = delete;
+  SampleStream& operator=(const SampleStream&) = delete;
+  ~SampleStream();
+  // capacity: the most samples one draw makes.  glibc_device: resolve the glibc stream on the device while it fits 32-bit
+  // positions (B200REC_GLIBC_HOST=1 forces the host replay: A/B runs, tests).
+  void init(int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* indptr, const int32_t* indices, const float* data,
+            bool bpr, double quota, size_t capacity, bool philox, unsigned c3, unsigned glibc_seed, bool glibc_device);
+  void draw_glibc(long long n, cudaStream_t st);  // nothing on a Philox stream
+  // users from [user_lo, user_lo + n_users), Philox key (seed, epoch); nothing on a glibc stream
+  void draw_philox(long long n, unsigned seed, unsigned epoch, int user_lo, int n_users, cudaStream_t st);
+  // the last draw was the host replay, whose vectors may still be uploading: the epoch synchronises before the next draw
+  bool host_vectors_in_flight() const { return host_drawn; }
+  void copy_out(int* u, int* i, int* j, float* r) const;  // the last draw (null: skipped); synchronises the device
+
+ private:
+  int n_users_ = 0, n_items_ = 0;
+  bool glibc_device = false, host_drawn = false;
+  GlibcRandHost rng;
+  HostSamples hs;
+  // the device replay: pinned raw draws with the unread tail of the previous epoch in front, their device copy, the jump
+  // tables, the consumed-draw counter
+  int* h_raw = nullptr;
+  long long raw_cap = 0, raw_have = 0, tables_cap = 0;
+  DevBuf<int> d_raw, d_tables, d_consumed;
+  void glibc_device_samples(long long n, cudaStream_t st);
 };
 
 }  // namespace b200

@@ -546,17 +546,6 @@ __global__ void slim_full_kernel(const float* __restrict__ S, int n, int symmetr
   out[g] = v;
 }
 
-// Philox stream of the epoch (sampler.cuh)
-__global__ void slim_sample_kernel(const int* __restrict__ indptr, const int* __restrict__ indices, int n_users, int n_items,
-                                   long long n_samples, unsigned seed, unsigned epoch, int* su, int* si, int* sj) {
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= n_samples) return;
-  PhiloxDraws d{(unsigned long long)g, seed, epoch, 0x243F6A88u};
-  Sample s;
-  draw_sample(d, indptr, indices, nullptr, 0, n_users, n_items, true, 0.0, s);
-  su[g] = s.u; si[g] = s.i; sj[g] = s.j;
-}
-
 // grows a scratch buffer to at least `count` elements (contents are not kept)
 template <typename T>
 void reserve(DevBuf<T>& b, size_t count) {
@@ -641,13 +630,11 @@ using namespace b200::slim;
 
 struct b200_slim_s {
   Params p{};
-  int sampler = 0, hogwild = 0;
+  SampleStream ss;
+  int hogwild = 0;
   unsigned seed = 1, epoch = 0;
-  GlibcRandHost rng;
-  std::vector<int> h_indptr, h_indices;
-  HostSamples hs;
-  DevBuf<int> d_indptr, d_indices, su, si, sj;
-  DevBuf<float> S, c, m1, m2;
+  DevBuf<float> S;
+  AdaptBuffers state;  // per item
   DevBuf<double> pow_out;
   EpochTimer timer;
   int shard_lo = 0, shard_hi = 0;  // column-sharded handle (b200_slim_create_sharded): S is [n_items, shard_hi - shard_lo]
@@ -719,46 +706,39 @@ static void tree_epoch(b200_slim_s* h, cudaStream_t st) {
   count_launch(launches - 1);  // the last one is counted by the caller
 }
 
-extern "C" {
-
-int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* h_indptr,
-                     const int32_t* h_indices, float learning_rate, float li_reg, float lj_reg, int symmetric, int sgd_mode,
-                     float gamma, float beta_1, float beta_2, int has_seed, uint32_t random_seed, int sampler, int hogwild) {
+// The body of b200_slim_create and b200_slim_create_sharded: every check before any CUDA call, then the handle.  A sharded
+// handle holds the columns [col_lo, col_hi) of S from the start; a single-GPU one allocates S when a call first needs it
+// (ensure_dense_S), so a handle that becomes a tree handle (b200_slim_enable_tree) never holds one.
+static int create(const char* fn, b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* h_indptr,
+                  const int32_t* h_indices, float learning_rate, float li_reg, float lj_reg, int symmetric, int sgd_mode, float gamma,
+                  float beta_1, float beta_2, uint32_t seed, int sampler, int hogwild, bool sharded, int col_lo, int col_hi) {
   if (out) *out = nullptr;
   b200_slim_s* h = nullptr;
   int rc = guarded([&] {
-    B200_REQUIRE(out && h_indptr && (nnz == 0 || h_indices), "b200_slim_create: NULL argument");
-    B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_slim_create: bad shape");
-    B200_REQUIRE(sgd_mode >= B200_SGD && sgd_mode <= B200_ADAM, "b200_slim_create: unknown sgd_mode %d", sgd_mode);
+    B200_REQUIRE(out && h_indptr && (nnz == 0 || h_indices), "%s: NULL argument", fn);
+    B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "%s: bad shape", fn);
+    B200_REQUIRE(sgd_mode >= B200_SGD && sgd_mode <= B200_ADAM, "%s: unknown sgd_mode %d", fn, sgd_mode);
+    B200_REQUIRE(!sharded || (0 <= col_lo && col_lo < col_hi && col_hi <= n_items), "%s: bad column range [%d,%d)", fn, col_lo, col_hi);
     B200_REQUIRE(sampler == 0 || has_sampleable_user(h_indptr, 0, n_users, n_items),
-                 "b200_slim_create: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
+                 "%s: no user has 0 < profile length < n_items, the device sampler cannot draw a sample", fn);
     h = new b200_slim_s();
     Params& p = h->p;
     p.n_users = (int)n_users; p.n_items = (int)n_items; p.symmetric = symmetric != 0; p.sgd_mode = sgd_mode;
     p.lr = learning_rate; p.li_reg = li_reg; p.lj_reg = lj_reg; p.gamma = gamma; p.beta1 = beta_1; p.beta2 = beta_2;
     p.b1_pow = beta_1; p.b2_pow = beta_2;  // pyx:157-158
-    h->sampler = sampler; h->hogwild = hogwild != 0;
-    h->seed = has_seed ? random_seed : 1u;
-    h->rng.seed(h->seed);
-    h->h_indptr.assign(h_indptr, h_indptr + n_users + 1);
-    h->h_indices.assign(h_indices, h_indices + nnz);
-    h->d_indptr.alloc((size_t)n_users + 1);
-    h->d_indices.alloc((size_t)std::max<int64_t>(nnz, 1));
-    B200_CUDA(cudaMemcpy(h->d_indptr.get(), h_indptr, sizeof(int) * ((size_t)n_users + 1), cudaMemcpyHostToDevice));
-    if (nnz) B200_CUDA(cudaMemcpy(h->d_indices.get(), h_indices, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice));
-    p.indptr = h->d_indptr.get(); p.indices = h->d_indices.get();
-    // S starts at zero (pyx:122-125): a dense S is allocated by the first call that needs it (ensure_dense_S), so a handle
-    // that becomes a tree handle (b200_slim_enable_tree) never holds one
-    if (sgd_mode == B200_ADAGRAD || sgd_mode == B200_RMSPROP) {
-      h->c.alloc((size_t)n_items); B200_CUDA(cudaMemset(h->c.get(), 0, sizeof(float) * (size_t)n_items)); p.c = h->c.get();
-    } else if (sgd_mode == B200_ADAM) {
-      h->m1.alloc((size_t)n_items); h->m2.alloc((size_t)n_items);
-      B200_CUDA(cudaMemset(h->m1.get(), 0, sizeof(float) * (size_t)n_items));
-      B200_CUDA(cudaMemset(h->m2.get(), 0, sizeof(float) * (size_t)n_items));
-      p.m1 = h->m1.get(); p.m2 = h->m2.get();
+    h->hogwild = hogwild != 0;
+    h->seed = seed;
+    h->shard_lo = col_lo; h->shard_hi = col_hi;
+    h->ss.init(n_users, n_items, nnz, h_indptr, h_indices, nullptr, true, 0.0, (size_t)n_users, sampler != 0, 0x243F6A88u, seed, false);
+    p.indptr = h->ss.indptr.get(); p.indices = h->ss.indices.get();
+    p.su = h->ss.su.get(); p.si = h->ss.si.get(); p.sj = h->ss.sj.get();
+    const AdaptState a = h->state.alloc(sgd_mode, (size_t)n_items);
+    if (sgd_mode == B200_ADAM) p.m1 = a.s1; else p.c = a.s1;
+    p.m2 = a.s2;
+    if (sharded) {
+      h->S.alloc_zeroed((size_t)n_items * (size_t)(col_hi - col_lo));  // pyx:122-125
+      p.S = h->S.get();
     }
-    h->su.alloc((size_t)n_users); h->si.alloc((size_t)n_users); h->sj.alloc((size_t)n_users);
-    p.su = h->su.get(); p.si = h->si.get(); p.sj = h->sj.get();
     h->pow_out.alloc(2);
     p.pow_out = h->pow_out.get();
     *out = h;
@@ -767,51 +747,20 @@ int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t
   return rc;
 }
 
+extern "C" {
+
+int b200_slim_create(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* h_indptr,
+                     const int32_t* h_indices, float learning_rate, float li_reg, float lj_reg, int symmetric, int sgd_mode,
+                     float gamma, float beta_1, float beta_2, int has_seed, uint32_t random_seed, int sampler, int hogwild) {
+  return create("b200_slim_create", out, n_users, n_items, nnz, h_indptr, h_indices, learning_rate, li_reg, lj_reg, symmetric,
+                sgd_mode, gamma, beta_1, beta_2, has_seed ? random_seed : 1u, sampler, hogwild, false, 0, 0);
+}
+
 int b200_slim_create_sharded(b200_slim_t* out, int64_t n_users, int64_t n_items, int64_t nnz, const int32_t* h_indptr,
                              const int32_t* h_indices, float learning_rate, float li_reg, float lj_reg, int sgd_mode, float gamma,
                              float beta_1, float beta_2, uint32_t random_seed, int col_lo, int col_hi) {
-  if (out) *out = nullptr;
-  b200_slim_s* h = nullptr;
-  int rc = guarded([&] {
-    B200_REQUIRE(out && h_indptr && (nnz == 0 || h_indices), "b200_slim_create_sharded: NULL argument");
-    B200_REQUIRE(n_users > 0 && n_items > 0 && nnz >= 0 && nnz < (1ll << 31) - 1, "b200_slim_create_sharded: bad shape");
-    B200_REQUIRE(sgd_mode >= B200_SGD && sgd_mode <= B200_ADAM, "b200_slim_create_sharded: unknown sgd_mode %d", sgd_mode);
-    B200_REQUIRE(0 <= col_lo && col_lo < col_hi && col_hi <= n_items, "b200_slim_create_sharded: bad column range [%d,%d)", col_lo, col_hi);
-    B200_REQUIRE(has_sampleable_user(h_indptr, 0, n_users, n_items),
-                 "b200_slim_create_sharded: no user has 0 < profile length < n_items, the device sampler cannot draw a sample");
-    h = new b200_slim_s();
-    Params& p = h->p;
-    p.n_users = (int)n_users; p.n_items = (int)n_items; p.symmetric = 0; p.sgd_mode = sgd_mode;
-    p.lr = learning_rate; p.li_reg = li_reg; p.lj_reg = lj_reg; p.gamma = gamma; p.beta1 = beta_1; p.beta2 = beta_2;
-    p.b1_pow = beta_1; p.b2_pow = beta_2;
-    h->sampler = 1; h->hogwild = 1;
-    h->seed = random_seed;
-    h->shard_lo = col_lo; h->shard_hi = col_hi;
-    h->d_indptr.alloc((size_t)n_users + 1);
-    h->d_indices.alloc((size_t)std::max<int64_t>(nnz, 1));
-    B200_CUDA(cudaMemcpy(h->d_indptr.get(), h_indptr, sizeof(int) * ((size_t)n_users + 1), cudaMemcpyHostToDevice));
-    if (nnz) B200_CUDA(cudaMemcpy(h->d_indices.get(), h_indices, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice));
-    p.indptr = h->d_indptr.get(); p.indices = h->d_indices.get();
-    const size_t cells = (size_t)n_items * (size_t)(col_hi - col_lo);
-    h->S.alloc(cells);
-    B200_CUDA(cudaMemset(h->S.get(), 0, cells * sizeof(float)));
-    p.S = h->S.get();
-    if (sgd_mode == B200_ADAGRAD || sgd_mode == B200_RMSPROP) {
-      h->c.alloc((size_t)n_items); B200_CUDA(cudaMemset(h->c.get(), 0, sizeof(float) * (size_t)n_items)); p.c = h->c.get();
-    } else if (sgd_mode == B200_ADAM) {
-      h->m1.alloc((size_t)n_items); h->m2.alloc((size_t)n_items);
-      B200_CUDA(cudaMemset(h->m1.get(), 0, sizeof(float) * (size_t)n_items));
-      B200_CUDA(cudaMemset(h->m2.get(), 0, sizeof(float) * (size_t)n_items));
-      p.m1 = h->m1.get(); p.m2 = h->m2.get();
-    }
-    h->su.alloc((size_t)n_users); h->si.alloc((size_t)n_users); h->sj.alloc((size_t)n_users);
-    p.su = h->su.get(); p.si = h->si.get(); p.sj = h->sj.get();
-    h->pow_out.alloc(2);
-    p.pow_out = h->pow_out.get();
-    *out = h;
-  });
-  if (rc != B200_OK && h) delete h;
-  return rc;
+  return create("b200_slim_create_sharded", out, n_users, n_items, nnz, h_indptr, h_indices, learning_rate, li_reg, lj_reg, 0, sgd_mode,
+                gamma, beta_1, beta_2, random_seed, 1, 1, true, col_lo, col_hi);
 }
 
 int b200_slim_shard_partial_device(b200_slim_t h, int64_t first, int n_batch, float* d_x, void* stream) {
@@ -821,9 +770,7 @@ int b200_slim_shard_partial_device(b200_slim_t h, int64_t first, int n_batch, fl
                  (long long)first, n_batch);
     cudaStream_t st = (cudaStream_t)stream;
     if (h->drawn_epoch != (long long)h->epoch) {  // the epoch's whole stream, identical on every rank
-      slim_sample_kernel<<<div_up(h->p.n_users, 256), 256, 0, st>>>(h->p.indptr, h->p.indices, h->p.n_users, h->p.n_items, h->p.n_users,
-                                                                  h->seed, h->epoch, h->su.get(), h->si.get(), h->sj.get());
-      count_launch();
+      h->ss.draw_philox(h->p.n_users, h->seed, h->epoch, 0, h->p.n_users, st);
       h->drawn_epoch = (long long)h->epoch;
     }
     ShardParams sp{h->p, h->shard_lo, h->shard_hi, h->shard_hi - h->shard_lo, (long long)first, n_batch};
@@ -878,18 +825,9 @@ int b200_slim_epoch(b200_slim_t h, void* stream) {
     const long long n = p.n_users;  // pyx:231: n_users samples per epoch
     p.n_samples = n;
     p.prof = getenv("B200REC_SLIM_PROF") != nullptr;
-    if (h->sampler == 0) {
-      h->hs.draw(h->rng, h->h_indptr.data(), h->h_indices.data(), nullptr, p.n_users, p.n_items, true, 0.0, n);
-      B200_CUDA(cudaMemcpyAsync(h->su.get(), h->hs.u.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->si.get(), h->hs.i.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->sj.get(), h->hs.j.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
-    }
+    h->ss.draw_glibc(n, st);
     h->timer.begin(st);
-    if (h->sampler != 0) {
-      slim_sample_kernel<<<div_up(n, 256), 256, 0, st>>>(p.indptr, p.indices, p.n_users, p.n_items, n, h->seed, h->epoch,
-                                                        h->su.get(), h->si.get(), h->sj.get());
-      count_launch();
-    }
+    h->ss.draw_philox(n, h->seed, h->epoch, 0, p.n_users, st);
     if (!h->tree) ensure_dense_S(h, st);
     if (h->hogwild) {
       slim_hogwild_kernel<<<sm_count() * 8, 256, 0, st>>>(p);
@@ -904,7 +842,7 @@ int b200_slim_epoch(b200_slim_t h, void* stream) {
     h->timer.end(st);
     if (!h->hogwild && p.sgd_mode == B200_ADAM) {
       read_powers(h->pow_out.get(), p.b1_pow, p.b2_pow, st);
-    } else if (h->sampler == 0) {
+    } else if (h->ss.host_vectors_in_flight()) {
       B200_CUDA(cudaStreamSynchronize(st));
     }
     h->epoch += 1;
@@ -996,11 +934,7 @@ int b200_slim_tree_cells(b200_slim_t h, int64_t* cells) {
 int b200_slim_get_samples(b200_slim_t h, int32_t* u, int32_t* i, int32_t* j) {
   return guarded([&] {
     B200_REQUIRE(h && u && i && j, "b200_slim_get_samples: NULL argument");
-    B200_CUDA(cudaDeviceSynchronize());
-    const size_t n = (size_t)h->p.n_users;
-    B200_CUDA(cudaMemcpy(u, h->su.get(), sizeof(int) * n, cudaMemcpyDeviceToHost));
-    B200_CUDA(cudaMemcpy(i, h->si.get(), sizeof(int) * n, cudaMemcpyDeviceToHost));
-    B200_CUDA(cudaMemcpy(j, h->sj.get(), sizeof(int) * n, cudaMemcpyDeviceToHost));
+    h->ss.copy_out(u, i, j, nullptr);
   });
 }
 

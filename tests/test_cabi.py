@@ -83,3 +83,52 @@ def test_argument_errors_mirror_the_reference():
     Xbad = X.copy(); Xbad.data[0] = np.inf
     with pytest.raises(AssertionError):
         Compute_Similarity(Xbad)  # Compute_Similarity.py:44
+
+
+def _sgd_create_calls():
+    """Each SGD trainer's create entry point as f(out, n_users=.., sgd_mode=.., indptr=.., col_lo=.., col_hi=..) on a valid
+    4 x 3 URM, so that one argument at a time can be made bad."""
+    from recsys2019_deeplearning_evaluation_b200 import _lib
+    L = _lib.load()
+    indptr = np.array([0, 1, 2, 3, 3], np.int32)
+    indices = np.array([0, 1, 2], np.int32)
+    data = np.ones(3, np.float32)
+    U = np.zeros((4, 2), np.float64)
+    V = np.zeros((3, 2), np.float64)
+    keep = (indptr, indices, data, U, V)
+
+    def mf(out, n_users=4, sgd_mode=0, indptr=_lib.ptr(indptr), **_):
+        return L.b200_mf_create(out, n_users, 3, 3, indptr, _lib.ptr(indices), _lib.ptr(data), 2, 0, 1, 0.5, 0.1, 0, 0.0, 0.0,
+                                0.0, 0.0, 0.0, sgd_mode, 0.9, 0.9, 0.999, _lib.ptr(U), _lib.ptr(V), 1, 7, 1, 0)
+
+    def slim(out, n_users=4, sgd_mode=0, indptr=_lib.ptr(indptr), **_):
+        return L.b200_slim_create(out, n_users, 3, 3, indptr, _lib.ptr(indices), 0.1, 0.0, 0.0, 0, sgd_mode, 0.9, 0.9, 0.999,
+                                  1, 7, 1, 0)
+
+    def slim_sharded(out, n_users=4, sgd_mode=0, indptr=_lib.ptr(indptr), col_lo=0, col_hi=3):
+        return L.b200_slim_create_sharded(out, n_users, 3, 3, indptr, _lib.ptr(indices), 0.1, 0.0, 0.0, sgd_mode, 0.9, 0.9,
+                                          0.999, 7, col_lo, col_hi)
+
+    def asysvd(out, n_users=4, sgd_mode=0, indptr=_lib.ptr(indptr), **_):
+        return L.b200_asysvd_create(out, n_users, 3, 3, indptr, _lib.ptr(indices), _lib.ptr(data), 2, 0.5, 0.1, 0, 0.0, 0.0,
+                                    0.0, sgd_mode, 0.9, 0.9, 0.999, _lib.ptr(V), _lib.ptr(V), 1, 7)
+
+    calls = {"b200_mf_create": mf, "b200_slim_create": slim, "b200_slim_create_sharded": slim_sharded,
+             "b200_asysvd_create": asysvd}
+    return L, calls, keep
+
+
+@pytest.mark.parametrize("bad", [dict(n_users=0), dict(sgd_mode=99), dict(indptr=None), dict(col_lo=2, col_hi=2)],
+                         ids=["shape", "sgd_mode", "null_array", "column_range"])
+def test_sgd_create_rejects_bad_arguments_before_any_cuda_call(bad):
+    """Every SGD trainer's create entry point checks its arguments before it touches the device: B200_E_INVALID, *out left
+    NULL, and an error text that names the entry point."""
+    L, calls, keep = _sgd_create_calls()
+    for fn, call in calls.items():
+        if "col_lo" in bad and fn != "b200_slim_create_sharded":
+            continue
+        h = ctypes.c_void_p(1)
+        rc = call(ctypes.byref(h), **bad)
+        assert rc == -1, (fn, bad)
+        assert h.value is None, (fn, bad)
+        assert L.b200_last_error().decode().startswith(fn + ":"), (fn, bad, L.b200_last_error())
